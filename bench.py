@@ -40,6 +40,7 @@ RING = 8            # distinct PD-target / torque sets cycled through (synthetic
 SETTLE = 40         # untimed control steps run while BUILDING the workload: robots are dropped from 0.75 m and must stand
                     # on the terrain before warm-up starts, whatever --warmup the caller passes
 L2_FLUSH_BYTES = 256 << 20
+DUMP_BYTES = 64 << 20      # --dump-outputs: cap on everything written
 SOLVER = dict(threshold=1e-6)   # everything else at the library defaults (rsb_params_default): accel_m=2, accel_start=6, stall_window=8, stall_reg=0.02
 
 
@@ -109,7 +110,7 @@ class Workload:
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md): NVML in a
+    """SM clock and throttle reasons sampled DURING the timed region: NVML in a
     background thread every 5 ms (nvidia-smi -lms needs > 100 ms to produce its first row, longer
     than a short timed region)."""
     BAD = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
@@ -124,6 +125,7 @@ class ClockSampler:
             idx = int(uuid_order.split(",")[index]) if uuid_order and uuid_order.split(",")[index].isdigit() else index
             self.h = pynvml.nvmlDeviceGetHandleByIndex(idx)
             self.max_mhz = float(pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM))
+            self.power_limit_w = pynvml.nvmlDeviceGetPowerManagementLimit(self.h) / 1000.0     # part of every number measured here
         except Exception:
             self.nv = None
 
@@ -149,7 +151,8 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["NVML unavailable"]}
         self.stop_flag = True
         self.t.join(timeout=1)
-        return {"sm_mhz": float(np.median(self.sm)) if self.sm else None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": len(self.sm)}
+        return {"sm_mhz": float(np.median(self.sm)) if self.sm else None, "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w,
+                "reasons": sorted(self.reasons), "samples": len(self.sm)}
 
 
 def usable_cores():
@@ -338,9 +341,26 @@ class GpuSim:
                 "non_converged_fraction": float((res >= SOLVER["threshold"]).mean()), "standing_fraction": float((g[:, 2] > zmin).mean())}
 
 
+def dump_outputs(out_dir, sim, obs):
+    """what the caller of the last timed step holds: the observation rows it returned (every rank's rows at N > 1) and this
+    rank's state and contact counts after it, float32 as computed (contact counts converted).  Above DUMP_BYTES in all, every
+    array keeps the same fraction of its rows, a fixed seeded sample whose row indices go to <name>_rows.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    gc, gv = sim.bt.get_state()
+    _, cnt = sim.bt.contacts()
+    arrays = {"obs": np.asarray(obs, np.float32), "gc": gc, "gv": gv, "ncontacts": cnt}
+    frac = min(1.0, DUMP_BYTES / sum(3 * a.nbytes for a in arrays.values()))   # x3: float32 rows plus float64 row indices
+    for name, a in arrays.items():
+        if frac < 1.0:
+            rows = np.sort(np.random.default_rng(0).choice(len(a), max(1, int(len(a) * frac)), replace=False))
+            np.save(os.path.join(out_dir, name + "_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def side_result(key, local, stream, flush, steps, warmup):
     """N = 1 side measurement of another BASELINE config: same timing rules as the headline (CUDA events per launch on the
-    launching stream, L2 flushed between timed iterations), fewer steps; with its own bounded CPU baseline"""
+    launching stream, L2 flushed between timed iterations); with its own bounded CPU baseline"""
     import torch
     wl = Workload(key, 0, ENVS_PER_GPU)
     sim = GpuSim(wl, local, stream)
@@ -386,8 +406,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-side-results", action="store_true")
     ap.add_argument("--nccl-gather", action="store_true", help="N > 1: NCCL all-gather after the step instead of the fused peer-memory gather, for comparison")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step returned to its caller "
+                    "(rank 0: observation rows, state, contact counts) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs dumps the GPU path's outputs; it does not apply to --impl reference")
         return run_reference(args)
 
     import torch
@@ -437,7 +461,7 @@ def main():
         kev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)] if inner else ev
         barrier()
         for k in range(steps):
-            flush.fill_(float(k))                            # evict L2 between timed iterations (256 MiB > 126 MB L2)
+            flush.fill_(float(k))                            # evict L2 between timed iterations (256 MiB > 50 MB L2 of an H100)
             ev[k][0].record(stream)
             if host_io:
                 sim.step_host(step0 + k, shared.local if world > 1 else None)
@@ -477,6 +501,8 @@ def main():
     launches = bt.launch_count() - l0
     ms_e2e, _ = timed(True, args.steps, W + args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, sim, shared.all if world > 1 else sim.obs_host.numpy())
     st = sim.stats()
     keys = ["mean_contacts_per_env", "mean_solver_sweeps", "non_converged_fraction", "standing_fraction"]
     stats = torch.tensor([st[k] for k in keys] + [float(st["max_solver_sweeps"])], dtype=torch.float64, device="cuda")
@@ -494,15 +520,10 @@ def main():
         B = algorithmic_bytes_per_env_step(19, 18, 12, kbar)
         launch_ms = ms_kernel / args.steps
         achieved = B * n * SUBSTEPS / (launch_ms * 1e-3) / 1e9
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
         try:
             mp = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
             peak, peak_src = float(mp["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))["dram_bytes_per_launch"]
         except Exception:
             pass
         line = {
@@ -523,10 +544,11 @@ def main():
                     "path": "pinned host targets and observation rows read / written in place by the step kernel (zero-copy over PCIe)"
                             + ("; rows of all ranks land in one shared page-locked array, shared-memory flags as barrier" if world > 1 else "")},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "kernel": "rsb_step_kernel (fused FK+CRBA+RNEA+narrow-phase+contact solver+integrate)",
                          "algorithmic_bytes_per_env_step": B, "launch_ms": launch_ms, "peak_source": peak_src,
                          "note": "path is FP32-latency/issue bound, not HBM bound (SURVEY.md 7 hard part 2); see DESIGN.md roofline"},
+            "device": torch.cuda.get_device_name(local),
             "clocks": clocks,
         }
         if gather is not None:
@@ -536,9 +558,8 @@ def main():
     del sim
     if rank == 0:
         if world == 1 and not args.no_side_results:
-            side_steps = max(10, min(40, args.steps))
-            line["side_results"] = {"config2_flat_random_torques_fallen": side_result("c2", local, stream, flush, side_steps, 5),
-                                    "config4_atlas_standing": side_result("c4", local, stream, flush, side_steps, 5)}
+            line["side_results"] = {"config2_flat_random_torques_fallen": side_result("c2", local, stream, flush, args.steps, 5),
+                                    "config4_atlas_standing": side_result("c4", local, stream, flush, args.steps, 5)}
         if not args.no_cpu_baseline and world == 1:
             line["cpu_baseline"] = cpu_baseline("c3", n, 100, 12.0, both_precisions=True)
         print(json.dumps(line), flush=True)

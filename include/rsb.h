@@ -1,4 +1,4 @@
-/* rsb.h -- C-ABI of the B200-native batched rigid-body step ("raisim batch").
+/* rsb.h -- C-ABI of the H100-native batched rigid-body step ("raisim batch").
  *
  * This is the drop-in boundary for the hot path raisim::World::integrate() =
  * integrate1() + integrate2() and the ArticulatedSystem state/force/PD accessors around it

@@ -1,4 +1,4 @@
-"""raisimlib_b200 -- B200-native batched rigid-body step behind the RaiSim World::integrate() surface.
+"""raisimlib_b200 -- H100-native batched rigid-body step behind the RaiSim World::integrate() surface.
 
 The product is the CUDA library (csrc/ -> librsb.so, C-ABI in include/rsb.h) and the header-only
 C++ facade in include/raisim/.  This Python package only binds the C-ABI for tests and bench.py.

@@ -1,5 +1,5 @@
 // C-ABI implementation (include/rsb.h): batch memory, model-constant blob, kernel launches.
-// No CPU fallback: every compute entry point launches the sm_100a kernel or fails loudly.
+// No CPU fallback: every compute entry point launches the sm_90a kernel or fails loudly.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -225,8 +225,10 @@ extern "C" int rsb_batch_ob_dim(const rsb_batch* b);
 static int pick_config(rsb_batch* b) {
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, b->device));
-  if (prop.major < 10) return fail(RSB_ERR_UNSUPPORTED, "raisimlib_b200 needs an sm_100a (B200) device; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
-  const size_t budget = prop.sharedMemPerBlockOptin;   // 227 KB on B200
+  // sm_90a code runs on compute capability 9.0 only (arch-specific features are not forward compatible)
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(RSB_ERR_UNSUPPORTED, "raisimlib_b200 is compiled for sm_90a and needs an H100-class device (compute capability 9.0); found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+  const size_t budget = prop.sharedMemPerBlockOptin;   // 227 KB on H100
   const size_t blob_bytes = (size_t)b->blob_host.size() * 4;
   const size_t per_warp = (size_t)b->ws.words * 4;
   const int sms = prop.multiProcessorCount;
@@ -245,10 +247,12 @@ static int pick_config(rsb_batch* b) {
   b->spec = quad_topology ? 1 : (same_dims(b->dims, kHumanoid30) ? 2 : 0);
   if (const char* e = getenv("RSB_FORCE_GENERIC")) if (atoi(e)) b->spec = 0;
   // Warps per CTA (= resident environments per CTA).  A round of w resident warps per SM costs ~ max(13, w): latency-bound up to a
-  // dozen warps (32 k cycles per sub-step), issue-bound beyond (2.5 k cycles per warp; profiles/).  Choose the option with the
-  // smallest rounds x cost, ties to the larger CTA (one sub-step barrier group, one copy of
-  // the model block).  4096 ANYmal-like environments: 28 (one round).  4096 Atlas-like ones, whose 10.9 KB workspaces allow 16 per
-  // SM: 14 (two balanced rounds: 0.98 ms per launch) rather than 16 (a full round and a 73 % one: 1.29 ms).
+  // dozen warps, issue-bound beyond.  Choose the option with the smallest rounds x cost, ties to the larger CTA (one sub-step
+  // barrier group, one copy of the model block).  On the 132 SMs of an H100, 4096 ANYmal-like environments (7.5 KB workspaces, at
+  // most 29 per SM) take two rounds whatever the CTA: 16 (two full rounds, 0.263 ms per control step of 4 sub-steps) rather than
+  // 28 (a full round and an 11 % one, 0.320 ms) or 14 (0.310 ms).  4096 Atlas-like ones (10.9 KB workspaces): 16 as well
+  // (1.41 ms, against 1.68 ms with 14).  One warp per environment: the choice does not change the results (bench.py outputs are
+  // bit-identical for 8, 14, 16 and 28).
   static const int options[] = {28, 16, 14, 8, 4, 1};
   int best = 0; long best_cost = 0;
   for (int w : options) {

@@ -1,4 +1,4 @@
-// Fused World::integrate() for a batch of environments -- hand-written sm_100a CUDA.
+// Fused World::integrate() for a batch of environments -- hand-written sm_90a CUDA.
 //
 // One warp == one environment (BASELINE.json north_star).  A CTA of WPC warps shares the model
 // constant block, staged global -> shared ONCE per CTA by a TMA bulk copy (cp.async.bulk +

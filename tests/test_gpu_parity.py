@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Everything goes through the C-ABI
+"""GPU parity tests (run on an H100: pytest -m gpu).  Everything goes through the C-ABI
 (raisimlib_b200/librsb.so) and is compared with the CPU oracle on the same seeded inputs.
 
 Tolerances (float32 kernel vs float64 oracle) are written next to each assertion.  Integer results
@@ -710,7 +710,7 @@ def test_control_step_equals_separate_calls(capi):
 @pytest.mark.parametrize("n", [1, 5, 4097, 9000])
 def test_ragged_batch_sizes(capi, n):
     """batch sizes that do not fill a CTA / an SM wave, and more environments than resident warps
-    (9000 > 148 x 28: the per-warp environment loop runs three times)."""
+    (9000 > 132 x 29, more than an H100 holds at once: the per-warp environment loop runs several times)."""
     t, bt, o64, o32, gc, gv, tau = _setup(capi, "anymal_c_like.urdf", n, seed=131 + n, base_z=0.5, joint_scale=0.3, params=dict(stall_window=0))
     bt.integrate(3)
     g, v = bt.get_state()
@@ -1101,7 +1101,7 @@ def test_fused_peer_observation_gather_two_gpus(capi):
     NVLink peer memory (CUDA IPC), counters + a wait kernel close the exchange; rows must equal each rank's own rows, in rank order."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

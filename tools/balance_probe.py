@@ -104,7 +104,7 @@ def main():
 
     restore()
     tot, tD, cnt1, it1 = stage_report(bt, tg, obs, k0, "as is, barrier 1")
-    wpc = 28
+    wpc = 16          # pick_config's choice for 4096 quadrupeds on the 132 SMs of an H100
     ncta = (n + wpc - 1) // wpc
     pad = np.full((ncta * wpc, 4), np.nan); pad[:n] = tot
     cta = pad.reshape(ncta, wpc, 4)
@@ -120,12 +120,13 @@ def main():
     idx = int(np.argsort(cost, kind="stable")[n // 2])
     restore(np.tile(gc[idx], (n, 1)), np.tile(gv[idx], (n, 1)))
     stage_report(bt, tg, obs, k0, "all envs = median env, barrier 1", perm=torch.full((n,), idx, dtype=torch.long, device="cuda"))
-    b2, t2, o2, s2 = setup(148)
-    b2.set_state(gc[:148], gv[:148])
-    stage_report(b2, t2, o2, k0, "148 envs (one warp per SM)")
-    b2, t2, o2, s2 = setup(148 * 4)
-    b2.set_state(gc[:148 * 4], gv[:148 * 4])
-    stage_report(b2, t2, o2, k0, "592 envs")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    b2, t2, o2, s2 = setup(sms)
+    b2.set_state(gc[:sms], gv[:sms])
+    stage_report(b2, t2, o2, k0, "%d envs (one warp per SM)" % sms)
+    b2, t2, o2, s2 = setup(sms * 4)
+    b2.set_state(gc[:sms * 4], gv[:sms * 4])
+    stage_report(b2, t2, o2, k0, "%d envs" % (sms * 4))
 
     order = np.argsort(cost, kind="stable")
     for name, idx in (("median-cost env", order[n // 2]), ("p90-cost env", order[int(n * 0.9)]), ("worst env", order[-1]), ("cheapest env", order[0])):
@@ -148,7 +149,7 @@ def main():
     os.environ["RSB_SUBSTEP_BARRIER"] = "1"
 
     # fewer environments than warp slots: how does the launch time fall with the resident count?
-    for m in (2048, 1024, 512, 148):
+    for m in (2048, 1024, 512, sms):
         b2, t2, o2, s2 = setup(m)
         b2.set_state(gc[:m], gv[:m])
         r = time_launches(b2, t2, o2, s2, k0=k0)
