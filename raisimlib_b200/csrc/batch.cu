@@ -249,10 +249,12 @@ static int pick_config(rsb_batch* b) {
   // Warps per CTA (= resident environments per CTA).  A round of w resident warps per SM costs ~ max(13, w): latency-bound up to a
   // dozen warps, issue-bound beyond.  Choose the option with the smallest rounds x cost, ties to the larger CTA (one sub-step
   // barrier group, one copy of the model block).  On the 132 SMs of an H100, 4096 ANYmal-like environments (7.5 KB workspaces, at
-  // most 29 per SM) take two rounds whatever the CTA: 16 (two full rounds, 0.263 ms per control step of 4 sub-steps) rather than
-  // 28 (a full round and an 11 % one, 0.320 ms) or 14 (0.310 ms).  4096 Atlas-like ones (10.9 KB workspaces): 16 as well
-  // (1.41 ms, against 1.68 ms with 14).  One warp per environment: the choice does not change the results (bench.py outputs are
-  // bit-identical for 8, 14, 16 and 28).
+  // most 29 per SM) take two rounds whatever the CTA: 16 (a round of 2112 and one of 1984, each re-aligned at every sub-step:
+  // 0.197 ms per control step of 4 sub-steps at 400 W) rather than 28 (a full round and an 11 % one, 0.282 ms), 14 (two CTAs per SM,
+  // 0.248 ms) or 8 (four rounds, 0.312 ms); the model ranks 8 above 14 and 28 (52 against 56) and is only checked to pick the
+  // fastest, 16.  4096 Atlas-like ones (10.9 KB workspaces): 16 as well (1.41 ms, against 1.68 ms with 14, measured without the
+  // sub-step barrier).  One warp per environment: the choice does not change the results (bench.py outputs are bit-identical for
+  // 8, 14, 16 and 28).
   static const int options[] = {28, 16, 14, 8, 4, 1};
   int best = 0; long best_cost = 0;
   for (int w : options) {
@@ -311,10 +313,9 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
     b->peer_epoch++;
     a.peer_expected = b->peer_epoch * (unsigned)b->grid; a.peer_done = b->peer_done;
   }
-  {
+  if (phase_mask == 0) {   // every round of warps re-aligns at each sub-step (the kernel counts the warps of the round)
     const char* e = getenv("RSB_SUBSTEP_BARRIER");
-    const int level = e ? atoi(e) : 1;
-    a.substep_barrier = ((size_t)b->grid * b->wpc >= (size_t)b->N && phase_mask == 0) ? level : 0;
+    a.substep_barrier = e ? atoi(e) : 1;
   }
   cudaError_t e;
   switch (b->wpc) {
@@ -1088,6 +1089,13 @@ int rsb_internal_batch_info(rsb_batch* b, int* device, void** stream, int* num_e
 }
 // profiling hook (tools/balance_probe.py): device buffer [num_envs][4][8] of SM-clock stamps, or null to switch off
 int rsb_internal_set_profile(rsb_batch* b, unsigned* dev) { if (!b) return -1; b->prof = dev; return 0; }
+// launch shape of the step kernel (tools/stage_probe.py, tests): warps per CTA and CTAs; environment e runs in round
+// e / (wpc * grid) on CTA (e % (wpc * grid)) / wpc
+int rsb_internal_launch_config(const rsb_batch* b, int* wpc, int* grid) {
+  if (!b || !wpc || !grid) return fail(RSB_ERR_INVALID, "null argument");
+  *wpc = b->wpc; *grid = b->grid;
+  return RSB_OK;
+}
 void rsb_internal_set_error(const char* msg) { g_err = msg ? msg : ""; }
 
 }  // extern "C"

@@ -216,7 +216,7 @@ struct StepArgs {
   unsigned char* gym_done;         // [num_envs]
   int phase_mask;      // bit0: stop after stage B (integrate1: no state update); bit2: kinematics only (stage A + getters' buffers,
                        // the contact records of the last integrate() stay as they are)
-  int substep_barrier; // 1: re-align the CTA's warps at every sub-step (instruction-cache locality experiment)
+  int substep_barrier; // 1: re-align the CTA's warps of one round at every sub-step (2, 3: also before stages C, E)
 };
 
 // ------------------------------------------------------------------ small device math ----------
@@ -644,14 +644,45 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 #define MYB(f) (bodyi[(f) * nbp + bb])
   // (row, col) of the base 6x6 lower triangle owned by lanes 0..20, packed row | col << 3: one table per CTA
   __shared__ uint8_t s_tri[32];
+  __shared__ int s_work[2];   // this CTA's environments in the last launch: sum over rounds of (warps x the round's largest solver work), total work
   if (threadIdx.x < 32) {
     int pr = 0;
     for (int r = 0, e = 0; r < 6; r++) for (int c = 0; c <= r; c++, e++) if (e == (int)threadIdx.x) pr = r | (c << 3);
     s_tri[threadIdx.x] = (uint8_t)pr;
+    if (threadIdx.x < 2) s_work[threadIdx.x] = 0;
   }
   __syncthreads();
 
   const int warps_total = gridDim.x * WPC;
+  // The sub-step barrier makes every warp of a round wait for the round's slowest solve at each sub-step.  It pays (instruction-cache
+  // locality; the slowest warp finishes alone at single-warp speed) while the largest solver work of a round is at most twice the
+  // mean: on an H100, 4096 quadrupeds standing on rough ground (ratio 1.6) and humanoids standing on box feet (1.3) run 28 % and
+  // 12 % faster with it, fallen quadrupeds under random torques (ratio 3.1) 20 % slower.  Each CTA decides for itself from the work
+  // (sweeps x contacts of the last sub-step) that the environments of its rounds and of the same rounds of the next NEIGH - 1 CTAs
+  // did in the last launch: one CTA's two rounds alone scatter too widely (on the H100, per-CTA ratios of the first workload reach
+  // 2.0, those of the third go down to 1.8).  Every thread reads the same integer sums, so all warps of the CTA agree (kept in shared
+  // memory: a register live across the loop costs spills at 72 registers); another CTA may already have stored new work for some of
+  // those environments, which changes the decision of this CTA, never a result.
+  if (args.substep_barrier) {
+    constexpr int NEIGH = 8;
+    const int neigh = min(NEIGH, (int)gridDim.x);
+#pragma unroll 1
+    for (int q = warp; (q / neigh) * warps_total < args.num_envs; q += WPC) {   // round q / neigh of CTA blockIdx + q % neigh: lane = warp
+      const int first = (q / neigh) * warps_total + (((int)blockIdx.x + q % neigh) % (int)gridDim.x) * WPC, e = first + lane;
+      const int w = (lane < WPC && e < args.num_envs) ? args.iters[e] * args.ncontacts[e] : 0;
+      const int wmax = __reduce_max_sync(FULL, w), wsum = __reduce_add_sync(FULL, w);
+      if (lane == 0 && first < args.num_envs) { atomicAdd(&s_work[0], min(WPC, args.num_envs - first) * wmax); atomicAdd(&s_work[1], wsum); }
+    }
+    __syncthreads();
+  }
+  // Sub-step barrier: the warps of this CTA that own an environment in this round (env - warp = the CTA's first one).  Counts of
+  // two rounds never meet on barrier 1: a warp arrives at it only at the sub-steps of its current round, and the last barrier of
+  // round r (its last sub-step) completes only once every warp of round r has arrived, so no round-r warp is still to arrive when
+  // the first warp of round r + 1 does.  A warp without an environment in round r + 1 (environments are dense, so those are the
+  // highest warps of the CTA) leaves the loop and never arrives again.
+#define SUBSTEP_BARRIER(level) \
+  if (args.substep_barrier >= (level) && s_work[0] <= 2 * s_work[1])             \
+    asm volatile("bar.sync 1, %0;" ::"r"(min(WPC, args.num_envs - (env - warp)) * 32))
 #pragma unroll 1
   for (int env = blockIdx.x * WPC + warp; env < args.num_envs; env += warps_total) {
     // ---- load this environment's rows (coalesced: one row per warp) -----------------------------
@@ -688,11 +719,9 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 
 #pragma unroll 1
     for (int sub = 0; sub < args.substeps; sub++) {
-      // Re-align the CTA's warps (instruction-cache locality: 28 warps drifting through a 75 KB kernel miss the
-      // instruction cache far more often than 28 warps in the same stage).  Only set by the host when every warp
-      // owns exactly one environment, so all of them reach the barrier the same number of times.
-      const int bar_threads = min(WPC, args.num_envs - (int)blockIdx.x * WPC) * 32;
-      if (args.substep_barrier >= 1) asm volatile("bar.sync 1, %0;" ::"r"(bar_threads));
+      // Re-align the round's warps (instruction-cache locality: warps drifting through a 75 KB kernel miss the instruction
+      // cache far more often than warps in the same stage, and the slowest warp of a sub-step finishes its solve alone).
+      SUBSTEP_BARRIER(1);
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 0] = (unsigned)clock64();
       // =========================== stage A: FK + RNEA + CRBA =====================================
       float R[9]; f3 p, w, v, wd, vd, ax;
@@ -889,7 +918,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 2] = (unsigned)clock64();
       if (args.phase_mask & 1) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // integrate1(): kinematics, collision, M, h only
 
-      if (args.substep_barrier >= 2) asm volatile("bar.sync 1, %0;" ::"r"(bar_threads));
+      SUBSTEP_BARRIER(2);
       // =========================== stage C: b, Mhat = L^T L, z, Y, G ==============================
       // a9 joint limits: the first LMAX joints found beyond their URDF limit become unilateral rows sign * qdot >= target
       int Lm = 0;
@@ -1280,7 +1309,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       }
       __syncwarp();
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 4] = (unsigned)clock64();
-      if (args.substep_barrier >= 3) asm volatile("bar.sync 1, %0;" ::"r"(bar_threads));
+      SUBSTEP_BARRIER(3);
       // =========================== stage E: v+ = v + L^-1 (dt z + Y lam), integration ============
       if constexpr (QUAD) {
         // w_i = dt z_i + sum over the rows whose chain holds dof i of Y[depth i][row] lam_row, lane = dof
@@ -1505,6 +1534,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
     }
     __syncwarp();
   }
+#undef SUBSTEP_BARRIER
   if (args.peer_world > 0 && args.obs) {
     // every row this CTA stored must be visible on the peers before they see the arrival count: the CTA barrier orders the warps'
     // stores before the signalling threads, whose release at system scope is cumulative over them (one fence per signalling

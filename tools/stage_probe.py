@@ -2,7 +2,8 @@
 """In-kernel stage timers for any bench workload (run under gpurun; exploratory, never a bench value).
 
 usage: stage_probe.py c3|c2|c4 [n_envs] -- prints cycles per sub-step of one environment in stages A..E (SM-clock stamps written by the
-step kernel through rsb_internal_set_profile), launch times with the sub-step barrier on / off, and the sweep / contact histograms."""
+step kernel through rsb_internal_set_profile), launch times with the sub-step barrier on / off, the sweep / contact histograms, and
+what the slowest warp of each CTA-round costs behind the sub-step barrier."""
 import ctypes, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -53,6 +54,10 @@ def main():
         os.environ["RSB_SUBSTEP_BARRIER"] = os.environ["RSB_PROBE_STAGE_LEVEL"]
     lib = capi.lib()
     lib.rsb_internal_set_profile.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+    lib.rsb_internal_launch_config.argtypes = [ctypes.c_void_p] * 3
+    wpc, grid = ctypes.c_int(), ctypes.c_int()
+    lib.rsb_internal_launch_config(sim.bt.h, ctypes.byref(wpc), ctypes.byref(grid))
+    wpc, grid = wpc.value, grid.value
     sim.bt.set_state(g, v)
     prof = torch.zeros((n, 4, 8), dtype=torch.int32, device="cuda")
     lib.rsb_internal_set_profile(sim.bt.h, ctypes.c_void_p(prof.data_ptr()))
@@ -72,6 +77,15 @@ def main():
     it = sim.bt.solver_iterations(); _, cnt = sim.bt.contacts()
     upd = np.maximum(1, it * cnt)
     print("  D cycles per contact update (last sub-step): median %.0f" % np.median(tD[:, 3] / upd))
+    # behind the sub-step barrier a CTA-round (the warps of one CTA in one round) lasts, per sub-step, as long as its slowest warp:
+    # sum over the sub-steps of the group maximum against the mean busy time (the stamps exclude the barrier wait)
+    T = wpc * grid
+    e = np.arange(n)
+    group = (e // T) * grid + (e % T) // wpc
+    gmax = np.zeros((group.max() + 1, tot.shape[1]))
+    np.maximum.at(gmax, group, tot)
+    print("  CTA-rounds (%d warps x %d CTAs, %d environments per round): mean of the per-sub-step group max %.0f cycles per launch, "
+          "mean busy %.0f (%.2fx)" % (wpc, grid, T, gmax.sum(1).mean(), tot.sum(1).mean(), gmax.sum(1).mean() / tot.sum(1).mean()))
 
 
 if __name__ == "__main__":
