@@ -253,8 +253,8 @@ static int pick_config(rsb_batch* b) {
   // 0.197 ms per control step of 4 sub-steps at 400 W) rather than 28 (a full round and an 11 % one, 0.282 ms), 14 (two CTAs per SM,
   // 0.248 ms) or 8 (four rounds, 0.312 ms); the model ranks 8 above 14 and 28 (52 against 56) and is only checked to pick the
   // fastest, 16.  4096 Atlas-like ones (10.9 KB workspaces): 16 as well (1.41 ms, against 1.68 ms with 14, measured without the
-  // sub-step barrier).  One warp per environment: the choice does not change the results (bench.py outputs are bit-identical for
-  // 8, 14, 16 and 28).
+  // sub-step barrier).  One warp per environment: the choice does not change the results (every option that fits, for every compiled instance:
+  // tests/test_gpu_instances.py::test_warps_per_cta_bit_identical).
   static const int options[] = {28, 16, 14, 8, 4, 1};
   int best = 0; long best_cost = 0;
   for (int w : options) {
@@ -1090,10 +1090,18 @@ int rsb_internal_batch_info(rsb_batch* b, int* device, void** stream, int* num_e
 // profiling hook (tools/balance_probe.py): device buffer [num_envs][4][8] of SM-clock stamps, or null to switch off
 int rsb_internal_set_profile(rsb_batch* b, unsigned* dev) { if (!b) return -1; b->prof = dev; return 0; }
 // launch shape of the step kernel (tools/stage_probe.py, tests): warps per CTA and CTAs; environment e runs in round
-// e / (wpc * grid) on CTA (e % (wpc * grid)) / wpc
+// e / (wpc * grid) on CTA (e % (wpc * grid)) / wpc.  RSB_FORCE_WPC is dropped without a message when the CTA does not fit in shared
+// memory, so a caller that forces a configuration reads back what it got here.
 int rsb_internal_launch_config(const rsb_batch* b, int* wpc, int* grid) {
   if (!b || !wpc || !grid) return fail(RSB_ERR_INVALID, "null argument");
   *wpc = b->wpc; *grid = b->grid;
+  return RSB_OK;
+}
+// compiled instance of the step kernel that the batch launches (dispatch_spec): spec 0 generic, 1 quadruped, 2 humanoid; slots =
+// candidate points per lane (tests).  A hook of its own, so that callers of rsb_internal_launch_config keep their signature
+int rsb_internal_launch_instance(const rsb_batch* b, int* spec, int* slots) {
+  if (!b || !spec || !slots) return fail(RSB_ERR_INVALID, "null argument");
+  *spec = b->spec; *slots = b->slots;
   return RSB_OK;
 }
 void rsb_internal_set_error(const char* msg) { g_err = msg ? msg : ""; }

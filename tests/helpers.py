@@ -1,5 +1,12 @@
-"""Shared test helpers: independent numpy restatements used to pin the oracle (SURVEY.md 4(3))."""
+"""Shared test helpers: independent numpy restatements used to pin the oracle (SURVEY.md 4(3)), the test models, and the
+batch / oracle set-up the GPU parity tests share."""
+import os
+import xml.etree.ElementTree as ET
+
 import numpy as np
+
+MARGIN = 2e-6          # metres; contact candidates shallower than this are excluded from index parity
+THRESH = 1e-6          # solver threshold used on both sides
 
 ANYMAL_GC0 = np.array([0, 0, 0.60, 1, 0, 0, 0, 0.03, 0.4, -0.8, -0.03, 0.4, -0.8, 0.03, -0.4, 0.8, -0.03, -0.4, 0.8], dtype=np.float64)
 
@@ -157,3 +164,194 @@ REALISTIC_URDF = """<?xml version="1.0" ?>
   <transmission name="t"><type>transmission_interface/SimpleTransmission</type><joint name="hip"><hardwareInterface>hardware_interface/EffortJointInterface</hardwareInterface></joint></transmission>
   <gazebo reference="leg"><mu1>0.8</mu1><self_collide>1</self_collide></gazebo>
 </robot>"""
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Test models for the compiled instances of the step kernel (batch.cu dispatch_spec): which instance a model takes depends on its
+# dimensions (nb, nq, nv, floating base, tree depth, dof-tree depth), its parent table, and whether it has more than 32 contact
+# candidates (two candidate slots per lane).  Each model below is built to reach one instance, or one bound of the loader.
+
+_RSC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "raisimlib_b200", "rsc")
+
+
+def _anymal_tree():
+    return ET.parse(os.path.join(_RSC, "anymal_c_like.urdf")).getroot()
+
+
+def _anymal_variant(feet_only=False, prismatic_knees=False):
+    root = _anymal_tree()
+    if feet_only:                       # the ANYmal-like tree with the four foot spheres as its only collision bodies
+        for link in root.findall("link"):
+            if not link.get("name").endswith("_FOOT"):
+                for c in link.findall("collision"):
+                    link.remove(c)
+    if prismatic_knees:                 # KFE joints slide along the shank instead of turning: jtype 2 inside the compiled chains
+        for j in root.findall("joint"):
+            if j.get("name").endswith("_KFE"):
+                j.set("type", "prismatic")
+                j.find("axis").set("xyz", "0 0 1")
+                lim = j.find("limit")
+                lim.set("lower", "-0.12"); lim.set("upper", "0.12"); lim.set("effort", "300")
+    return ET.tostring(root, encoding="unicode")
+
+
+def _urdf(name, links, joints):
+    """links: (name, mass, com, (ixx, iyy, izz), [collision geometry xml, xyz, rpy]); joints: (name, type, parent, child, xyz, rpy,
+    axis, (lower, upper, effort) or None)"""
+    s = f'<robot name="{name}">\n'
+    for ln, m, com, I, colls in links:
+        s += (f'  <link name="{ln}"><inertial><origin xyz="{com[0]} {com[1]} {com[2]}"/><mass value="{m}"/>'
+              f'<inertia ixx="{I[0]}" ixy="0" ixz="0" iyy="{I[1]}" iyz="0" izz="{I[2]}"/></inertial>\n')
+        for g, xyz, rpy in colls:
+            s += f'    <collision><origin xyz="{xyz[0]} {xyz[1]} {xyz[2]}" rpy="{rpy[0]} {rpy[1]} {rpy[2]}"/><geometry>{g}</geometry></collision>\n'
+        s += '  </link>\n'
+    for jn, jt, par, ch, xyz, rpy, ax, lim in joints:
+        s += (f'  <joint name="{jn}" type="{jt}"><parent link="{par}"/><child link="{ch}"/>'
+              f'<origin xyz="{xyz[0]} {xyz[1]} {xyz[2]}" rpy="{rpy[0]} {rpy[1]} {rpy[2]}"/><axis xyz="{ax[0]} {ax[1]} {ax[2]}"/>')
+        if lim is not None:
+            s += f'<limit lower="{lim[0]}" upper="{lim[1]}" effort="{lim[2]}" velocity="10"/>'
+        s += '</joint>\n'
+    return s + '</robot>\n'
+
+
+_Z3 = (0, 0, 0)
+
+
+def _quad_branched():
+    """The quadruped's dimensions (nb 13, nq 19, nv 18, floating, depth 3, dof depth 8) in a different tree: the left front hip
+    carries two children and the right hind leg has no shank, so the compiled 4 x 3-chain arithmetic does not apply."""
+    links = [("base", 25.0, (0, 0, 0.02), (0.22, 0.86, 0.93), [('<box size="0.58 0.28 0.18"/>', _Z3, _Z3)])]
+    joints = []
+    for leg, fx, fy, kids in (("LF", 1, 1, 3), ("RF", 1, -1, 2), ("LH", -1, 1, 2), ("RH", -1, -1, 1)):
+        links.append((f"{leg}_HIP", 2.0, (fx * 0.05, 0, 0), (0.0034, 0.0041, 0.004), []))
+        joints.append((f"{leg}_HAA", "revolute", "base", f"{leg}_HIP", (fx * 0.3, fy * 0.1, 0), _Z3, (1, 0, 0), (-0.72, 0.49, 80)))
+        links.append((f"{leg}_THIGH", 3.0, (0, fy * 0.04, -0.12), (0.024, 0.023, 0.0045), []))
+        joints.append((f"{leg}_HFE", "revolute", f"{leg}_HIP", f"{leg}_THIGH", (fx * 0.06, fy * 0.08, 0), _Z3, (0, 1, 0), (-3, 3, 80)))
+        if kids >= 2:
+            links.append((f"{leg}_SHANK", 0.85, (0, 0, -0.15), (0.006, 0.006, 0.0005), [('<sphere radius="0.03"/>', (0, 0, -0.3), _Z3)]))
+            joints.append((f"{leg}_KFE", "revolute", f"{leg}_THIGH", f"{leg}_SHANK", (0, fy * 0.1, -0.285), _Z3, (0, 1, 0), (-3, 3, 80)))
+        if kids >= 3:           # second child of the hip
+            links.append((f"{leg}_ARM", 0.5, (0.05, 0, 0), (0.001, 0.002, 0.002), [('<sphere radius="0.04"/>', (0.1, 0, 0), _Z3)]))
+            joints.append((f"{leg}_ARM_J", "revolute", f"{leg}_HIP", f"{leg}_ARM", (0.05, 0, 0.05), _Z3, (0, 0, 1), (-1, 1, 40)))
+    return _urdf("quad_branched", links, joints)
+
+
+def _hexapod():
+    """Floating base and six 3-joint legs: nb 19 (more than 16 bodies), exactly 32 contact candidates (one slot per lane)."""
+    links = [("base", 10.0, (0, 0, 0), (0.09, 0.3, 0.37), [('<box size="0.6 0.3 0.12"/>', _Z3, _Z3)])]     # 8 corners + 1 face
+    joints = []
+    for i, (x, s) in enumerate(((0.25, 1), (0.0, 1), (-0.25, 1), (0.25, -1), (0.0, -1), (-0.25, -1))):
+        links.append((f"coxa{i}", 0.5, (0, s * 0.03, 0), (0.0005, 0.0004, 0.0005),
+                      [('<sphere radius="0.04"/>', (0, s * 0.03, 0), _Z3)] if i < 5 else []))
+        joints.append((f"yaw{i}", "revolute", "base", f"coxa{i}", (x, s * 0.15, 0), _Z3, (0, 0, 1), (-0.6, 0.6, 40)))
+        links.append((f"femur{i}", 0.8, (0, s * 0.08, 0), (0.002, 0.0004, 0.002),
+                      [('<capsule radius="0.03" length="0.12"/>', (0, s * 0.08, 0), (1.5707963267948966, 0, 0))] if i < 4 else []))
+        joints.append((f"lift{i}", "revolute", f"coxa{i}", f"femur{i}", (0, s * 0.06, 0), _Z3, (1, 0, 0), (-1.2, 1.2, 40)))
+        links.append((f"tibia{i}", 0.3, (0, s * 0.01, -0.1), (0.001, 0.001, 0.0002), [('<sphere radius="0.025"/>', (0, s * 0.02, -0.2), _Z3)]))
+        joints.append((f"knee{i}", "revolute", f"femur{i}", f"tibia{i}", (0, s * 0.16, 0), _Z3, (1, 0, 0), (-2.0, 0.3, 30)))
+    return _urdf("hexapod", links, joints)
+
+
+def _max32():
+    """Every bound the loader accepts: nb 32 (one body per lane), nv 37 (> 32 dofs), depth 6, exactly 64 contact candidates of every
+    type (spheres, capsules, box corners and faces, cylinder rims), a prismatic joint, position and effort limits on every joint.
+    A floating star: five 6-link chains lying in the base plane (link 1 turns about the base normal), and a mast carrying a cylinder."""
+    links = [("base", 15.0, (0, 0, 0), (0.22, 0.33, 0.5), [('<box size="0.5 0.4 0.15"/>', _Z3, _Z3)])]
+    joints = [("mast_j", "revolute", "base", "mast", (0, 0, 0.1), _Z3, (0, 0, 1), (-1.0, 1.0, 20))]
+    links.append(("mast", 1.0, (0, 0, 0.1), (0.004, 0.004, 0.001), [('<cylinder radius="0.05" length="0.2"/>', (0, 0, 0.1), _Z3)]))
+    axes = [(0, 0, 1), (0, 1, 0), (1, 0, 0), (0, 1, 0), (1, 0, 0), (0, 1, 0)]
+    cap = ('<capsule radius="0.03" length="0.06"/>', (0.05, 0, 0), (0, 1.5707963267948966, 0))       # along the link
+    for c in range(5):
+        phi = 2 * np.pi * c / 5
+        parent = "base"
+        for k in range(6):
+            ln = f"c{c}_l{k + 1}"
+            colls = []
+            if k == 1 or (k == 2 and c in (1, 3, 4)):
+                colls.append(cap)
+            if k in (3, 5) or (k == 4 and c == 2):
+                colls.append(('<sphere radius="0.04"/>', (0.1, 0, 0), _Z3))
+            if k == 5 and c == 0:
+                colls.append(('<box size="0.06 0.04 0.03"/>', (0.05, 0, 0), _Z3))
+            links.append((ln, 0.6 - 0.07 * k, (0.05, 0, 0), (0.0004, 0.001, 0.001), colls))
+            xyz = (0.28 * np.cos(phi), 0.22 * np.sin(phi), 0) if k == 0 else (0.1, 0, 0)
+            rpy = (0, 0, phi) if k == 0 else _Z3
+            prismatic = c == 2 and k == 3
+            joints.append((f"c{c}_j{k + 1}", "prismatic" if prismatic else "revolute", parent, ln, xyz, rpy, (1, 0, 0) if prismatic else axes[k],
+                           (-0.05, 0.05, 200) if prismatic else (-0.5, 0.5, 15 + 5 * (k % 3))))
+            parent = ln
+    return _urdf("max32", links, joints)
+
+
+QUAD_FEET = _anymal_variant(feet_only=True)
+QUAD_PRISMATIC = _anymal_variant(prismatic_knees=True)
+QUAD_BRANCHED = _quad_branched()
+HEXAPOD = _hexapod()
+MAX32 = _max32()
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# GPU batch and oracles on the same seeded inputs
+
+def setup_batch(capi, urdf, n, seed, terrain="ground", base_z=0.45, vel=0.5, tau_scale=20.0, params=None, joint_scale=0.5):
+    from oracle.oracle import Oracle
+    from oracle.urdf_tables import load_tables
+    path = os.path.join(_RSC, urdf) if urdf.endswith(".urdf") else urdf
+    t = load_tables(path)
+    m = capi.Model(path)
+    bt = capi.Batch(m, n)
+    rng = np.random.default_rng(seed)
+    gc, gv = random_state(t, rng, n, vel_scale=vel, base_z=base_z, pos_scale=2.0, joint_scale=joint_scale)
+    tau = rng.uniform(-tau_scale, tau_scale, (n, t["nv"]))
+    if t["floating"]:
+        tau[:, :6] = 0
+    prm = dict(threshold=THRESH)     # everything else at the library defaults = what bench.py runs (accelerated sweeps, stagnation
+                                     # window 8 with the compliant fallback); tests of the plain published method pass accel_m=0, stall_window=0
+    prm.update(params or {})
+    o64, o32 = Oracle(t, params=prm), Oracle(t, precision="f32", params=prm)
+    bt.set_params(**{k: v for k, v in prm.items() if k not in ("gx", "gy", "gz")})
+    if any(k in prm for k in ("gx", "gy", "gz")):
+        bt.set_params(gravity=(prm.get("gx", 0.0), prm.get("gy", 0.0), prm.get("gz", -9.81)))
+    if terrain == "ground":
+        for o in (o64, o32):
+            o.set_ground(0.0)
+        bt.set_ground(0.0)
+    elif terrain == "hm":
+        xs, ys = 65, 49
+        H = (0.1 * rng.uniform(-1, 1, (ys, xs))).astype(np.float32)
+        for o in (o64, o32):
+            o.set_heightmap(xs, ys, 12.8, 9.6, 0.1, -0.2, H.astype(np.float64))
+        bt.set_heightmap(xs, ys, 12.8, 9.6, 0.1, -0.2, H)
+    gc32, gv32, tau32 = gc.astype(np.float32), gv.astype(np.float32), tau.astype(np.float32)
+    bt.set_control_mode(capi.FORCE_AND_TORQUE)
+    bt.set_state(gc32, gv32)
+    bt.set_generalized_force(tau32)
+    return t, bt, o64, o32, gc32.astype(np.float64), gv32.astype(np.float64), tau32.astype(np.float64)
+
+
+def index_parity(pts_gpu, cnt_gpu, d_ref, label):
+    """bit-exact contact lists, excluding environments that hold a candidate inside the margin."""
+    n = len(cnt_gpu)
+    shallow = (np.abs(d_ref["c_depth"]) < MARGIN) & (d_ref["c_pt"] >= 0)
+    ok_env = ~shallow.any(1)
+    excluded = int((~ok_env).sum())
+    mism = (pts_gpu != d_ref["c_pt"]).any(1) | (cnt_gpu != d_ref["ncontacts"])
+    # an environment may only mismatch if it has a margin candidate in the reference ...
+    hard = mism & ok_env
+    # ... or a candidate that the reference rejected by less than the margin (not recorded): allow
+    # those only if the contact COUNT differs by the extra near-zero candidates
+    print(f"[{label}] envs={n} contacts={int(cnt_gpu.sum())} margin-excluded envs={excluded} mismatching={int(mism.sum())}")
+    return hard
+
+
+def launch_config(capi, bt):
+    """the step kernel's launch as pick_config chose it: warps per CTA, CTAs, compiled instance (spec 0 generic, 1 quadruped,
+    2 humanoid) and candidate slots per lane"""
+    import ctypes
+    L = capi.lib()
+    L.rsb_internal_launch_config.argtypes = [ctypes.c_void_p] * 3
+    L.rsb_internal_launch_instance.argtypes = [ctypes.c_void_p] * 3
+    v = [ctypes.c_int() for _ in range(4)]
+    assert L.rsb_internal_launch_config(bt.h, ctypes.byref(v[0]), ctypes.byref(v[1])) == 0
+    assert L.rsb_internal_launch_instance(bt.h, ctypes.byref(v[2]), ctypes.byref(v[3])) == 0
+    return dict(zip(("wpc", "grid", "spec", "slots"), [x.value for x in v]))

@@ -9,7 +9,7 @@ import pytest
 from conftest import ROOT, RSC
 from raisimlib_b200 import capi
 from oracle.urdf_tables import load_tables
-from helpers import PENDULUM_URDF, BOX_URDF, REALISTIC_URDF
+from helpers import PENDULUM_URDF, BOX_URDF, REALISTIC_URDF, QUAD_FEET, QUAD_PRISMATIC, QUAD_BRANCHED, HEXAPOD, MAX32
 
 
 def _declared_symbols():
@@ -32,7 +32,9 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(capi.Params) == 4 * 19      # rsb_params: 16 words of round 1 + accel_m, accel_start, stall_reg
 
 
-@pytest.mark.parametrize("src", ["anymal_c_like.urdf", "atlas_like.urdf", PENDULUM_URDF, BOX_URDF, REALISTIC_URDF])
+@pytest.mark.parametrize("src", ["anymal_c_like.urdf", "atlas_like.urdf", PENDULUM_URDF, BOX_URDF, REALISTIC_URDF,
+                                 pytest.param(QUAD_FEET, id="quad_feet"), pytest.param(QUAD_PRISMATIC, id="quad_prismatic"),
+                                 pytest.param(QUAD_BRANCHED, id="quad_branched"), pytest.param(HEXAPOD, id="hexapod"), pytest.param(MAX32, id="max32")])
 def test_model_tables_match_python_restatement(src):
     path = os.path.join(RSC, src) if src.endswith(".urdf") else src
     a = capi.Model(path).tables()

@@ -14,14 +14,11 @@ import numpy as np
 import pytest
 
 from conftest import RSC
-from helpers import ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, random_state
+from helpers import ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, MARGIN, THRESH, setup_batch, index_parity
 from oracle.oracle import Oracle
 from oracle.urdf_tables import load_tables
 
 pytestmark = pytest.mark.gpu
-
-MARGIN = 2e-6          # metres; contact candidates shallower than this are excluded from index parity
-THRESH = 1e-6          # solver threshold used on both sides
 
 
 @pytest.fixture(scope="module")
@@ -32,58 +29,13 @@ def capi():
     return c
 
 
-def _setup(capi, urdf, n, seed, terrain="ground", base_z=0.45, vel=0.5, tau_scale=20.0, params=None, joint_scale=0.5):
-    path = os.path.join(RSC, urdf) if urdf.endswith(".urdf") else urdf
-    t = load_tables(path)
-    m = capi.Model(path)
-    bt = capi.Batch(m, n)
-    rng = np.random.default_rng(seed)
-    gc, gv = random_state(t, rng, n, vel_scale=vel, base_z=base_z, pos_scale=2.0, joint_scale=joint_scale)
-    tau = rng.uniform(-tau_scale, tau_scale, (n, t["nv"]))
-    if t["floating"]:
-        tau[:, :6] = 0
-    prm = dict(threshold=THRESH)     # everything else at the library defaults = what bench.py runs (accelerated sweeps, stagnation
-                                     # window 8 with the compliant fallback); tests of the plain published method pass accel_m=0, stall_window=0
-    prm.update(params or {})
-    o64, o32 = Oracle(t, params=prm), Oracle(t, precision="f32", params=prm)
-    bt.set_params(**{k: v for k, v in prm.items() if k not in ("gx", "gy", "gz")})
-    if any(k in prm for k in ("gx", "gy", "gz")):
-        bt.set_params(gravity=(prm.get("gx", 0.0), prm.get("gy", 0.0), prm.get("gz", -9.81)))
-    if terrain == "ground":
-        for o in (o64, o32):
-            o.set_ground(0.0)
-        bt.set_ground(0.0)
-    elif terrain == "hm":
-        xs, ys = 65, 49
-        H = (0.1 * rng.uniform(-1, 1, (ys, xs))).astype(np.float32)
-        for o in (o64, o32):
-            o.set_heightmap(xs, ys, 12.8, 9.6, 0.1, -0.2, H.astype(np.float64))
-        bt.set_heightmap(xs, ys, 12.8, 9.6, 0.1, -0.2, H)
-    gc32, gv32, tau32 = gc.astype(np.float32), gv.astype(np.float32), tau.astype(np.float32)
-    bt.set_control_mode(capi.FORCE_AND_TORQUE)
-    bt.set_state(gc32, gv32)
-    bt.set_generalized_force(tau32)
-    return t, bt, o64, o32, gc32.astype(np.float64), gv32.astype(np.float64), tau32.astype(np.float64)
-
-
-def _index_parity(pts_gpu, cnt_gpu, d_ref, label):
-    """bit-exact contact lists, excluding environments that hold a candidate inside the margin."""
-    n = len(cnt_gpu)
-    shallow = (np.abs(d_ref["c_depth"]) < MARGIN) & (d_ref["c_pt"] >= 0)
-    ok_env = ~shallow.any(1)
-    excluded = int((~ok_env).sum())
-    mism = (pts_gpu != d_ref["c_pt"]).any(1) | (cnt_gpu != d_ref["ncontacts"])
-    # an environment may only mismatch if it has a margin candidate in the reference ...
-    hard = mism & ok_env
-    # ... or a candidate that the reference rejected by less than the margin (not recorded): allow
-    # those only if the contact COUNT differs by the extra near-zero candidates
-    print(f"[{label}] envs={n} contacts={int(cnt_gpu.sum())} margin-excluded envs={excluded} mismatching={int(mism.sum())}")
-    return hard
+_setup = setup_batch
+_index_parity = index_parity
 
 
 @pytest.mark.parametrize("urdf,base_z", [("anymal_c_like.urdf", 0.45), ("atlas_like.urdf", 0.9), (PENDULUM_URDF, 0.0)])
 def test_stage_outputs_fk_crba_rnea(capi, urdf, base_z):
-    """a2 FK, a3 CRBA, a4 RNEA through integrate1() + the lazy getters."""
+    """a2 FK, a3 CRBA, a4 RNEA through integrate1() + the lazy getters (every compiled instance: tests/test_gpu_instances.py)."""
     t, bt, o64, o32, gc, gv, tau = _setup(capi, urdf, 128, seed=11, base_z=base_z, tau_scale=1.0)
     bt.integrate1()
     M, h = bt.mass_matrix(), bt.nonlinearities()

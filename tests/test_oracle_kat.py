@@ -10,9 +10,18 @@ import pytest
 from oracle.oracle import Oracle
 from oracle.urdf_tables import load_tables
 from helpers import (ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, mass_matrix_numpy, potential_energy,
-                     integrate_gc, random_state, fk_numpy, body_jacobians)
+                     integrate_gc, random_state, fk_numpy, body_jacobians, QUAD_FEET, QUAD_PRISMATIC, QUAD_BRANCHED, HEXAPOD, MAX32)
 
 G = 9.81
+# the models that reach every compiled instance of the step kernel (tests/test_gpu_instances.py): the oracle those tests compare with
+# is pinned on their shapes here first
+INSTANCE_MODELS = {"quad_feet": QUAD_FEET, "quad_prismatic": QUAD_PRISMATIC, "quad_branched": QUAD_BRANCHED, "hexapod": HEXAPOD, "max32": MAX32}
+
+
+def _tables(which, anymal_tables, atlas_tables):
+    if which in INSTANCE_MODELS:
+        return load_tables(INSTANCE_MODELS[which])
+    return {"anymal": anymal_tables, "atlas": atlas_tables}.get(which) or load_tables(PENDULUM_URDF)
 
 
 def test_tables_shapes(anymal_tables, atlas_tables):
@@ -41,9 +50,9 @@ def test_free_fall_closed_form(anymal_tables):
     assert np.allclose(gc[0, 3:7], [1, 0, 0, 0], atol=1e-12)
 
 
-@pytest.mark.parametrize("which", ["anymal", "atlas", "pendulum"])
+@pytest.mark.parametrize("which", ["anymal", "atlas", "pendulum", *INSTANCE_MODELS])
 def test_mass_matrix_vs_jacobian_sum(which, anymal_tables, atlas_tables):
-    t = {"anymal": anymal_tables, "atlas": atlas_tables}.get(which) or load_tables(PENDULUM_URDF)
+    t = _tables(which, anymal_tables, atlas_tables)
     o = Oracle(t)
     rng = np.random.default_rng(1)
     gc, gv = random_state(t, rng, 4, pos_scale=20.0)
@@ -71,9 +80,9 @@ def test_single_pendulum_closed_form():
     assert abs(d["h"][0, 0] - m * G * l * np.sin(q)) < 1e-12
 
 
-@pytest.mark.parametrize("which", ["anymal", "pendulum", "atlas"])
+@pytest.mark.parametrize("which", ["anymal", "pendulum", "atlas", *INSTANCE_MODELS])
 def test_gravity_bias_is_potential_gradient(which, anymal_tables, atlas_tables):
-    t = {"anymal": anymal_tables, "atlas": atlas_tables}.get(which) or load_tables(PENDULUM_URDF)
+    t = _tables(which, anymal_tables, atlas_tables)
     o = Oracle(t)
     rng = np.random.default_rng(2)
     gc, gv = random_state(t, rng, 2, vel_scale=0.0)
@@ -88,11 +97,11 @@ def test_gravity_bias_is_potential_gradient(which, anymal_tables, atlas_tables):
         assert np.allclose(d["h"][e], grad, atol=2e-5 * max(1.0, np.abs(grad).max()))
 
 
-@pytest.mark.parametrize("which", ["anymal", "pendulum", "atlas"])
+@pytest.mark.parametrize("which", ["anymal", "pendulum", "atlas", *INSTANCE_MODELS])
 def test_coriolis_bias_vs_lagrangian(which, anymal_tables, atlas_tables):
     """h(q,v) - h(q,0) must equal Mdot v - 1/2 d(v^T M v)/dq, with M from the independent numpy
     restatement and derivatives by central differences along the oracle's own (+) operator."""
-    t = {"anymal": anymal_tables, "atlas": atlas_tables}.get(which) or load_tables(PENDULUM_URDF)
+    t = _tables(which, anymal_tables, atlas_tables)
     o = Oracle(t, params=dict(gx=0.0, gy=0.0, gz=0.0))
     rng = np.random.default_rng(3)
     gc, gv = random_state(t, rng, 1, vel_scale=1.0)
