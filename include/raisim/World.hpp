@@ -52,6 +52,10 @@ class Contact {
   explicit Contact(const rsb_contact& c) : c_(c) {}
   size_t getlocalBodyIndex() const { return size_t(c_.local_body); }
   size_t getPairObjectIndex() const { return 0; }            // the terrain is object 0 of the world
+  // self-collision (ArticulatedSystem::setSelfCollisionPairs): a contact between two bodies of the robot.  The impulse and the normal act
+  // on getlocalBodyIndex() (normal from the other body towards it); the other body receives the negative impulse.
+  bool isSelfCollision() const { return c_.pair_index < 0; }
+  int getPairLocalBodyIndex() const { return c_.pair_index < 0 ? -1 - c_.pair_index : -1; }   // the other body of a self contact, -1 on terrain
   int getPairContactIndexInPairObject() const { return c_.pair_index; }
   Vec<3> getPosition() const { return {c_.position[0], c_.position[1], c_.position[2]}; }
   Vec<3> getNormal() const { return {c_.normal[0], c_.normal[1], c_.normal[2]}; }
@@ -456,6 +460,35 @@ class ArticulatedSystem {
   void setCollisionBodyFriction(size_t collisionBodyIdx, double mu) {
     rsbCheck(rsb_batch_set_collision_friction(w_->batch(), int(collisionBodyIdx), float(mu)), "setCollisionBodyFriction");
   }
+  // Self-collision.  Upstream checks the bodies of an articulated system against each other and user code switches single pairs off
+  // with ignoreCollisionBetween; here self-collision is OFF until explicit pairs of collision bodies are enabled ("LINK/k" names as in
+  // getCollisionBody; at most RSB_MAX_SELF_PAIRS; sphere / capsule pairs and sphere-box), optionally each with its own friction.  The
+  // pairs hold for every environment of the batch.  An empty list switches self-collision off again.
+  void setSelfCollisionPairs(const std::vector<std::pair<std::string, std::string>>& pairs, const std::vector<double>& mu = {}) {
+    if (!mu.empty() && mu.size() != pairs.size()) throw std::runtime_error("setSelfCollisionPairs: one friction value per pair");
+    std::vector<int32_t> idx;
+    for (const auto& p : pairs) {
+      for (const std::string* n : {&p.first, &p.second}) {
+        const int i = rsb_model_collision_index(w_->model(), n->c_str());
+        rsbCheck(i, "setSelfCollisionPairs");
+        idx.push_back(i);
+      }
+    }
+    applySelfPairs(idx, std::vector<float>(mu.begin(), mu.end()));
+  }
+  // removes the enabled self-collision pairs between the two bodies (local body indices), in either order
+  void ignoreCollisionBetween(size_t bodyIdx1, size_t bodyIdx2) {
+    rsb_model_tables t{};
+    rsbCheck(rsb_model_get_tables(w_->model(), &t), "ignoreCollisionBetween");
+    std::vector<int32_t> idx; std::vector<float> mu;
+    for (size_t j = 0; j < selfMu_.size(); j++) {
+      const int b1 = t.cbody[selfPairs_[2 * j]], b2 = t.cbody[selfPairs_[2 * j + 1]];
+      if ((b1 == int(bodyIdx1) && b2 == int(bodyIdx2)) || (b1 == int(bodyIdx2) && b2 == int(bodyIdx1))) continue;
+      idx.push_back(selfPairs_[2 * j]); idx.push_back(selfPairs_[2 * j + 1]); mu.push_back(selfMu_[j]);
+    }
+    applySelfPairs(idx, mu);
+  }
+  size_t getNumberOfSelfCollisionPairs() const { return selfMu_.size(); }
   VecDyn getNonlinearities() const {
     std::vector<float> h(w_->nv());
     rsbCheck(rsb_batch_get_nonlinearities(w_->batch(), env_, 1, h.data(), RSB_HOST), "getNonlinearities");
@@ -660,8 +693,16 @@ class ArticulatedSystem {
   void pushWrench() {
     rsbCheck(rsb_batch_set_external_wrench(w_->batch(), extBody_, extF_, extT_, extP_, env_, 1, RSB_HOST), "setExternalForce");
   }
+  void applySelfPairs(const std::vector<int32_t>& idx, const std::vector<float>& mu) {
+    const int n = int(idx.size() / 2);
+    rsbCheck(rsb_batch_set_self_collision(w_->batch(), idx.data(), n, mu.empty() ? nullptr : mu.data()), "setSelfCollisionPairs");
+    selfPairs_ = idx;
+    selfMu_ = mu.empty() ? std::vector<float>(n, -1.f) : mu;
+  }
   std::map<size_t, std::string> collisionMaterial_;   // collision body -> material name (absent = "default")
   bool materialsDirty_ = false;
+  std::vector<int32_t> selfPairs_;                    // enabled self-collision pairs: [n][2] collision bodies
+  std::vector<float> selfMu_;                         // their friction (< 0: default material)
   int extBody_ = -1; bool extHasForce_ = false;
   float extF_[3] = {0, 0, 0}, extT_[3] = {0, 0, 0}, extP_[3] = {0, 0, 0};
   struct Poses { std::vector<float> R, p; };
@@ -851,7 +892,8 @@ class World {
   };
   ContactSolverView getContactSolver() const { need(); return ContactSolverView{this}; }
   ArticulatedSystem* getObject(const std::string& name) { return (robot_ && robot_->getName() == name) ? robot_.get() : nullptr; }
-  // object-object and self collisions are not part of this path (robot vs terrain only): nothing to ignore
+  // object-object collisions are not part of this path (one robot against the terrain): nothing to ignore.  Self-collision pairs of the
+  // robot are removed with ArticulatedSystem::ignoreCollisionBetween(bodyIdx1, bodyIdx2).
   void ignoreCollisionBetween(size_t, size_t, size_t, size_t) {}
   // one World::integrate() of THIS environment's batch.  Views of a shared batch must not call this
   // per environment -- the vectorized wrapper steps the whole batch once (see VectorizedEnvironment.hpp).

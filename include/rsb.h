@@ -82,9 +82,10 @@ typedef struct rsb_params {
 /* raisim::Contact as returned by ArticulatedSystem::getContacts(): 12 words */
 typedef struct rsb_contact {
   int32_t local_body;  /* Contact::getlocalBodyIndex()                                      */
-  int32_t pair_index;  /* terrain feature: 0 = Ground plane, 2*cell+tri on a HeightMap     */
+  int32_t pair_index;  /* terrain feature: 0 = Ground plane, 2*cell+tri on a HeightMap;   */
+                       /* self contact: -1 - the pair's second body (always < 0)           */
   float position[3];   /* Contact::getPosition()  (world)                                   */
-  float normal[3];     /* Contact::getNormal()    (world, terrain -> robot)                 */
+  float normal[3];     /* Contact::getNormal()    (world, terrain -> robot; self: second -> first body) */
   float impulse[3];    /* Contact::getImpulse()   (world, on the robot)                     */
   float depth;         /* Contact::getDepth()                                               */
 } rsb_contact;
@@ -154,6 +155,19 @@ int rsb_params_default(rsb_params* p);
 /* friction of one collision body (index in rsb_model_tables order) against the terrain; mu < 0 = default material.
  * The per-body half of World::setMaterialPairProp / getCollisionBody(name).setMaterial */
 int rsb_batch_set_collision_friction(rsb_batch* b, int collision_body, float mu);
+/* Self-collision between the bodies of the robot (ArticulatedSystem collisions between its own bodies): OFF unless pairs are enabled
+ * here.  pairs[n][2] are collision-body indices (rsb_model_tables / rsb_model_collision_index order), at most RSB_MAX_SELF_PAIRS; there
+ * is no "all pairs" mode.  Supported: sphere-sphere, sphere-capsule, capsule-capsule, sphere-box (RSB_ERR_UNSUPPORTED, naming the pair,
+ * for capsule-box, box-box and anything with a cylinder); two collision bodies of the same body are RSB_ERR_INVALID; parent-child pairs
+ * are allowed; the world-welded root of a fixed-base robot acts as a static obstacle.  One contact per pair at the deepest point: normal
+ * from the pair's second body to its first, position = midpoint of the two surface points, depth = penetration.  The impulse acts on the
+ * first body and its negative on the second; friction mu[j] (NULL or mu[j] < 0: the default material; the per-collision-body terrain
+ * friction does not apply); ERP and restitution as on terrain contacts.  Self contacts share the RSB_KMAX contacts with the terrain:
+ * pair j is candidate npts + j (rsb_batch_get_contact_points), its rsb_contact has local_body = first body and
+ * pair_index = -1 - second body.  n = 0 clears the pairs.  Everything is checked first: a refused call changes nothing.  A batch with
+ * pairs runs the generic (not the model-specific) instance of the step kernel. */
+#define RSB_MAX_SELF_PAIRS 32
+int rsb_batch_set_self_collision(rsb_batch* b, const int32_t* pairs, int n, const float* mu);
 
 /* ---- state and actuation (ArticulatedSystem::setState/getState/setPdGains/setPdTarget/
  *      setGeneralizedForce/setControlMode); buffers are tight [env_count][nq|nv] float32 ---------- */

@@ -96,7 +96,7 @@ EXPORTED = [
     "rsb_model_body_name", "rsb_model_collision_index", "rsb_model_joint_name", "rsb_model_frame_index", "rsb_model_frame",
     "rsb_batch_create", "rsb_batch_destroy", "rsb_batch_set_stream", "rsb_batch_sync", "rsb_batch_num_envs",
     "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
-    "rsb_batch_set_collision_friction",
+    "rsb_batch_set_collision_friction", "rsb_batch_set_self_collision",
     "rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_gains", "rsb_batch_set_pd_target",
     "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
     "rsb_batch_integrate1", "rsb_batch_integrate2", "rsb_batch_integrate",
@@ -144,6 +144,7 @@ def lib():
         L.rsb_batch_set_heightmap.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p]
         L.rsb_batch_clear_terrain.argtypes = [C.c_void_p]
         L.rsb_batch_set_collision_friction.argtypes = [C.c_void_p, C.c_int, C.c_float]
+        L.rsb_batch_set_self_collision.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.rsb_batch_set_params.argtypes = [C.c_void_p, C.POINTER(Params)]
         L.rsb_batch_get_params.argtypes = [C.c_void_p, C.POINTER(Params)]
         L.rsb_params_default.argtypes = [C.POINTER(Params)]
@@ -310,6 +311,16 @@ class Batch:
 
     def set_collision_friction(self, collision_body, mu):
         _ck(lib().rsb_batch_set_collision_friction(self.h, collision_body, mu))
+
+    def set_self_collision(self, pairs, mu=None):
+        """enable self-collision between pairs of collision bodies ([n, 2] indices, or collision-body names "LINK/k"); mu [n] per-pair
+        friction (None: the default material).  An empty list clears the pairs.  Pair j's contacts have candidate index npts + j and
+        pair_index -1 - second body."""
+        rows = [[self.model.collision_index(c) if isinstance(c, str) else int(c) for c in p] for p in pairs]
+        pp = np.ascontiguousarray(np.asarray(rows, np.int32).reshape(-1, 2))
+        m = None if mu is None else np.ascontiguousarray(np.broadcast_to(np.asarray(mu, np.float32), (len(pp),)))
+        _ck(lib().rsb_batch_set_self_collision(self.h, pp.ctypes.data_as(C.c_void_p), len(pp),
+                                               None if m is None else m.ctypes.data_as(C.c_void_p)))
 
     def get_params(self):
         p = Params()

@@ -74,6 +74,8 @@ struct rsb_batch {
   int slots = 1;
   TerrainDesc ter{};
   std::vector<float> kp, kd;
+  std::vector<int32_t> self_pairs;   // [n][2] collision bodies of the enabled self-collision pairs (rsb_batch_set_self_collision)
+  std::vector<float> self_mu;        // [n] their friction (< 0: default material)
   int wpc = 0, grid = 0;
   size_t smem_bytes = 0;
   int64_t launches = 0;
@@ -112,7 +114,8 @@ static void build_blob(rsb_batch* b) {
   }
   lvl[DL] = (int)lvldofs.size(); entstart[DL] = (int)ent.size();
   b->dims = Dims{md.nb, md.nq, md.nv, md.floating, md.maxdepth, maxdd};
-  H = make_blob_header(b->dims, md.npts(), (int)ent.size(), md.ncoll());
+  const int npairs = (int)b->self_mu.size();
+  H = make_blob_header(b->dims, md.npts(), (int)ent.size(), md.ncoll(), npairs);
   {
     bool ident = true;
     for (int i = 1; i < md.nb; i++) for (int k = 0; k < 9; k++) if (std::fabs(md.jrot[9 * i + k] - ((k % 4 == 0) ? 1.0 : 0.0)) > 0.0) ident = false;
@@ -197,10 +200,42 @@ static void build_blob(rsb_batch* b) {
       F(H.off_sec + NROUNDS * SEC_STRIDE + r * SEC_STRIDE + k, (float)std::sin(width * k / NSEC));
     }
   }
+  for (int j = 0; j < npairs; j++) {   // self-collision pairs (PairField): spheres and capsules as swept segments, sphere-box with the sphere in A
+    const int c1 = b->self_pairs[2 * j], c2 = b->self_pairs[2 * j + 1];
+    const bool box = md.ctype[c1] == CT_BOX || md.ctype[c2] == CT_BOX, flip = md.ctype[c1] == CT_BOX;
+    const int ca = flip ? c2 : c1, cb = flip ? c1 : c2;
+    const int o = H.off_pair + PAIR_WORDS * j;
+    I(o + PR_KIND, box ? 1 : 0); I(o + PR_FLIP, flip ? 1 : 0); I(o + PR_BODY1, md.cbody[c1]); I(o + PR_BODY2, md.cbody[c2]);
+    I(o + PR_BA, md.cbody[ca]); I(o + PR_BB, md.cbody[cb]);
+    // segment ends in the body frame: centre -/+ half length along the shape's z axis (a sphere: both ends at the centre)
+    auto seg = [&](int c, int f0, int f1, double& half) {
+      const double* p = &md.cpos[3 * c]; const double* R = &md.crot[9 * c];
+      half = md.ctype[c] == CT_CAPSULE ? md.csize[3 * c + 1] : 0.0;
+      for (int q = 0; q < 3; q++) { F(o + f0 + q, (float)(p[q] - half * R[3 * q + 2])); F(o + f1 + q, (float)(p[q] + half * R[3 * q + 2])); }
+    };
+    double ha = 0, hb = 0;
+    seg(ca, PR_A0, PR_A1, ha);
+    F(o + PR_RA, (float)md.csize[3 * ca]);
+    double cull_b;
+    if (box) {
+      for (int q = 0; q < 3; q++) { F(o + PR_B0 + q, (float)md.cpos[3 * cb + q]); F(o + PR_B1 + q, (float)md.csize[3 * cb + q]); }
+      for (int q = 0; q < 9; q++) F(o + PR_BR + q, (float)md.crot[9 * cb + q]);
+      F(o + PR_RB, 0.f);
+      cull_b = std::sqrt(md.csize[3 * cb] * md.csize[3 * cb] + md.csize[3 * cb + 1] * md.csize[3 * cb + 1] + md.csize[3 * cb + 2] * md.csize[3 * cb + 2]);
+    } else {
+      seg(cb, PR_B0, PR_B1, hb);
+      for (int q = 0; q < 9; q++) F(o + PR_BR + q, q % 4 == 0 ? 1.f : 0.f);
+      F(o + PR_RB, (float)md.csize[3 * cb]);
+      cull_b = md.csize[3 * cb] + hb;
+    }
+    F(o + PR_MU, b->self_mu[j]);
+    // bounding spheres of the stage-B cull, widened so that float32 rounding never culls a touching pair
+    F(o + PR_CULL_A, (float)((md.csize[3 * ca] + ha) * 1.0001 + 1e-6)); F(o + PR_CULL_B, (float)(cull_b * 1.0001 + 1e-6));
+  }
   std::memcpy(B.data(), &H, sizeof(H));
 }
 
-static void build_ws_layout(rsb_batch* b) { b->ws = make_ws_layout(b->dims); }
+static void build_ws_layout(rsb_batch* b) { b->ws = make_ws_layout(b->dims, (int)b->self_mu.size()); }
 
 // ------------------------------------------------------------------ launches --------------------
 // static specialisations: every 12-joint quadruped (ANYmal, A1, Go1, ...) shares (13,19,18,floating,3,8);
@@ -246,6 +281,7 @@ static int pick_config(rsb_batch* b) {
   }
   b->spec = quad_topology ? 1 : (same_dims(b->dims, kHumanoid30) ? 2 : 0);
   if (const char* e = getenv("RSB_FORCE_GENERIC")) if (atoi(e)) b->spec = 0;
+  if (!b->self_mu.empty()) b->spec = 0;   // self-collision pairs are compiled into the generic instance only
   // Warps per CTA (= resident environments per CTA).  A round of w resident warps per SM costs ~ max(13, w): latency-bound up to a
   // dozen warps, issue-bound beyond.  Choose the option with the smallest rounds x cost, ties to the larger CTA (one sub-step
   // barrier group, one copy of the model block).  On the 132 SMs of an H100, 4096 ANYmal-like environments (7.5 KB workspaces, at
@@ -664,6 +700,59 @@ int rsb_batch_set_collision_friction(rsb_batch* b, int collision_body, float mu)
   CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
+// self-collision between explicit pairs of collision bodies (n = 0: none, the default).  Everything is checked before anything changes:
+// a refused call leaves the batch as it was.  The pair table goes to the end of the model blob; a batch with pairs runs the generic
+// instance of the step kernel (pick_config) with room for the pairs in stage B's hit list and a second column block for stage C.
+int rsb_batch_set_self_collision(rsb_batch* b, const int32_t* pairs, int n, const float* mu) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (n < 0 || n > MAX_SELF_PAIRS) return fail(RSB_ERR_INVALID, "at most " + std::to_string(MAX_SELF_PAIRS) + " self-collision pairs per batch (got " + std::to_string(n) + ")");
+  if (n > 0 && !pairs) return fail(RSB_ERR_INVALID, "null pair list");
+  const Model& md = b->model->md;
+  static const char* shape[] = {"sphere", "box", "capsule", "cylinder"};
+  for (int j = 0; j < n; j++) {
+    const int c1 = pairs[2 * j], c2 = pairs[2 * j + 1];
+    if (c1 < 0 || c1 >= md.ncoll() || c2 < 0 || c2 >= md.ncoll())
+      return fail(RSB_ERR_INVALID, "self-collision pair " + std::to_string(j) + ": collision body index out of range (the model has " + std::to_string(md.ncoll()) + ")");
+    if (md.cbody[c1] == md.cbody[c2])
+      return fail(RSB_ERR_INVALID, "self-collision pair " + std::to_string(j) + ": collision bodies " + md.coll_names[c1] + " and " + md.coll_names[c2] + " are on the same body");
+    const int t1 = md.ctype[c1], t2 = md.ctype[c2];
+    const bool round1 = t1 == CT_SPHERE || t1 == CT_CAPSULE, round2 = t2 == CT_SPHERE || t2 == CT_CAPSULE;
+    const bool ok = (round1 && round2) || (t1 == CT_SPHERE && t2 == CT_BOX) || (t1 == CT_BOX && t2 == CT_SPHERE);
+    if (!ok)
+      return fail(RSB_ERR_UNSUPPORTED, "self-collision pair " + std::to_string(j) + " (" + md.coll_names[c1] + ", " + md.coll_names[c2] + "): " + shape[t1] + "-" + shape[t2] +
+                                           " is not supported (sphere-sphere, sphere-capsule, capsule-capsule and sphere-box are)");
+    if (mu && !(mu[j] < 0.f || mu[j] >= 0.f)) return fail(RSB_ERR_INVALID, "self-collision pair " + std::to_string(j) + ": friction is not a number");
+  }
+  CK(cudaSetDevice(b->device));
+  CK(cudaStreamSynchronize(b->stream));
+  // the friction overrides of rsb_batch_set_collision_friction live in the blob: carry them over (the candidate table does not move)
+  const std::vector<uint32_t> old_fric(b->blob_host.begin() + b->hdr.off_pts + 5 * b->hdr.nptp, b->blob_host.begin() + b->hdr.off_pts + 6 * b->hdr.nptp);
+  std::vector<int32_t> old_pairs = b->self_pairs; std::vector<float> old_mu = b->self_mu;
+  auto apply = [&]() -> int {
+    build_blob(b);
+    std::copy(old_fric.begin(), old_fric.end(), b->blob_host.begin() + b->hdr.off_pts + 5 * b->hdr.nptp);
+    build_ws_layout(b);
+    return pick_config(b);
+  };
+  b->self_pairs.assign(pairs ? pairs : nullptr, pairs ? pairs + 2 * n : nullptr);
+  b->self_mu.assign(n, -1.f);
+  for (int j = 0; j < n && mu; j++) b->self_mu[j] = mu[j];
+  int rc = apply();
+  uint32_t* blob = nullptr;
+  if (rc == RSB_OK && cudaMalloc((void**)&blob, b->blob_host.size() * 4) != cudaSuccess) rc = fail(RSB_ERR_CUDA, "rsb_batch_set_self_collision: out of device memory");
+  if (rc != RSB_OK) {   // back to the previous pair set (the message of the failure stays)
+    const std::string msg = g_err;
+    b->self_pairs = old_pairs; b->self_mu = old_mu;
+    apply();
+    g_err = msg;
+    return rc;
+  }
+  CK(cudaMemcpy(blob, b->blob_host.data(), b->blob_host.size() * 4, cudaMemcpyHostToDevice));
+  cudaFree(b->blob);
+  b->blob = blob;
+  return RSB_OK;
+}
+
 int rsb_batch_set_pd_target(rsb_batch* b, const float* ptarget, const float* vtarget, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (ptarget) b->pt_bound = nullptr;     // copying targets in ends a zero-copy binding

@@ -70,15 +70,24 @@ struct BlobHeader {
   int off_coll, ncoll; // collision-body table (box features): [ncoll][COLL_WORDS] = half extents, body-frame position, rotation
   int words, flags;    // flags bit0: every joint origin has identity rotation (rpy = 0 in the URDF); bits 8..15: largest
                        // non-root subtree size - 1 (loop bound of stage A's subtree accumulation)
+  int npairs, off_pair; // enabled self-collision pairs (rsb_batch_set_self_collision; 0 = off) and their table: [npairs][PAIR_WORDS]
 };
-static_assert(sizeof(BlobHeader) == 136, "header is 34 words");
-constexpr int HEADER_WORDS = 36;      // padded to a 16-byte multiple
+static_assert(sizeof(BlobHeader) == 144, "header is 36 words");
+constexpr int HEADER_WORDS = 36;      // a 16-byte multiple
 constexpr int PT_ROWS = 15;           // candidate table rows: body, pos(3), radius, friction override, type, pos2(3), collision body, cull point(3), cull radius
 constexpr int COLL_WORDS = 16;
+constexpr int MAX_SELF_PAIRS = RSB_MAX_SELF_PAIRS;   // one lane of stage B each
+// Self-collision pair row (one contact per pair, candidate index npts + j).  Geometry in the frames of two bodies A and B: kind 0 = the
+// segment a0..a1 swept by rA against b0..b1 swept by rB (a sphere is a segment of length 0), kind 1 = the sphere a0, rA against the box of
+// centre b0, half extents b1 and rotation bR in the frame of B.  The normal points from B to A, negated when flip = 1 (the caller listed
+// the box first).  The impulse acts on body1, its negative on body2.  Cull radii: bounding spheres about the middle of a0..a1 and of
+// b0..b1 (kind 0) or about b0 (kind 1).
+enum PairField { PR_KIND = 0, PR_FLIP = 1, PR_BODY1 = 2, PR_BODY2 = 3, PR_BA = 4, PR_BB = 5, PR_A0 = 6, PR_A1 = 9, PR_B0 = 12, PR_B1 = 15,
+                 PR_BR = 18, PR_RA = 27, PR_RB = 28, PR_MU = 29, PR_CULL_A = 30, PR_CULL_B = 31, PAIR_WORDS = 32 };
 
 // Every offset except off_ent / words depends on Dims only: the two variable-size tables
 // (candidate points, factorisation entry list) sit at the end.
-__host__ __device__ constexpr BlobHeader make_blob_header(Dims d, int npts, int nent, int ncoll = 0) {
+__host__ __device__ constexpr BlobHeader make_blob_header(Dims d, int npts, int nent, int ncoll = 0, int npairs = 0) {
   BlobHeader H{};
   H.nb = d.nb; H.nq = d.nq; H.nv = d.nv; H.npts = npts; H.floating = d.floating; H.maxdepth = d.maxdepth;
   H.nbp = d.nb | 1;                       // odd stride: field-major reads by body index stay conflict-free
@@ -105,9 +114,14 @@ __host__ __device__ constexpr BlobHeader make_blob_header(Dims d, int npts, int 
   H.off_pts = off; off += PT_ROWS * H.nptp;           // body, pos(3), radius, friction override (< 0: default material), type, pos2(3), collision body, cull point(3) + radius
   H.ncoll = ncoll; H.off_coll = off; off += COLL_WORDS * ncoll;
   H.off_ent = off; off += max_c(1, nent);
+  H.npairs = npairs; H.off_pair = off; off += PAIR_WORDS * npairs;   // at the end: without pairs the blob is what it was
   H.words = round_up_c(off, 4);
   return H;
 }
+
+// second column block of the self contacts (stage C): Y of the pair's second body, [ancestor depth][contact row], at the end of the
+// workspace; allocated only when pairs are enabled (make_ws_layout)
+__host__ __device__ constexpr int self_y_words(int maxdd) { return round_up_c((maxdd + 1) * (3 * RSB_KMAX + RSB_LMAX + 1), 4); }
 
 // per-warp workspace layout (word offsets)
 struct WsLayout {
@@ -117,7 +131,7 @@ struct WsLayout {
   int words;
 };
 
-__host__ __device__ constexpr WsLayout make_ws_layout(Dims d) {
+__host__ __device__ constexpr WsLayout make_ws_layout(Dims d, int npairs = 0) {
   WsLayout L{};
   const int nvp = round_up_c(max_c(d.nv, 1), 4), nqp = round_up_c(max_c(d.nq, 1), 4), nbp = d.nb | 1, dlp = (d.maxdd + 1) | 1;
   int o = 0;
@@ -138,6 +152,7 @@ __host__ __device__ constexpr WsLayout make_ws_layout(Dims d) {
   L.o_sat = o; o += nvp;                                          // dof driven at its actuator effort limit in this sub-step (stage C -> E)
   L.o_hist = o; o += HIST_WORDS;                                  // Anderson acceleration: u0, x, g, f, dG, dF (one value per constraint row each)
   if (o - L.o_Y < 9 * 64) o = L.o_Y + 9 * 64;                     // stage B keeps its hit list (HL_CAP rows of HL_WORDS) in [o_Y, here): dead until stage C
+  if (npairs > 0 && o - L.o_Y < 9 * (64 + npairs)) o = L.o_Y + 9 * (64 + npairs);   // ... and one row per self-collision pair
   // union: {h, b, poses} (stages A-C) overlaid by G (stages C-D)
   int ua = 0;
   L.o_h = o + ua; ua += nvp;
@@ -146,6 +161,7 @@ __host__ __device__ constexpr WsLayout make_ws_layout(Dims d) {
   L.o_G = o;
   const int ub = round_up_c(RMAX * GP, 4);
   o += max_c(ua, ub);
+  if (npairs > 0) o += self_y_words(d.maxdd);                     // the self contacts' second column block: the last self_y_words of the workspace
   L.words = round_up_c(o, 32);
   return L;
 }
@@ -392,11 +408,77 @@ __device__ __forceinline__ QuadLeg quad_factor_legs(float* s_L, float* s_invd, i
 constexpr int HL_WORDS = 9;            // depth (<= 0: dropped), normal, position, pair, candidate index; odd stride: conflict-free by lane
 constexpr int HL_CAP = 64;             // two candidate slots per lane at most
 
+// ---- self-collision pairs (generic instance only): the narrow phase of one pair, the oracle's SelfPair routine in float32
+// (oracle/self_collision.hpp self_pair_geometry: same closest-point rule for parallel and degenerate segments, same face rule inside a box)
+__device__ __forceinline__ void self_closest_segments(f3 p1, f3 d1, f3 p2, f3 d2, float& s, float& t) {
+  const f3 r = p1 - p2;
+  const float a = dot(d1, d1), e = dot(d2, d2), f = dot(d2, r);
+  if (a == 0.f && e == 0.f) { s = t = 0.f; return; }
+  if (a == 0.f) { s = 0.f; t = fminf(fmaxf(f / e, 0.f), 1.f); return; }
+  const float c = dot(d1, r);
+  if (e == 0.f) { t = 0.f; s = fminf(fmaxf(-c / a, 0.f), 1.f); return; }
+  const float b = dot(d1, d2), den = a * e - b * b;
+  s = den > 1e-6f * a * e ? fminf(fmaxf((b * f - c * e) / den, 0.f), 1.f) : 0.f;
+  t = (b * s + f) / e;
+  if (t < 0.f) { t = 0.f; s = fminf(fmaxf(-c / a, 0.f), 1.f); }
+  else if (t > 1.f) { t = 1.f; s = fminf(fmaxf((b - c) / a, 0.f), 1.f); }
+}
+// pair row pr (PairField), body poses of stage A: false when the shapes do not overlap; else depth, normal (second body -> first), position
+__device__ __noinline__ bool self_pair_contact(const float* pr, const float* s_pose, int nbp, float& depth, f3& n, f3& pos) {
+  const int* pri = reinterpret_cast<const int*>(pr);
+  const int bA = pri[PR_BA], bB = pri[PR_BB];
+  float RA[9], RB[9];
+#pragma unroll
+  for (int q = 0; q < 9; q++) { RA[q] = s_pose[(PF_R + q) * nbp + bA]; RB[q] = s_pose[(PF_R + q) * nbp + bB]; }
+  const f3 pA = mk(s_pose[(PF_P + 0) * nbp + bA], s_pose[(PF_P + 1) * nbp + bA], s_pose[(PF_P + 2) * nbp + bA]);
+  const f3 pB = mk(s_pose[(PF_P + 0) * nbp + bB], s_pose[(PF_P + 1) * nbp + bB], s_pose[(PF_P + 2) * nbp + bB]);
+  const float ra = pr[PR_RA], rb = pr[PR_RB];
+  f3 ng, SA, SB;
+  if (pri[PR_KIND] == 0) {
+    const f3 A0 = pA + mulR(RA, mk(pr[PR_A0], pr[PR_A0 + 1], pr[PR_A0 + 2])), A1 = pA + mulR(RA, mk(pr[PR_A1], pr[PR_A1 + 1], pr[PR_A1 + 2]));
+    const f3 B0 = pB + mulR(RB, mk(pr[PR_B0], pr[PR_B0 + 1], pr[PR_B0 + 2])), B1 = pB + mulR(RB, mk(pr[PR_B1], pr[PR_B1 + 1], pr[PR_B1 + 2]));
+    float s, t;
+    self_closest_segments(A0, A1 - A0, B0, B1 - B0, s, t);
+    const f3 QA = A0 + s * (A1 - A0), QB = B0 + t * (B1 - B0), v = QA - QB;
+    const float dist = sqrtf(dot(v, v));
+    depth = ra + rb - dist;
+    if (!(depth > 0.f)) return false;
+    ng = dist > 1e-9f ? (1.0f / dist) * v : mk(0.f, 0.f, 1.f);      // coincident centres / axes: +z, a fixed rule
+    SA = QA - ra * ng; SB = QB + rb * ng;
+  } else {
+    const f3 C = pA + mulR(RA, mk(pr[PR_A0], pr[PR_A0 + 1], pr[PR_A0 + 2])), cb = pB + mulR(RB, mk(pr[PR_B0], pr[PR_B0 + 1], pr[PR_B0 + 2]));
+    float R[9];
+    matmul3(RB, pr + PR_BR, R);
+    const f3 q = mulRt(R, C - cb), h = mk(pr[PR_B1], pr[PR_B1 + 1], pr[PR_B1 + 2]);
+    const f3 cl = mk(fminf(fmaxf(q.x, -h.x), h.x), fminf(fmaxf(q.y, -h.y), h.y), fminf(fmaxf(q.z, -h.z), h.z));
+    f3 nl, bp;
+    if (q.x != cl.x || q.y != cl.y || q.z != cl.z) {                  // centre outside the box: the clamped point is the closest one
+      const f3 d = q - cl;
+      const float dist = sqrtf(dot(d, d));
+      depth = ra - dist;
+      if (!(depth > 0.f)) return false;
+      nl = (1.0f / dist) * d; bp = cl;
+    } else {                                                           // inside: out through the nearest face, ties to the lowest axis
+      const float px = h.x - fabsf(q.x), py = h.y - fabsf(q.y), pz = h.z - fabsf(q.z);
+      bp = q;
+      if (px <= py && px <= pz) { depth = ra + px; nl = mk(q.x >= 0.f ? 1.f : -1.f, 0.f, 0.f); bp.x = nl.x * h.x; }
+      else if (py <= pz) { depth = ra + py; nl = mk(0.f, q.y >= 0.f ? 1.f : -1.f, 0.f); bp.y = nl.y * h.y; }
+      else { depth = ra + pz; nl = mk(0.f, 0.f, q.z >= 0.f ? 1.f : -1.f); bp.z = nl.z * h.z; }
+    }
+    ng = mulR(R, nl);
+    SA = C - ra * ng; SB = cb + mulR(R, bp);
+  }
+  n = pri[PR_FLIP] ? -1.f * ng : ng;
+  pos = 0.5f * (SA + SB);
+  return true;
+}
+
 #ifndef RSB_STAGE_B_INLINE
 #define RSB_STAGE_B_INLINE __forceinline__
 #endif
 // ter: the kernel parameter itself (constant bank); ter_s: its shared-memory copy, for the out-of-line shape routines
-template <int SLOTS>
+// SELF: the generic instance, which also runs the self-collision pairs of the blob (lane = pair, after the terrain candidates)
+template <int SLOTS, bool SELF = false>
 __device__ RSB_STAGE_B_INLINE int stage_b_narrow_phase(const TerrainDesc& ter, const TerrainDesc& ter_s, const uint32_t* blob_s, const float* s_pose, float* s_ct, float* s_list,
                                                  int env, int lane, int nbp, unsigned* prof) {
   const BlobHeader& H = *reinterpret_cast<const BlobHeader*>(blob_s);
@@ -506,6 +588,40 @@ __device__ RSB_STAGE_B_INLINE int stage_b_narrow_phase(const TerrainDesc& ter, c
       }
     }
   }
+  if constexpr (SELF) {
+    // self-collision pairs (with or without terrain): lane = pair j, candidate index npts + j, pair index -1 - second body.  Cull on the
+    // bounding spheres of the two shapes; a warp without survivors skips the narrow phase.
+    if (H.npairs > 0) {
+      const float* pr = reinterpret_cast<const float*>(blob_s + H.off_pair) + PAIR_WORDS * min(lane, H.npairs - 1);
+      const int* pri = reinterpret_cast<const int*>(pr);
+      bool alive = false;
+      if (lane < H.npairs) {
+        const int bA = pri[PR_BA], bB = pri[PR_BB];
+        float RA[9], RB[9];
+#pragma unroll
+        for (int q = 0; q < 9; q++) { RA[q] = s_pose[(PF_R + q) * nbp + bA]; RB[q] = s_pose[(PF_R + q) * nbp + bB]; }
+        const f3 cA = mk(s_pose[(PF_P + 0) * nbp + bA], s_pose[(PF_P + 1) * nbp + bA], s_pose[(PF_P + 2) * nbp + bA]) +
+                      mulR(RA, 0.5f * (mk(pr[PR_A0], pr[PR_A0 + 1], pr[PR_A0 + 2]) + mk(pr[PR_A1], pr[PR_A1 + 1], pr[PR_A1 + 2])));
+        const f3 lB = pri[PR_KIND] == 0 ? 0.5f * (mk(pr[PR_B0], pr[PR_B0 + 1], pr[PR_B0 + 2]) + mk(pr[PR_B1], pr[PR_B1 + 1], pr[PR_B1 + 2]))
+                                        : mk(pr[PR_B0], pr[PR_B0 + 1], pr[PR_B0 + 2]);
+        const f3 cB = mk(s_pose[(PF_P + 0) * nbp + bB], s_pose[(PF_P + 1) * nbp + bB], s_pose[(PF_P + 2) * nbp + bB]) + mulR(RB, lB);
+        const f3 dc = cA - cB;
+        const float rr = pr[PR_CULL_A] + pr[PR_CULL_B];
+        alive = dot(dc, dc) <= rr * rr;
+      }
+      if (__any_sync(FULL, alive)) {
+        float depth = 0.f; f3 n = mk(0.f, 0.f, 1.f), pos = mk(0.f, 0.f, 0.f);
+        const bool hit = alive && self_pair_contact(pr, s_pose, nbp, depth, n, pos);
+        const unsigned hmask = __ballot_sync(FULL, hit);
+        if (hit) {
+          float* e = s_list + HL_WORDS * (cnt + __popc(hmask & lt));
+          e[0] = depth; e[1] = n.x; e[2] = n.y; e[3] = n.z; e[4] = pos.x; e[5] = pos.y; e[6] = pos.z;
+          e[7] = __int_as_float(-1 - pri[PR_BODY2]); e[8] = __int_as_float(H.npts + lane);
+        }
+        cnt += __popc(hmask);
+      }
+    }
+  }
   __syncwarp();
   if (prof && lane == 0) { prof[6] = (unsigned)clock64(); prof[7] = (unsigned)cnt; }
   int total = cnt;
@@ -550,10 +666,54 @@ __device__ RSB_STAGE_B_INLINE int stage_b_narrow_phase(const TerrainDesc& ter, c
       ct[CF_T1] = t1.x; ct[CF_T1 + 1] = t1.y; ct[CF_T1 + 2] = t1.z;
       ct[CF_T2] = t2.x; ct[CF_T2 + 1] = t2.y; ct[CF_T2 + 2] = t2.z;
       ct[CF_DEPTH] = depth;
-      ct[CF_PT] = __int_as_float(cand); ct[CF_BODY] = __int_as_float(ptsi[cand]); ct[CF_PAIR] = le[7];
+      if constexpr (SELF) {   // a self contact's body is the first body of its pair
+        const int body = cand < H.npts ? ptsi[cand] : reinterpret_cast<const int*>(blob_s + H.off_pair)[PAIR_WORDS * (cand - H.npts) + PR_BODY1];
+        ct[CF_PT] = __int_as_float(cand); ct[CF_BODY] = __int_as_float(body); ct[CF_PAIR] = le[7];
+      } else {
+        ct[CF_PT] = __int_as_float(cand); ct[CF_BODY] = __int_as_float(ptsi[cand]); ct[CF_PAIR] = le[7];
+      }
     }
   }
   return total;
+}
+
+// Stage C, generic instance: the second half of a self contact's column (row c) -- the ordinary compact-by-depth column Y = L^-T J^T of
+// the point pos on the chain of dof i0 (the pair's second body; -1 = welded to the world: a zero column), base columns included -- into
+// Y2; jv = J v and yz = Y . z of that half.  The same arithmetic as the first half in the kernel.
+__device__ __forceinline__ void self_second_column(float* Y2, int c, f3 pos, f3 axd, f3 O, int i0, int floating, int nbase, int nvp, int DLP, int nbp,
+                                                   const int* ddepth, const int* danc, const int* dbody, const int* bodyi, const float* s_pose,
+                                                   const float* s_gv, const float* s_L, const float* s_invd, const float* s_z, float& jv, float& yz) {
+  jv = 0.f; yz = 0.f;
+  const int m = i0 >= 0 ? ddepth[i0] : -1;
+  if (m < 0) return;
+  if (floating) {
+    const f3 rc = cross(pos - O, axd);
+    Y2[0 * CP + c] = axd.x; Y2[1 * CP + c] = axd.y; Y2[2 * CP + c] = axd.z;
+    Y2[3 * CP + c] = rc.x; Y2[4 * CP + c] = rc.y; Y2[5 * CP + c] = rc.z;
+    jv = axd.x * s_gv[0] + axd.y * s_gv[1] + axd.z * s_gv[2] + rc.x * s_gv[3] + rc.y * s_gv[4] + rc.z * s_gv[5];
+  }
+#pragma unroll 1
+  for (int t = nbase; t <= m; t++) {
+    const int a_t = danc[t * nvp + i0], j = dbody[a_t];
+    const f3 aj = mk(s_pose[(PF_A + 0) * nbp + j], s_pose[(PF_A + 1) * nbp + j], s_pose[(PF_A + 2) * nbp + j]);
+    f3 col = aj;
+    if (bodyi[BF_JTYPE * nbp + j] == 1) {
+      const f3 pj = mk(s_pose[(PF_P + 0) * nbp + j], s_pose[(PF_P + 1) * nbp + j], s_pose[(PF_P + 2) * nbp + j]);
+      col = cross(aj, pos - pj);
+    }
+    const float val = dot(col, axd);
+    Y2[t * CP + c] = val;
+    jv += val * s_gv[a_t];
+  }
+#pragma unroll 1
+  for (int sI = m; sI >= 0; sI--) {
+    const int a_s = danc[sI * nvp + i0];
+    const float y = Y2[sI * CP + c] * s_invd[a_s];
+    Y2[sI * CP + c] = y;
+    yz += y * s_z[a_s];
+#pragma unroll 1
+    for (int t = 0; t < sI; t++) Y2[t * CP + c] -= s_L[a_s * DLP + t] * y;
+  }
 }
 
 // ------------------------------------------------------------------ the kernel -----------------
@@ -913,7 +1073,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       if (args.phase_mask & 4) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // kinematics for the getters only
 
       // =========================== stage B: narrow phase ========================================
-      K = stage_b_narrow_phase<SLOTS>(args.ter, s_ter, blob_s, s_pose, s_ct, s_Y, env, lane, nbp, args.prof ? args.prof + ((size_t)env * 4 + (sub & 3)) * 8 : nullptr);
+      K = stage_b_narrow_phase<SLOTS, !ST>(args.ter, s_ter, blob_s, s_pose, s_ct, s_Y, env, lane, nbp, args.prof ? args.prof + ((size_t)env * 4 + (sub & 3)) * 8 : nullptr);
       const int C = 3 * K;
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 2] = (unsigned)clock64();
       if (args.phase_mask & 1) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // integrate1(): kinematics, collision, M, h only
@@ -1232,6 +1392,18 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
             }
           }
           u_c = jv + args.prm.dt * yz;
+          if constexpr (!ST) {
+            // self contact: the column is Y_first - Y_second; the second half (the second body's chain column at the same point, base
+            // columns included) goes to its own block s_Y2, and u_c, the relative velocity jv, are differences of the two halves
+            const int pair = __float_as_int(ct[CF_PAIR]);
+            if (!is_lim && pair < 0) {
+              float* s_Y2 = ws + args.ws.words - self_y_words(maxdd);
+              float jv2 = 0.f, yz2 = 0.f;
+              self_second_column(s_Y2, c, pos, axd, O, bdof[-1 - pair], floating, nbase, nvp, DLP, nbp, ddepth, danc, dbody, bodyi, s_pose, s_gv, s_L, s_invd, s_z, jv2, yz2);
+              u_c -= jv2 + args.prm.dt * yz2;
+              jv -= jv2;
+            }
+          }
           if (is_lim) u_c -= args.prm.erp * lm[2] / args.prm.dt;
           else if (d == 2) {
             float target = args.prm.erp * ct[CF_DEPTH] / args.prm.dt;
@@ -1279,6 +1451,26 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
                 float sacc = 0.f;
   #pragma unroll (UNR)
                 for (int t = 0; t <= tmax; t++) sacc += s_Y[t * CP + a] * s_Y[t * CP + bcol];
+                if constexpr (!ST) {
+                  // self contacts: G_ab = (Y1_a - Y2_a) . (Y1_b - Y2_b), each product along the two chains' common part (lcad)
+                  if (H.npairs > 0) {
+                    const float* s_Y2 = ws + args.ws.words - self_y_words(maxdd);
+                    const int pa = a < C3 ? __float_as_int(s_ct[(a / 3) * CT_WORDS + CF_PAIR]) : 0;
+                    const int pb = bcol < C3 ? __float_as_int(s_ct[(bcol / 3) * CT_WORDS + CF_PAIR]) : 0;
+                    if (pa < 0) {
+                      const int t2 = lcad[(-1 - pa) * nbp + bbody];
+                      for (int t = 0; t <= t2; t++) sacc -= s_Y2[t * CP + a] * s_Y[t * CP + bcol];
+                    }
+                    if (pb < 0) {
+                      const int t2 = lcad[ba * nbp + (-1 - pb)];
+                      for (int t = 0; t <= t2; t++) sacc -= s_Y[t * CP + a] * s_Y2[t * CP + bcol];
+                    }
+                    if (pa < 0 && pb < 0) {
+                      const int t2 = lcad[(-1 - pa) * nbp + (-1 - pb)];
+                      for (int t = 0; t <= t2; t++) sacc += s_Y2[t * CP + a] * s_Y2[t * CP + bcol];
+                    }
+                  }
+                }
                 s_G[a * GP + bcol] = sacc; s_G[bcol * GP + a] = sacc;
               }
             }
@@ -1294,7 +1486,13 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           float c11 = a * f - cc * cc, c12 = bq * cc - a * e, c22 = a * d - bq * bq;
           float id = 1.0f / (a * c00 + bq * c01 + cc * c02);
           float* o = s_u + CB_WORDS * lane;
-          const float pm = ptsf[5 * H.nptp + __float_as_int(s_ct[lane * CT_WORDS + CF_PT])];
+          float pm;
+          if constexpr (!ST) {   // a self contact (candidate npts + j) takes the friction of its pair
+            const int cand = __float_as_int(s_ct[lane * CT_WORDS + CF_PT]);
+            pm = cand < H.npts ? ptsf[5 * H.nptp + cand] : reinterpret_cast<const float*>(blob_s + H.off_pair)[PAIR_WORDS * (cand - H.npts) + PR_MU];
+          } else {
+            pm = ptsf[5 * H.nptp + __float_as_int(s_ct[lane * CT_WORDS + CF_PT])];
+          }
           o[0] = a; o[1] = bq; o[2] = cc; o[3] = d; o[4] = e; o[5] = f;
           o[6] = pm >= 0.f ? pm : args.prm.mu;     // per-collision-body friction (World::setMaterialPairProp analogue)
           o[8] = c00 * id; o[9] = c01 * id; o[10] = c02 * id; o[11] = c11 * id; o[12] = c12 * id; o[13] = c22 * id;
@@ -1358,6 +1556,19 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
             const int i0 = bdof[__float_as_int(s_ct[k * CT_WORDS + CF_BODY])];
             if (i0 >= 0 && ddepth[i0] >= di && danc[di * nvp + i0] == i)
               sacc += s_Y[di * CP + 3 * k] * s_lam[3 * k] + s_Y[di * CP + 3 * k + 1] * s_lam[3 * k + 1] + s_Y[di * CP + 3 * k + 2] * s_lam[3 * k + 2];
+          }
+          if constexpr (!ST) {
+            // self contacts: the second body's half of the column with -lambda
+            if (H.npairs > 0) {
+              const float* s_Y2 = ws + args.ws.words - self_y_words(maxdd);
+  #pragma unroll 1
+              for (int k = 0; k < K; k++) {
+                const int pr = __float_as_int(s_ct[k * CT_WORDS + CF_PAIR]);
+                const int i2 = pr < 0 ? bdof[-1 - pr] : -1;
+                if (i2 >= 0 && ddepth[i2] >= di && danc[di * nvp + i2] == i)
+                  sacc -= s_Y2[di * CP + 3 * k] * s_lam[3 * k] + s_Y2[di * CP + 3 * k + 1] * s_lam[3 * k + 1] + s_Y2[di * CP + 3 * k + 2] * s_lam[3 * k + 2];
+              }
+            }
           }
   #pragma unroll 1
           for (int l = 0; l < Lm; l++) {
