@@ -50,6 +50,7 @@ struct rsb_batch {
   unsigned* peer_done = nullptr;          // device counter of finished CTAs (in-kernel arrival wait)
   bool kin_dirty = true;             // the getters' buffers (M, h, poses) do not describe the current state
   unsigned* prof = nullptr;          // rsb_internal_set_profile
+  unsigned* prof_a = nullptr;        // rsb_internal_set_profile_stage_a
   int* hmap_index = nullptr;         // terrain atlas: map index per environment
   float* ext = nullptr;              // [N][EXT_WORDS] external wrench rows; ext_active: rows hold a wrench for the next launch
   bool ext_active = false;
@@ -336,7 +337,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   a.tau_applied = b->tau_applied;
   a.ncontacts = b->ncontacts; a.contacts = b->contacts; a.contact_pt = b->contact_pt; a.iters = b->iters; a.diverged = b->diverged; a.resid = b->resid; a.solver_status = b->solver_status;
   if (debug) { a.dbg_M = b->dbg_M; a.dbg_h = b->dbg_h; a.dbg_R = b->dbg_R; a.dbg_p = b->dbg_p; }
-  a.phase_mask = phase_mask; a.prof = b->prof;
+  a.phase_mask = phase_mask; a.prof = b->prof; a.prof_a = b->prof_a;
   a.ext = b->ext_active ? b->ext : nullptr;
   a.obs = obs_dev; a.ob_dim = rsb_batch_ob_dim(b);
   if (gym) {       // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
@@ -352,6 +353,8 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   if (phase_mask == 0) {   // every round of warps re-aligns at each sub-step (the kernel counts the warps of the round)
     const char* e = getenv("RSB_SUBSTEP_BARRIER");
     a.substep_barrier = e ? atoi(e) : 1;
+    const char* p = getenv("RSB_PAIR_STAGE_A");   // quadruped instance: one warp runs stage A of two environments (0 = off, for A/B runs)
+    a.pair_stage_a = p ? atoi(p) : 1;
   }
   cudaError_t e;
   switch (b->wpc) {
@@ -1178,6 +1181,8 @@ int rsb_internal_batch_info(rsb_batch* b, int* device, void** stream, int* num_e
 }
 // profiling hook (tools/balance_probe.py): device buffer [num_envs][4][8] of SM-clock stamps, or null to switch off
 int rsb_internal_set_profile(rsb_batch* b, unsigned* dev) { if (!b) return -1; b->prof = dev; return 0; }
+// profiling hook (tools/stage_probe.py): device buffer [num_envs][4][4] of SM-clock stamps inside stage A, or null to switch off
+int rsb_internal_set_profile_stage_a(rsb_batch* b, unsigned* dev) { if (!b) return -1; b->prof_a = dev; return 0; }
 // launch shape of the step kernel (tools/stage_probe.py, tests): warps per CTA and CTAs; environment e runs in round
 // e / (wpc * grid) on CTA (e % (wpc * grid)) / wpc.  RSB_FORCE_WPC is dropped without a message when the CTA does not fit in shared
 // memory, so a caller that forces a configuration reads back what it got here.

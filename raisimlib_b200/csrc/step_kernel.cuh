@@ -216,6 +216,8 @@ struct StepArgs {
   int ob_dim;
   const float* ext;    // optional [num_envs][EXT_WORDS] external wrench rows (body, F world, T world, point in body frame); null = none
   unsigned* prof;      // optional [num_envs][4 sub-steps][8] SM-clock stamps at the stage boundaries (tools/balance_probe.py)
+  unsigned* prof_a;    // optional [num_envs][4 sub-steps][4] SM-clock stamps inside stage A: after the FK walk, the per-body terms, the
+                       // subtree sums, the M columns (tools/stage_probe.py)
   // fused observation all-gather (SURVEY 8e): every rank's kernel stores its observation rows straight into every peer's
   // [world * num_envs][ob_dim] buffer over NVLink (peer memory mapped into this process), then signals one counter per peer
   float* peer_obs[MAX_PEERS];      // peer p's gathered-rows buffer of this step (null = not in use)
@@ -233,6 +235,7 @@ struct StepArgs {
   int phase_mask;      // bit0: stop after stage B (integrate1: no state update); bit2: kinematics only (stage A + getters' buffers,
                        // the contact records of the last integrate() stay as they are)
   int substep_barrier; // 1: re-align the CTA's warps of one round at every sub-step (2, 3: also before stages C, E)
+  int pair_stage_a;    // 1: quadruped instance, CTAs that keep the sub-step barrier: one warp runs stage A of two environments
 };
 
 // ------------------------------------------------------------------ small device math ----------
@@ -874,6 +877,17 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       }
     }
     __syncwarp();
+    // Paired stage A (quadruped instance): stage A uses 13 of 32 lanes and the sub-step barrier releases the warps of a round into it
+    // together, so warps w and w ^ 4 (the same scheduler when warps map to schedulers by w % 4) share one instruction stream there:
+    // the leader w runs its own environment on lanes 0-15 and the partner's on lanes 16-31, reading and writing the partner's
+    // workspace, while the partner waits on their named barrier (2-13), then runs stages B-E itself.  Only where the CTA keeps the
+    // sub-step barrier: its bar.sync orders the partner's previous sub-step (and row load) before the leader's reads.  pair_a: 1 leader
+    // with a partner, -1 partner, 0 alone (other instances; a leader whose partner has no environment in this round).
+    int pair_a = 0;
+    if constexpr (QUAD) {
+      if (args.pair_stage_a && args.substep_barrier >= 1 && s_work[0] <= 2 * s_work[1])
+        pair_a = (warp & 4) ? -1 : (warp + 4 < min(WPC, args.num_envs - (env - warp)) ? 1 : 0);
+    }
     int K = 0, iters = 0;
     float resid = 0.f; int gs_status = RSB_SOLVER_CONVERGED;
 
@@ -884,189 +898,211 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       SUBSTEP_BARRIER(1);
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 0] = (unsigned)clock64();
       // =========================== stage A: FK + RNEA + CRBA =====================================
-      float R[9]; f3 p, w, v, wd, vd, ax;
-      if (floating) {
-        float qw = s_gc[3], qx = s_gc[4], qy = s_gc[5], qz = s_gc[6];
-        float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
-        qw *= inv; qx *= inv; qy *= inv; qz *= inv;
-        R[0] = 1.f - 2.f * (qy * qy + qz * qz); R[1] = 2.f * (qx * qy - qw * qz); R[2] = 2.f * (qx * qz + qw * qy);
-        R[3] = 2.f * (qx * qy + qw * qz); R[4] = 1.f - 2.f * (qx * qx + qz * qz); R[5] = 2.f * (qy * qz - qw * qx);
-        R[6] = 2.f * (qx * qz - qw * qy); R[7] = 2.f * (qy * qz + qw * qx); R[8] = 1.f - 2.f * (qx * qx + qy * qy);
-        p = mk(s_gc[0], s_gc[1], s_gc[2]);
-        v = mk(s_gv[0], s_gv[1], s_gv[2]); w = mk(s_gv[3], s_gv[4], s_gv[5]);
-      } else {
+      f3 O;                                  // base origin: centre of the world-aligned CRBA frame (stages A and C)
+      if (pair_a >= 0) {
+        // the environment this lane computes (pair_a: lanes 16-31 of a leader take the partner's) and its workspace, a_*; with 16 lanes
+        // per environment the quadruped's body is lane & 15, the upper lanes of a warp that runs alone hold no body
+        const bool up = QUAD && lane >= 16 && pair_a > 0;
+        const int envA = up ? env + 4 : env;
+        float* const wsA = up ? ws + 4 * LS.words : ws;
+        const float* const a_gc = wsA + (s_gc - ws); const float* const a_gv = wsA + (s_gv - ws);
+        float* const a_L = wsA + (s_L - ws); float* const a_h = wsA + (s_h - ws); float* const a_pose = wsA + (s_pose - ws);
+        const int b = QUAD ? (lane & 15) : lane;
+        const bool bvalid = b < nb && (!QUAD || lane < 16 || pair_a > 0);
+        const int bb = bvalid ? b : 0;
+        unsigned* const prof_a = (QUAD && args.prof_a && bvalid && b == 0) ? args.prof_a + ((size_t)envA * 4 + (sub & 3)) * 4 : nullptr;   // quadruped only
+        float R[9]; f3 p, w, v, wd, vd, ax;
+        if (floating) {
+          float qw = a_gc[3], qx = a_gc[4], qy = a_gc[5], qz = a_gc[6];
+          float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
+          qw *= inv; qx *= inv; qy *= inv; qz *= inv;
+          R[0] = 1.f - 2.f * (qy * qy + qz * qz); R[1] = 2.f * (qx * qy - qw * qz); R[2] = 2.f * (qx * qz + qw * qy);
+          R[3] = 2.f * (qx * qy + qw * qz); R[4] = 1.f - 2.f * (qx * qx + qz * qz); R[5] = 2.f * (qy * qz - qw * qx);
+          R[6] = 2.f * (qx * qz - qw * qy); R[7] = 2.f * (qy * qz + qw * qx); R[8] = 1.f - 2.f * (qx * qx + qy * qy);
+          p = mk(a_gc[0], a_gc[1], a_gc[2]);
+          v = mk(a_gv[0], a_gv[1], a_gv[2]); w = mk(a_gv[3], a_gv[4], a_gv[5]);
+        } else {
 #pragma unroll
-        for (int k = 0; k < 9; k++) R[k] = bodyf[(BF_JROT + k) * nbp];
-        p = mk(bodyf[(BF_JPOS + 0) * nbp], bodyf[(BF_JPOS + 1) * nbp], bodyf[(BF_JPOS + 2) * nbp]);
-        v = mk(0.f, 0.f, 0.f); w = mk(0.f, 0.f, 0.f);
-      }
-      const f3 O = p;                      // base origin: centre of the world-aligned CRBA frame
-      const bool jrot_identity = (H.flags & 1) != 0;
-      wd = mk(0.f, 0.f, 0.f); vd = mk(-args.prm.gravity[0], -args.prm.gravity[1], -args.prm.gravity[2]); ax = mk(0.f, 0.f, 0.f);
+          for (int k = 0; k < 9; k++) R[k] = bodyf[(BF_JROT + k) * nbp];
+          p = mk(bodyf[(BF_JPOS + 0) * nbp], bodyf[(BF_JPOS + 1) * nbp], bodyf[(BF_JPOS + 2) * nbp]);
+          v = mk(0.f, 0.f, 0.f); w = mk(0.f, 0.f, 0.f);
+        }
+        O = p;
+        const bool jrot_identity = (H.flags & 1) != 0;
+        wd = mk(0.f, 0.f, 0.f); vd = mk(-args.prm.gravity[0], -args.prm.gravity[1], -args.prm.gravity[2]); ax = mk(0.f, 0.f, 0.f);
 #pragma unroll 1
-      for (int d = 1; d <= maxdepth; d++) {
-        int j = (bvalid && d <= MYB(BF_DEPTH)) ? anc[(d - 1) * nbp + b] : -1;
-        if (j >= 0) {
-          f3 jp = mk(bodyf[(BF_JPOS + 0) * nbp + j], bodyf[(BF_JPOS + 1) * nbp + j], bodyf[(BF_JPOS + 2) * nbp + j]);
-          float Rj[9];
-          f3 al = mk(bodyf[(BF_AXIS + 0) * nbp + j], bodyf[(BF_AXIS + 1) * nbp + j], bodyf[(BF_AXIS + 2) * nbp + j]);
-          f3 r = mulR(R, jp);
-          if (jrot_identity) {
+        for (int d = 1; d <= maxdepth; d++) {
+          int j = (bvalid && d <= MYB(BF_DEPTH)) ? anc[(d - 1) * nbp + b] : -1;
+          if (j >= 0) {
+            f3 jp = mk(bodyf[(BF_JPOS + 0) * nbp + j], bodyf[(BF_JPOS + 1) * nbp + j], bodyf[(BF_JPOS + 2) * nbp + j]);
+            float Rj[9];
+            f3 al = mk(bodyf[(BF_AXIS + 0) * nbp + j], bodyf[(BF_AXIS + 1) * nbp + j], bodyf[(BF_AXIS + 2) * nbp + j]);
+            f3 r = mulR(R, jp);
+            if (jrot_identity) {
 #pragma unroll
-            for (int k = 0; k < 9; k++) Rj[k] = R[k];
-          } else {
-            float Jr[9];      // scoped here: declared outside the branch it was a maybe-uninitialised value carried (through the stack) round the loop
+              for (int k = 0; k < 9; k++) Rj[k] = R[k];
+            } else {
+              float Jr[9];      // scoped here: declared outside the branch it was a maybe-uninitialised value carried (through the stack) round the loop
 #pragma unroll
-            for (int k = 0; k < 9; k++) Jr[k] = bodyf[(BF_JROT + k) * nbp + j];
-            matmul3(R, Jr, Rj);
-          }
-          f3 aj = mulR(Rj, al);
-          float q = s_gc[bodyi[BF_QIDX * nbp + j]], qd = s_gv[bodyi[BF_VIDX * nbp + j]];
-          const bool rev = bodyi[BF_JTYPE * nbp + j] == 1;
-          if (!rev) r = r + q * aj;
-          f3 wxr = cross(w, r);
-          f3 vn = v + wxr;
-          f3 vdn = vd + cross(wd, r) + cross(w, wxr);
-          f3 qa = qd * aj;
-          if (rev) {
-            float sq, cq;
-            sincosf(q, &sq, &cq);
-            float t = 1.f - cq;
-            float Rq[9] = {t * al.x * al.x + cq, t * al.x * al.y - sq * al.z, t * al.x * al.z + sq * al.y,
-                           t * al.x * al.y + sq * al.z, t * al.y * al.y + cq, t * al.y * al.z - sq * al.x,
-                           t * al.x * al.z - sq * al.y, t * al.y * al.z + sq * al.x, t * al.z * al.z + cq};
-            matmul3(Rj, Rq, R);
-            wd = wd + cross(w, qa);
-            w = w + qa;
-          } else {
+              for (int k = 0; k < 9; k++) Jr[k] = bodyf[(BF_JROT + k) * nbp + j];
+              matmul3(R, Jr, Rj);
+            }
+            f3 aj = mulR(Rj, al);
+            float q = a_gc[bodyi[BF_QIDX * nbp + j]], qd = a_gv[bodyi[BF_VIDX * nbp + j]];
+            const bool rev = bodyi[BF_JTYPE * nbp + j] == 1;
+            if (!rev) r = r + q * aj;
+            f3 wxr = cross(w, r);
+            f3 vn = v + wxr;
+            f3 vdn = vd + cross(wd, r) + cross(w, wxr);
+            f3 qa = qd * aj;
+            if (rev) {
+              float sq, cq;
+              sincosf(q, &sq, &cq);
+              float t = 1.f - cq;
+              float Rq[9] = {t * al.x * al.x + cq, t * al.x * al.y - sq * al.z, t * al.x * al.z + sq * al.y,
+                             t * al.x * al.y + sq * al.z, t * al.y * al.y + cq, t * al.y * al.z - sq * al.x,
+                             t * al.x * al.z - sq * al.y, t * al.y * al.z + sq * al.x, t * al.z * al.z + cq};
+              matmul3(Rj, Rq, R);
+              wd = wd + cross(w, qa);
+              w = w + qa;
+            } else {
 #pragma unroll
-            for (int k = 0; k < 9; k++) R[k] = Rj[k];
-            vn = vn + qa;
-            vdn = vdn + 2.f * cross(w, qa);
-          }
-          p = p + r; v = vn; vd = vdn; ax = aj;
-        }
-      }
-      // publish poses for stages B and C
-      if (bvalid) {
-#pragma unroll
-        for (int k = 0; k < 9; k++) s_pose[(PF_R + k) * nbp + b] = R[k];
-        s_pose[(PF_P + 0) * nbp + b] = p.x; s_pose[(PF_P + 1) * nbp + b] = p.y; s_pose[(PF_P + 2) * nbp + b] = p.z;
-        s_pose[(PF_A + 0) * nbp + b] = ax.x; s_pose[(PF_A + 1) * nbp + b] = ax.y; s_pose[(PF_A + 2) * nbp + b] = ax.z;
-      }
-      // per-body force and inertia terms about O
-      float X[16];   // F(3) N_O(3) m h(3) I_O(6)
-      {
-        float m = bvalid ? bodyf[BF_MASS * nbp + bb] : 0.f;
-        f3 cl = mk(bodyf[(BF_COM + 0) * nbp + bb], bodyf[(BF_COM + 1) * nbp + bb], bodyf[(BF_COM + 2) * nbp + bb]);
-        f3 c = mulR(R, cl);
-        f3 cO = (p - O) + c;
-        f3 ac = vd + cross(wd, c) + cross(w, cross(w, c));
-        f3 f = m * ac;
-        float I0 = bodyf[(BF_INERTIA + 0) * nbp + bb], I1 = bodyf[(BF_INERTIA + 1) * nbp + bb], I2 = bodyf[(BF_INERTIA + 2) * nbp + bb];
-        float I3 = bodyf[(BF_INERTIA + 3) * nbp + bb], I4 = bodyf[(BF_INERTIA + 4) * nbp + bb], I5 = bodyf[(BF_INERTIA + 5) * nbp + bb];
-        if (!bvalid) { I0 = I1 = I2 = I3 = I4 = I5 = 0.f; }
-        // Iw = R I R^T
-        float RI[9];
-#pragma unroll
-        for (int r = 0; r < 3; r++) {
-          RI[3 * r + 0] = R[3 * r] * I0 + R[3 * r + 1] * I1 + R[3 * r + 2] * I2;
-          RI[3 * r + 1] = R[3 * r] * I1 + R[3 * r + 1] * I3 + R[3 * r + 2] * I4;
-          RI[3 * r + 2] = R[3 * r] * I2 + R[3 * r + 1] * I4 + R[3 * r + 2] * I5;
-        }
-        float W0 = RI[0] * R[0] + RI[1] * R[1] + RI[2] * R[2], W1 = RI[0] * R[3] + RI[1] * R[4] + RI[2] * R[5], W2 = RI[0] * R[6] + RI[1] * R[7] + RI[2] * R[8];
-        float W3 = RI[3] * R[3] + RI[4] * R[4] + RI[5] * R[5], W4 = RI[3] * R[6] + RI[4] * R[7] + RI[5] * R[8], W5 = RI[6] * R[6] + RI[7] * R[7] + RI[8] * R[8];
-        f3 Iw = mk(W0 * w.x + W1 * w.y + W2 * w.z, W1 * w.x + W3 * w.y + W4 * w.z, W2 * w.x + W4 * w.y + W5 * w.z);
-        f3 Iwd = mk(W0 * wd.x + W1 * wd.y + W2 * wd.z, W1 * wd.x + W3 * wd.y + W4 * wd.z, W2 * wd.x + W4 * wd.y + W5 * wd.z);
-        f3 n = Iwd + cross(w, Iw) + cross(cO, f);
-        float cc = dot(cO, cO);
-        X[0] = f.x; X[1] = f.y; X[2] = f.z; X[3] = n.x; X[4] = n.y; X[5] = n.z;
-        X[6] = m; X[7] = m * cO.x; X[8] = m * cO.y; X[9] = m * cO.z;
-        X[10] = W0 + m * (cc - cO.x * cO.x); X[11] = W1 - m * cO.x * cO.y; X[12] = W2 - m * cO.x * cO.z;
-        X[13] = W3 + m * (cc - cO.y * cO.y); X[14] = W4 - m * cO.y * cO.z; X[15] = W5 + m * (cc - cO.z * cO.z);
-      }
-      if (args.ext) {   // ArticulatedSystem::setExternalForce / setExternalTorque: h -= J^T wrench, through the RNEA force terms
-        const float* e = args.ext + (size_t)env * EXT_WORDS;
-        if (bvalid && __float_as_int(e[0]) == b) {
-          const f3 Fe = mk(e[1], e[2], e[3]), Te = mk(e[4], e[5], e[6]);
-          const f3 re = (p - O) + mulR(R, mk(e[7], e[8], e[9]));
-          const f3 Me = cross(re, Fe) + Te;
-          X[0] -= Fe.x; X[1] -= Fe.y; X[2] -= Fe.z; X[3] -= Me.x; X[4] -= Me.y; X[5] -= Me.z;
-        }
-      }
-      // subtree sums: bodies are in DFS pre-order, so subtree(b) = lanes [b, b + size)
-      float A[16];
-#pragma unroll
-      for (int k = 0; k < 16; k++) A[k] = X[k];
-      const int my_sub = MYB(BF_SUBTREE);
-      const int max_inner = (H.flags >> 8) & 0xff;   // largest non-root subtree size - 1
-#pragma unroll 1
-      for (int s = 1; s <= max_inner; s++) {
-        bool take = (b > 0) && (s < my_sub);
-#pragma unroll
-        for (int k = 0; k < 16; k++) {
-          float x = __shfl_down_sync(FULL, X[k], s);
-          if (take) A[k] += x;
-        }
-      }
-      {   // root: everything
-        float T[16];
-#pragma unroll
-        for (int k = 0; k < 16; k++) {
-          float t = X[k];
-          // lanes >= nb hold exact zeros (zero mass and inertia): with at most 16 bodies the xor-16 step adds 0 and is skipped
-#pragma unroll
-          for (int o = (ST && SNB <= 16) ? 8 : 16; o > 0; o >>= 1) t += __shfl_xor_sync(FULL, t, o);
-          T[k] = t;
-        }
-        if (b == 0) {
-#pragma unroll
-          for (int k = 0; k < 16; k++) A[k] = T[k];
-        }
-      }
-      // bias force h and CRBA columns (row i of M stored compactly: column index = ancestor depth)
-      f3 rO = p - O;
-      const bool rev = MYB(BF_JTYPE) == 1;
-      f3 Sw = rev ? ax : mk(0.f, 0.f, 0.f);
-      f3 Sv = rev ? cross(rO, ax) : ax;
-      f3 Fc = mk(A[0], A[1], A[2]), Nc = mk(A[3], A[4], A[5]);
-      f3 hh = mk(A[7], A[8], A[9]);
-      f3 ff = A[6] * Sv + cross(Sw, hh);
-      f3 nn = mk(A[10] * Sw.x + A[11] * Sw.y + A[12] * Sw.z, A[11] * Sw.x + A[13] * Sw.y + A[14] * Sw.z, A[12] * Sw.x + A[14] * Sw.y + A[15] * Sw.z) + cross(hh, Sv);
-      const int my_vidx = MYB(BF_VIDX);
-      const int my_dd = nbase + MYB(BF_DEPTH) - 1;          // depth of this body's dof in the dof tree
-      if (bvalid && b > 0) {
-        float* row = s_L + my_vidx * DLP;
-        s_h[my_vidx] = dot(Sw, Nc) + dot(Sv, Fc);      // S^T [N_O; F]  (moment about O)
-        row[my_dd] = dot(Sw, nn) + dot(Sv, ff);
-        if (floating) { row[0] = ff.x; row[1] = ff.y; row[2] = ff.z; row[3] = nn.x; row[4] = nn.y; row[5] = nn.z; }
-      }
-      if (b == 0 && floating) {
-        s_h[0] = Fc.x; s_h[1] = Fc.y; s_h[2] = Fc.z; s_h[3] = Nc.x; s_h[4] = Nc.y; s_h[5] = Nc.z;
-        // lower triangle of [ m 1, -[h]x ; [h]x, I_O ]
-        s_L[0 * DLP + 0] = A[6]; s_L[1 * DLP + 0] = 0.f; s_L[1 * DLP + 1] = A[6];
-        s_L[2 * DLP + 0] = 0.f; s_L[2 * DLP + 1] = 0.f; s_L[2 * DLP + 2] = A[6];
-        s_L[3 * DLP + 0] = 0.f; s_L[3 * DLP + 1] = -hh.z; s_L[3 * DLP + 2] = hh.y;
-        s_L[4 * DLP + 0] = hh.z; s_L[4 * DLP + 1] = 0.f; s_L[4 * DLP + 2] = -hh.x;
-        s_L[5 * DLP + 0] = -hh.y; s_L[5 * DLP + 1] = hh.x; s_L[5 * DLP + 2] = 0.f;
-        s_L[3 * DLP + 3] = A[10]; s_L[4 * DLP + 3] = A[11]; s_L[5 * DLP + 3] = A[12];
-        s_L[4 * DLP + 4] = A[13]; s_L[5 * DLP + 4] = A[14]; s_L[5 * DLP + 5] = A[15];
-      }
-      {   // M[vi][vj] for proper ancestors j (excluding the root): column = depth of j's dof
-        int j = (bvalid && b > 0) ? MYB(BF_PARENT) : 0;
-        int tj = my_dd - 1;
-#pragma unroll 1
-        for (int d = 2; d <= maxdepth; d++) {
-          int src = j > 0 ? j : 0;
-          f3 Swj = shfl3(Sw, src), Svj = shfl3(Sv, src);
-          if (j > 0) {
-            s_L[my_vidx * DLP + tj] = dot(Swj, nn) + dot(Svj, ff);
-            j = bodyi[BF_PARENT * nbp + j];
-            tj--;
+              for (int k = 0; k < 9; k++) R[k] = Rj[k];
+              vn = vn + qa;
+              vdn = vdn + 2.f * cross(w, qa);
+            }
+            p = p + r; v = vn; vd = vdn; ax = aj;
           }
         }
+        // publish poses for stages B and C
+        if (bvalid) {
+#pragma unroll
+          for (int k = 0; k < 9; k++) a_pose[(PF_R + k) * nbp + b] = R[k];
+          a_pose[(PF_P + 0) * nbp + b] = p.x; a_pose[(PF_P + 1) * nbp + b] = p.y; a_pose[(PF_P + 2) * nbp + b] = p.z;
+          a_pose[(PF_A + 0) * nbp + b] = ax.x; a_pose[(PF_A + 1) * nbp + b] = ax.y; a_pose[(PF_A + 2) * nbp + b] = ax.z;
+        }
+        if (prof_a) prof_a[0] = (unsigned)clock64();
+        // per-body force and inertia terms about O
+        float X[16];   // F(3) N_O(3) m h(3) I_O(6)
+        {
+          float m = bvalid ? bodyf[BF_MASS * nbp + bb] : 0.f;
+          f3 cl = mk(bodyf[(BF_COM + 0) * nbp + bb], bodyf[(BF_COM + 1) * nbp + bb], bodyf[(BF_COM + 2) * nbp + bb]);
+          f3 c = mulR(R, cl);
+          f3 cO = (p - O) + c;
+          f3 ac = vd + cross(wd, c) + cross(w, cross(w, c));
+          f3 f = m * ac;
+          float I0 = bodyf[(BF_INERTIA + 0) * nbp + bb], I1 = bodyf[(BF_INERTIA + 1) * nbp + bb], I2 = bodyf[(BF_INERTIA + 2) * nbp + bb];
+          float I3 = bodyf[(BF_INERTIA + 3) * nbp + bb], I4 = bodyf[(BF_INERTIA + 4) * nbp + bb], I5 = bodyf[(BF_INERTIA + 5) * nbp + bb];
+          if (!bvalid) { I0 = I1 = I2 = I3 = I4 = I5 = 0.f; }
+          // Iw = R I R^T
+          float RI[9];
+#pragma unroll
+          for (int r = 0; r < 3; r++) {
+            RI[3 * r + 0] = R[3 * r] * I0 + R[3 * r + 1] * I1 + R[3 * r + 2] * I2;
+            RI[3 * r + 1] = R[3 * r] * I1 + R[3 * r + 1] * I3 + R[3 * r + 2] * I4;
+            RI[3 * r + 2] = R[3 * r] * I2 + R[3 * r + 1] * I4 + R[3 * r + 2] * I5;
+          }
+          float W0 = RI[0] * R[0] + RI[1] * R[1] + RI[2] * R[2], W1 = RI[0] * R[3] + RI[1] * R[4] + RI[2] * R[5], W2 = RI[0] * R[6] + RI[1] * R[7] + RI[2] * R[8];
+          float W3 = RI[3] * R[3] + RI[4] * R[4] + RI[5] * R[5], W4 = RI[3] * R[6] + RI[4] * R[7] + RI[5] * R[8], W5 = RI[6] * R[6] + RI[7] * R[7] + RI[8] * R[8];
+          f3 Iw = mk(W0 * w.x + W1 * w.y + W2 * w.z, W1 * w.x + W3 * w.y + W4 * w.z, W2 * w.x + W4 * w.y + W5 * w.z);
+          f3 Iwd = mk(W0 * wd.x + W1 * wd.y + W2 * wd.z, W1 * wd.x + W3 * wd.y + W4 * wd.z, W2 * wd.x + W4 * wd.y + W5 * wd.z);
+          f3 n = Iwd + cross(w, Iw) + cross(cO, f);
+          float cc = dot(cO, cO);
+          X[0] = f.x; X[1] = f.y; X[2] = f.z; X[3] = n.x; X[4] = n.y; X[5] = n.z;
+          X[6] = m; X[7] = m * cO.x; X[8] = m * cO.y; X[9] = m * cO.z;
+          X[10] = W0 + m * (cc - cO.x * cO.x); X[11] = W1 - m * cO.x * cO.y; X[12] = W2 - m * cO.x * cO.z;
+          X[13] = W3 + m * (cc - cO.y * cO.y); X[14] = W4 - m * cO.y * cO.z; X[15] = W5 + m * (cc - cO.z * cO.z);
+        }
+        if (args.ext) {   // ArticulatedSystem::setExternalForce / setExternalTorque: h -= J^T wrench, through the RNEA force terms
+          const float* e = args.ext + (size_t)envA * EXT_WORDS;
+          if (bvalid && __float_as_int(e[0]) == b) {
+            const f3 Fe = mk(e[1], e[2], e[3]), Te = mk(e[4], e[5], e[6]);
+            const f3 re = (p - O) + mulR(R, mk(e[7], e[8], e[9]));
+            const f3 Me = cross(re, Fe) + Te;
+            X[0] -= Fe.x; X[1] -= Fe.y; X[2] -= Fe.z; X[3] -= Me.x; X[4] -= Me.y; X[5] -= Me.z;
+          }
+        }
+        if (prof_a) prof_a[1] = (unsigned)clock64();
+        // subtree sums: bodies are in DFS pre-order, so subtree(b) = lanes [b, b + size)
+        float A[16];
+#pragma unroll
+        for (int k = 0; k < 16; k++) A[k] = X[k];
+        const int my_sub = MYB(BF_SUBTREE);
+        const int max_inner = (H.flags >> 8) & 0xff;   // largest non-root subtree size - 1
+#pragma unroll 1
+        for (int s = 1; s <= max_inner; s++) {
+          bool take = (b > 0) && (s < my_sub);
+#pragma unroll
+          for (int k = 0; k < 16; k++) {
+            float x = __shfl_down_sync(FULL, X[k], s);
+            if (take) A[k] += x;
+          }
+        }
+        {   // root: everything
+          float T[16];
+#pragma unroll
+          for (int k = 0; k < 16; k++) {
+            float t = X[k];
+            // lanes >= nb hold exact zeros (zero mass and inertia): with at most 16 bodies the xor-16 step adds 0 and is skipped
+#pragma unroll
+            for (int o = (ST && SNB <= 16) ? 8 : 16; o > 0; o >>= 1) t += __shfl_xor_sync(FULL, t, o);
+            T[k] = t;
+          }
+          if (b == 0) {
+#pragma unroll
+            for (int k = 0; k < 16; k++) A[k] = T[k];
+          }
+        }
+        if (prof_a) prof_a[2] = (unsigned)clock64();
+        // bias force h and CRBA columns (row i of M stored compactly: column index = ancestor depth)
+        f3 rO = p - O;
+        const bool rev = MYB(BF_JTYPE) == 1;
+        f3 Sw = rev ? ax : mk(0.f, 0.f, 0.f);
+        f3 Sv = rev ? cross(rO, ax) : ax;
+        f3 Fc = mk(A[0], A[1], A[2]), Nc = mk(A[3], A[4], A[5]);
+        f3 hh = mk(A[7], A[8], A[9]);
+        f3 ff = A[6] * Sv + cross(Sw, hh);
+        f3 nn = mk(A[10] * Sw.x + A[11] * Sw.y + A[12] * Sw.z, A[11] * Sw.x + A[13] * Sw.y + A[14] * Sw.z, A[12] * Sw.x + A[14] * Sw.y + A[15] * Sw.z) + cross(hh, Sv);
+        const int my_vidx = MYB(BF_VIDX);
+        const int my_dd = nbase + MYB(BF_DEPTH) - 1;          // depth of this body's dof in the dof tree
+        if (bvalid && b > 0) {
+          float* row = a_L + my_vidx * DLP;
+          a_h[my_vidx] = dot(Sw, Nc) + dot(Sv, Fc);      // S^T [N_O; F]  (moment about O)
+          row[my_dd] = dot(Sw, nn) + dot(Sv, ff);
+          if (floating) { row[0] = ff.x; row[1] = ff.y; row[2] = ff.z; row[3] = nn.x; row[4] = nn.y; row[5] = nn.z; }
+        }
+        if (bvalid && b == 0 && floating) {
+          a_h[0] = Fc.x; a_h[1] = Fc.y; a_h[2] = Fc.z; a_h[3] = Nc.x; a_h[4] = Nc.y; a_h[5] = Nc.z;
+          // lower triangle of [ m 1, -[h]x ; [h]x, I_O ]
+          a_L[0 * DLP + 0] = A[6]; a_L[1 * DLP + 0] = 0.f; a_L[1 * DLP + 1] = A[6];
+          a_L[2 * DLP + 0] = 0.f; a_L[2 * DLP + 1] = 0.f; a_L[2 * DLP + 2] = A[6];
+          a_L[3 * DLP + 0] = 0.f; a_L[3 * DLP + 1] = -hh.z; a_L[3 * DLP + 2] = hh.y;
+          a_L[4 * DLP + 0] = hh.z; a_L[4 * DLP + 1] = 0.f; a_L[4 * DLP + 2] = -hh.x;
+          a_L[5 * DLP + 0] = -hh.y; a_L[5 * DLP + 1] = hh.x; a_L[5 * DLP + 2] = 0.f;
+          a_L[3 * DLP + 3] = A[10]; a_L[4 * DLP + 3] = A[11]; a_L[5 * DLP + 3] = A[12];
+          a_L[4 * DLP + 4] = A[13]; a_L[5 * DLP + 4] = A[14]; a_L[5 * DLP + 5] = A[15];
+        }
+        {   // M[vi][vj] for proper ancestors j (excluding the root): column = depth of j's dof
+          int j = (bvalid && b > 0) ? MYB(BF_PARENT) : 0;
+          int tj = my_dd - 1;
+#pragma unroll 1
+          for (int d = 2; d <= maxdepth; d++) {
+            int src = (j > 0 ? j : 0) + (QUAD ? (lane & 16) : 0);      // the lane of body j in this lane's environment
+            f3 Swj = shfl3(Sw, src), Svj = shfl3(Sv, src);
+            if (j > 0) {
+              a_L[my_vidx * DLP + tj] = dot(Swj, nn) + dot(Svj, ff);
+              j = bodyi[BF_PARENT * nbp + j];
+              tj--;
+            }
+          }
+        }
+        __syncwarp();
+        if (prof_a) prof_a[3] = (unsigned)clock64();
       }
-      __syncwarp();
+      if constexpr (QUAD) {
+        if (pair_a != 0) asm volatile("bar.sync %0, 64;" ::"r"(2 + (warp & 3) + 4 * (warp >> 3)) : "memory");   // the pair's stage A is done
+        O = mk(s_gc[0], s_gc[1], s_gc[2]);   // this warp's own base (= p of the base lane in stage A)
+      }
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 1] = (unsigned)clock64();
       if (args.dbg_M)   // getters (integrate1): cold path, kept out of line to spare the instruction cache
         write_debug(args, env, lane, nv, nb, nvp, DLP, s_L, s_h, ddepth, danc, bvalid, s_pose, nbp);

@@ -3,7 +3,8 @@
 
 usage: stage_probe.py c3|c2|c4 [n_envs] -- prints cycles per sub-step of one environment in stages A..E (SM-clock stamps written by the
 step kernel through rsb_internal_set_profile), launch times with the sub-step barrier on / off, the sweep / contact histograms, and
-what the slowest warp of each CTA-round costs behind the sub-step barrier."""
+what the slowest warp of each CTA-round costs behind the sub-step barrier; for the quadruped instance also the split of stage A
+(RSB_PAIR_STAGE_A=0 runs it unpaired)."""
 import ctypes, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -58,14 +59,27 @@ def main():
     wpc, grid = ctypes.c_int(), ctypes.c_int()
     lib.rsb_internal_launch_config(sim.bt.h, ctypes.byref(wpc), ctypes.byref(grid))
     wpc, grid = wpc.value, grid.value
+    lib.rsb_internal_set_profile_stage_a.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     sim.bt.set_state(g, v)
     prof = torch.zeros((n, 4, 8), dtype=torch.int32, device="cuda")
+    prof_a = torch.zeros((n, 4, 4), dtype=torch.int32, device="cuda")      # quadruped instance: stamps inside stage A
     lib.rsb_internal_set_profile(sim.bt.h, ctypes.c_void_p(prof.data_ptr()))
+    lib.rsb_internal_set_profile_stage_a(sim.bt.h, ctypes.c_void_p(prof_a.data_ptr()))
     sim.step_resident(k0)
     torch.cuda.synchronize()
     lib.rsb_internal_set_profile(sim.bt.h, ctypes.c_void_p(0))
+    lib.rsb_internal_set_profile_stage_a(sim.bt.h, ctypes.c_void_p(0))
     P = prof.cpu().numpy().astype(np.int64) & 0xffffffff
     d = lambda a, b: ((P[:, :, b] - P[:, :, a]) & 0xffffffff).astype(np.float64)
+    PA = prof_a.cpu().numpy().astype(np.int64) & 0xffffffff
+    if (PA != 0).any():
+        # stage A from the environment's own start stamp: FK walk | per-body terms | subtree sums | M columns | to the end of stage A
+        # (a paired environment's last part is the wait for the pair barrier, an unpaired one's the stage-A prof stamp)
+        S = np.concatenate([P[:, :, :1], PA, P[:, :, 1:2]], axis=2)
+        parts = [((S[:, :, i + 1] - S[:, :, i]) & 0xffffffff).astype(np.float64) for i in range(5)]
+        print("  stage A split (cycles per sub-step):")
+        for name, a in zip(("FK walk", "per-body terms", "subtree sums", "M columns", "to the end"), parts):
+            print("     %-14s mean %.0f  p10 %.0f  p50 %.0f  p90 %.0f  max %.0f" % (name, a.mean(), np.quantile(a, .1), np.median(a), np.quantile(a, .9), a.max()))
     hasD = P[:, :, 3] != 0
     tA, tB = d(0, 1), d(1, 2)
     tC = np.where(hasD, d(2, 3), d(2, 4)); tD = np.where(hasD, d(3, 4), 0.0); tE = d(4, 5); tot = d(0, 5)
