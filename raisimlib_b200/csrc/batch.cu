@@ -6,7 +6,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <memory>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -351,8 +350,8 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
     a.peer_expected = b->peer_epoch * (unsigned)b->grid; a.peer_done = b->peer_done;
   }
   if (phase_mask == 0) {   // every round of warps re-aligns at each sub-step (the kernel counts the warps of the round)
-    const char* e = getenv("RSB_SUBSTEP_BARRIER");
-    a.substep_barrier = e ? atoi(e) : 1;
+    const char* e = getenv("RSB_SUBSTEP_BARRIER");   // 0 = off, for A/B runs
+    a.substep_barrier = e ? atoi(e) != 0 : 1;
     const char* p = getenv("RSB_PAIR_STAGE_A");   // quadruped instance: one warp runs stage A of two environments (0 = off, for A/B runs)
     a.pair_stage_a = p ? atoi(p) : 1;
   }
@@ -367,19 +366,42 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   }
   if (e != cudaSuccess) return fail(RSB_ERR_CUDA, std::string("step kernel launch: ") + cudaGetErrorString(e));
   b->launches++;
-  if (!(phase_mask & 1)) b->kin_dirty = !debug;   // the state advanced: M, h and poses are stale unless this launch refreshed them
+  if (!(phase_mask & PHASE_NO_UPDATE)) b->kin_dirty = !debug;   // the state advanced: M, h and poses are stale unless this launch refreshed them
   else if (debug) b->kin_dirty = false;
-  if (phase_mask == 0 || (phase_mask & 2)) b->ext_active = false;   // an external wrench lasts for one integrate() call (upstream semantics)
+  if (phase_mask == 0) b->ext_active = false;   // an external wrench lasts for one integrate() call (upstream semantics)
   return RSB_OK;
 }
 
 // rows: tight [n][w] <-> padded [n][stride].  Host buffers go through one CONTIGUOUS PCIe copy into a
 // device staging area and are (un)padded on the device: pitched H2D/D2H copies of 76-byte rows are slow.
-static int ensure_staging(rsb_batch* b, size_t words) {
-  if (b->staging_words >= words) return RSB_OK;
-  if (b->staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->staging); b->staging = nullptr; b->staging_words = 0; }
-  CK(cudaMalloc((void**)&b->staging, words * 4));
-  b->staging_words = words;
+// *slot = room for `words` in the staging area; back-to-back calls on the same stream take successive slots and stream order
+// keeps them apart
+static int staging_slot(rsb_batch* b, size_t words, float** slot) {
+  const size_t need = (size_t)b->N * 64 + 64;
+  if (b->staging_words < need) {
+    if (b->staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->staging); b->staging = nullptr; b->staging_words = 0; }
+    CK(cudaMalloc((void**)&b->staging, need * 4));
+    b->staging_words = need;
+  }
+  *slot = b->staging + b->staging_cursor;
+  b->staging_cursor = (b->staging_cursor + words + 31) / 32 * 32;
+  if (b->staging_cursor + (size_t)b->N * 40 > b->staging_words) b->staging_cursor = 0;
+  return RSB_OK;
+}
+// device -> the caller's buffer (where: RSB_HOST / RSB_DEVICE); a host destination has been written when this returns
+static int copy_out(rsb_batch* b, void* dst, const void* src, size_t bytes, int where) {
+  CK(cudaMemcpyAsync(dst, src, bytes, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
+  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
+  return RSB_OK;
+}
+// device rows of observations for a host destination
+static int ensure_obs_staging(rsb_batch* b) {
+  const size_t need = (size_t)b->N * rsb_batch_ob_dim(b);
+  if (b->obs_staging_words >= need) return RSB_OK;
+  if (b->obs_staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->obs_staging); }
+  b->obs_staging = nullptr; b->obs_staging_words = 0;
+  CK(cudaMalloc((void**)&b->obs_staging, need * 4));
+  b->obs_staging_words = need;
   return RSB_OK;
 }
 // device-side alias of a pinned, mapped host allocation (cudaHostAlloc / cudaHostRegister / torch pin_memory); null otherwise
@@ -393,11 +415,8 @@ static int copy_rows_in(rsb_batch* b, float* dst, int stride, const float* src, 
   if (!src || n == 0) return RSB_OK;
   const float* dsrc = src;
   if (where == RSB_HOST) {
-    int rc = ensure_staging(b, (size_t)b->N * 64 + 64); if (rc) return rc;
-    // the staging area is reused by back-to-back calls on the same stream: stream order keeps them apart
-    float* st = b->staging + b->staging_cursor;
-    b->staging_cursor = (b->staging_cursor + (size_t)n * w + 31) / 32 * 32;
-    if (b->staging_cursor + (size_t)b->N * 40 > b->staging_words) b->staging_cursor = 0;
+    float* st = nullptr;
+    int rc = staging_slot(b, (size_t)n * w, &st); if (rc) return rc;
     CK(cudaMemcpyAsync(st, src, (size_t)n * w * 4, cudaMemcpyHostToDevice, b->stream));
     dsrc = st;
   }
@@ -407,10 +426,8 @@ static int copy_rows_in(rsb_batch* b, float* dst, int stride, const float* src, 
 static int copy_rows_out(rsb_batch* b, float* dst, const float* src, int stride, int w, int env_begin, int n, int where) {
   if (!dst || n == 0) return RSB_OK;
   if (where == RSB_HOST) {
-    int rc = ensure_staging(b, (size_t)b->N * 64 + 64); if (rc) return rc;
-    float* st = b->staging + b->staging_cursor;
-    b->staging_cursor = (b->staging_cursor + (size_t)n * w + 31) / 32 * 32;
-    if (b->staging_cursor + (size_t)b->N * 40 > b->staging_words) b->staging_cursor = 0;
+    float* st = nullptr;
+    int rc = staging_slot(b, (size_t)n * w, &st); if (rc) return rc;
     CK(cudaMemcpy2DAsync(st, (size_t)w * 4, src + (size_t)env_begin * stride, (size_t)stride * 4, (size_t)w * 4, n, cudaMemcpyDeviceToDevice, b->stream));
     CK(cudaMemcpyAsync(dst, st, (size_t)n * w * 4, cudaMemcpyDeviceToHost, b->stream));
   } else {
@@ -439,16 +456,16 @@ int rsb_params_default(rsb_params* p) {
 }
 
 // ---- model ---------------------------------------------------------------------------------------
+// the limits of the step kernel, checked on every model that enters through the C-ABI
+static int adopt_model(Model md, rsb_model** out) {
+  if (md.nb > 32) return fail(RSB_ERR_UNSUPPORTED, "more than 32 movable bodies (one lane per body)");
+  if (md.npts() > 32 * MAX_PT_SLOTS) return fail(RSB_ERR_UNSUPPORTED, "more than 64 candidate contact points");
+  *out = new rsb_model{std::move(md)};
+  return RSB_OK;
+}
 int rsb_model_create_from_urdf(const char* path_or_xml, rsb_model** out) {
   if (!path_or_xml || !out) return fail(RSB_ERR_INVALID, "null argument");
-  try {
-    std::unique_ptr<rsb_model> m(new rsb_model);      // a parse error thrown below must not leak the half-built model
-    m->md = load_urdf(path_or_xml);
-    if (m->md.nb > 32) return fail(RSB_ERR_UNSUPPORTED, "more than 32 movable bodies (one lane per body)");
-    if (m->md.npts() > 32 * MAX_PT_SLOTS) return fail(RSB_ERR_UNSUPPORTED, "more than 64 candidate contact points");
-    *out = m.release();
-    return RSB_OK;
-  } catch (const std::exception& e) { return fail(RSB_ERR_PARSE, e.what()); }
+  try { return adopt_model(load_urdf(path_or_xml), out); } catch (const std::exception& e) { return fail(RSB_ERR_PARSE, e.what()); }
 }
 int rsb_model_save(const rsb_model* m, const char* path) {
   if (!m || !path) return fail(RSB_ERR_INVALID, "null argument");
@@ -456,14 +473,7 @@ int rsb_model_save(const rsb_model* m, const char* path) {
 }
 int rsb_model_load(const char* path, rsb_model** out) {
   if (!path || !out) return fail(RSB_ERR_INVALID, "null argument");
-  try {
-    std::unique_ptr<rsb_model> m(new rsb_model);
-    m->md = load_model(path);
-    if (m->md.nb > 32) return fail(RSB_ERR_UNSUPPORTED, "more than 32 movable bodies (one lane per body)");
-    if (m->md.npts() > 32 * MAX_PT_SLOTS) return fail(RSB_ERR_UNSUPPORTED, "more than 64 candidate contact points");
-    *out = m.release();
-    return RSB_OK;
-  } catch (const std::exception& e) { return fail(RSB_ERR_PARSE, e.what()); }
+  try { return adopt_model(load_model(path), out); } catch (const std::exception& e) { return fail(RSB_ERR_PARSE, e.what()); }
 }
 void rsb_model_destroy(rsb_model* m) { delete m; }
 int rsb_model_dims(const rsb_model* m, int* nq, int* nv, int* nb, int* ncoll, int* npts) {
@@ -602,32 +612,9 @@ int rsb_batch_clear_terrain(rsb_batch* b) {
   b->ter = TerrainDesc{};
   return RSB_OK;
 }
-int rsb_batch_set_heightmap(rsb_batch* b, int xs, int ys, float x_size, float y_size, float cx, float cy, const float* h) {
-  if (!b || !h || xs < 2 || ys < 2 || !(x_size > 0) || !(y_size > 0)) return fail(RSB_ERR_INVALID, "bad height map");
-  CK(cudaSetDevice(b->device));
-  CK(cudaStreamSynchronize(b->stream));
-  if (b->hmap) { cudaFree(b->hmap); b->hmap = nullptr; }
-  b->ter = TerrainDesc{};               // nothing may point at the freed map if an allocation below fails
-  CK(cudaMalloc((void**)&b->hmap, (size_t)xs * ys * 4));
-  CK(cudaMemcpy(b->hmap, h, (size_t)xs * ys * 4, cudaMemcpyHostToDevice));
-  TerrainDesc t{};
-  t.type = 2; t.xs = xs; t.ys = ys;
-  t.dx = x_size / (float)(xs - 1); t.dy = y_size / (float)(ys - 1); t.inv_dx = 1.0f / t.dx; t.inv_dy = 1.0f / t.dy;
-  t.x0 = cx - 0.5f * x_size; t.y0 = cy - 0.5f * y_size;
-  t.xmax = (float)(xs - 1); t.ymax = (float)(ys - 1);
-  t.h = b->hmap;
-  t.hmax = h[0];
-  for (size_t i = 1; i < (size_t)xs * ys; i++) t.hmax = std::max(t.hmax, h[i]);
-  b->ter = t;
-  return RSB_OK;
-}
-// terrain atlas (SURVEY 8f N3 "per-env distinct terrains"): `count` same-sized height maps back to back and one map
-// index per environment; every environment collides with its own map, everything else is as rsb_batch_set_heightmap
-int rsb_batch_set_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_size, float y_size, float cx, float cy, const float* h,
+// `count` same-sized height maps back to back; map_of_env: the map index of every environment (null: one map that all share)
+static int upload_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_size, float y_size, float cx, float cy, const float* h,
                              const int32_t* map_of_env) {
-  if (!b || !h || !map_of_env || count < 1 || xs < 2 || ys < 2 || !(x_size > 0) || !(y_size > 0)) return fail(RSB_ERR_INVALID, "bad height-map atlas");
-  if ((size_t)count * xs * ys > ((size_t)1 << 30)) return fail(RSB_ERR_INVALID, "height-map atlas too large");
-  for (int e = 0; e < b->N; e++) if (map_of_env[e] < 0 || map_of_env[e] >= count) return fail(RSB_ERR_INVALID, "height-map index out of range");
   CK(cudaSetDevice(b->device));
   CK(cudaStreamSynchronize(b->stream));
   if (b->hmap) { cudaFree(b->hmap); b->hmap = nullptr; }
@@ -636,8 +623,10 @@ int rsb_batch_set_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_si
   const size_t words = (size_t)count * xs * ys;
   CK(cudaMalloc((void**)&b->hmap, words * 4));
   CK(cudaMemcpy(b->hmap, h, words * 4, cudaMemcpyHostToDevice));
-  CK(cudaMalloc((void**)&b->hmap_index, (size_t)b->N * 4));
-  CK(cudaMemcpy(b->hmap_index, map_of_env, (size_t)b->N * 4, cudaMemcpyHostToDevice));
+  if (map_of_env) {
+    CK(cudaMalloc((void**)&b->hmap_index, (size_t)b->N * 4));
+    CK(cudaMemcpy(b->hmap_index, map_of_env, (size_t)b->N * 4, cudaMemcpyHostToDevice));
+  }
   TerrainDesc t{};
   t.type = 2; t.xs = xs; t.ys = ys;
   t.dx = x_size / (float)(xs - 1); t.dy = y_size / (float)(ys - 1); t.inv_dx = 1.0f / t.dx; t.inv_dy = 1.0f / t.dy;
@@ -648,6 +637,19 @@ int rsb_batch_set_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_si
   for (size_t i = 1; i < words; i++) t.hmax = std::max(t.hmax, h[i]);
   b->ter = t;
   return RSB_OK;
+}
+int rsb_batch_set_heightmap(rsb_batch* b, int xs, int ys, float x_size, float y_size, float cx, float cy, const float* h) {
+  if (!b || !h || xs < 2 || ys < 2 || !(x_size > 0) || !(y_size > 0)) return fail(RSB_ERR_INVALID, "bad height map");
+  return upload_heightmaps(b, 1, xs, ys, x_size, y_size, cx, cy, h, nullptr);
+}
+// terrain atlas (SURVEY 8f N3 "per-env distinct terrains"): `count` same-sized height maps back to back and one map
+// index per environment; every environment collides with its own map, everything else is as rsb_batch_set_heightmap
+int rsb_batch_set_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_size, float y_size, float cx, float cy, const float* h,
+                             const int32_t* map_of_env) {
+  if (!b || !h || !map_of_env || count < 1 || xs < 2 || ys < 2 || !(x_size > 0) || !(y_size > 0)) return fail(RSB_ERR_INVALID, "bad height-map atlas");
+  if ((size_t)count * xs * ys > ((size_t)1 << 30)) return fail(RSB_ERR_INVALID, "height-map atlas too large");
+  for (int e = 0; e < b->N; e++) if (map_of_env[e] < 0 || map_of_env[e] >= count) return fail(RSB_ERR_INVALID, "height-map index out of range");
+  return upload_heightmaps(b, count, xs, ys, x_size, y_size, cx, cy, h, map_of_env);
 }
 int rsb_batch_set_params(rsb_batch* b, const rsb_params* p) {
   if (!b || !p) return fail(RSB_ERR_INVALID, "null argument");
@@ -793,10 +795,8 @@ int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, co
   }
   const float *df = force, *dtq = torque;
   if (where == RSB_HOST && (force || torque)) {
-    rc = ensure_staging(b, (size_t)b->N * 64 + 64); if (rc) return rc;
-    float* st = b->staging + b->staging_cursor;
-    b->staging_cursor = (b->staging_cursor + (size_t)env_count * 6 + 31) / 32 * 32;
-    if (b->staging_cursor + (size_t)b->N * 40 > b->staging_words) b->staging_cursor = 0;
+    float* st = nullptr;
+    rc = staging_slot(b, (size_t)env_count * 6, &st); if (rc) return rc;
     if (force) { CK(cudaMemcpyAsync(st, force, (size_t)env_count * 12, cudaMemcpyHostToDevice, b->stream)); df = st; }
     if (torque) { CK(cudaMemcpyAsync(st + (size_t)env_count * 3, torque, (size_t)env_count * 12, cudaMemcpyHostToDevice, b->stream)); dtq = st + (size_t)env_count * 3; }
   }
@@ -826,13 +826,13 @@ int rsb_batch_integrate1(rsb_batch* b) {
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
   CK(cudaSetDevice(b->device));
   int rc = ensure_debug(b); if (rc) return rc;
-  return do_launch(b, 1, 1, true);
+  return do_launch(b, 1, PHASE_NO_UPDATE, true);
 }
 int rsb_batch_update_kinematics(rsb_batch* b) {
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
   CK(cudaSetDevice(b->device));
   int rc = ensure_debug(b); if (rc) return rc;
-  return do_launch(b, 1, 1 | 4, true);      // stage A + the getters' buffers; contact records of the last integrate() untouched
+  return do_launch(b, 1, PHASE_NO_UPDATE | PHASE_KINEMATICS, true);      // stage A + the getters' buffers; contact records of the last integrate() untouched
 }
 // lazy getters: refresh M, h and the poses when the state changed through this API since they were last computed
 static int ensure_kinematics(rsb_batch* b) {
@@ -857,72 +857,52 @@ int rsb_batch_get_mass_matrix(rsb_batch* b, int env_begin, int env_count, float*
   if (!out) return fail(RSB_ERR_INVALID, "null output buffer");
   if (env_count == 0) return RSB_OK;
   rc = ensure_kinematics(b); if (rc) return rc;
-  size_t w = (size_t)b->nv * b->nv;
-  CK(cudaMemcpyAsync(out, b->dbg_M + env_begin * w, env_count * w * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  const size_t w = (size_t)b->nv * b->nv;
+  return copy_out(b, out, b->dbg_M + env_begin * w, env_count * w * 4, where);
 }
 int rsb_batch_get_nonlinearities(rsb_batch* b, int env_begin, int env_count, float* out, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!out) return fail(RSB_ERR_INVALID, "null output buffer");
   if (env_count == 0) return RSB_OK;
   rc = ensure_kinematics(b); if (rc) return rc;
-  CK(cudaMemcpyAsync(out, b->dbg_h + (size_t)env_begin * b->nv, (size_t)env_count * b->nv * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  return copy_out(b, out, b->dbg_h + (size_t)env_begin * b->nv, (size_t)env_count * b->nv * 4, where);
 }
 int rsb_batch_get_body_poses(rsb_batch* b, int env_begin, int env_count, float* rot, float* pos, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (env_count == 0) return RSB_OK;
   rc = ensure_kinematics(b); if (rc) return rc;
-  cudaMemcpyKind kind = where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
-  if (rot) CK(cudaMemcpyAsync(rot, b->dbg_R + (size_t)env_begin * b->nb * 9, (size_t)env_count * b->nb * 9 * 4, kind, b->stream));
-  if (pos) CK(cudaMemcpyAsync(pos, b->dbg_p + (size_t)env_begin * b->nb * 3, (size_t)env_count * b->nb * 3 * 4, kind, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  rc = rot ? copy_out(b, rot, b->dbg_R + (size_t)env_begin * b->nb * 9, (size_t)env_count * b->nb * 9 * 4, where) : RSB_OK; if (rc) return rc;
+  return pos ? copy_out(b, pos, b->dbg_p + (size_t)env_begin * b->nb * 3, (size_t)env_count * b->nb * 3 * 4, where) : RSB_OK;
 }
 int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
-  cudaMemcpyKind kind = where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
-  if (out) CK(cudaMemcpyAsync(out, b->contacts + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * sizeof(rsb_contact), kind, b->stream));
-  if (counts) CK(cudaMemcpyAsync(counts, b->ncontacts + env_begin, (size_t)env_count * 4, kind, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  rc = out ? copy_out(b, out, b->contacts + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * sizeof(rsb_contact), where) : RSB_OK; if (rc) return rc;
+  return counts ? copy_out(b, counts, b->ncontacts + env_begin, (size_t)env_count * 4, where) : RSB_OK;
 }
 int rsb_batch_get_contact_points(rsb_batch* b, int32_t* pt, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!pt) return fail(RSB_ERR_INVALID, "null output buffer");
-  CK(cudaMemcpyAsync(pt, b->contact_pt + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  return copy_out(b, pt, b->contact_pt + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * 4, where);
 }
 int rsb_batch_get_solver_iterations(rsb_batch* b, int32_t* it, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!it) return fail(RSB_ERR_INVALID, "null output buffer");
-  CK(cudaMemcpyAsync(it, b->iters + env_begin, (size_t)env_count * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  return copy_out(b, it, b->iters + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_get_solver_status(rsb_batch* b, int32_t* status, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!status) return fail(RSB_ERR_INVALID, "null output buffer");
-  CK(cudaMemcpyAsync(status, b->solver_status + env_begin, (size_t)env_count * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  return copy_out(b, status, b->solver_status + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_get_solver_residual(rsb_batch* b, float* resid, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!resid) return fail(RSB_ERR_INVALID, "null output buffer");
-  CK(cudaMemcpyAsync(resid, b->resid + env_begin, (size_t)env_count * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  return copy_out(b, resid, b->resid + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_get_diverged(rsb_batch* b, int32_t* flags, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!flags) return fail(RSB_ERR_INVALID, "null output buffer");
-  CK(cudaMemcpyAsync(flags, b->diverged + env_begin, (size_t)env_count * 4, where == RSB_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, b->stream));
-  if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  return copy_out(b, flags, b->diverged + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_device_ptrs(rsb_batch* b, rsb_device_view* v) {
   if (!b || !v) return fail(RSB_ERR_INVALID, "null argument");
@@ -937,17 +917,11 @@ int rsb_batch_ob_dim(const rsb_batch* b) {
   if (!b) return 0;
   return b->model->md.floating ? (b->nq + b->nv - 3) : (b->nq + b->nv);
 }
-static int observe_impl(rsb_batch* b, float* obs, int env_begin, int env_count, int where, bool sync) {
+static int observe_impl(rsb_batch* b, float* obs, int env_begin, int env_count, int where) {
   const int od = rsb_batch_ob_dim(b);
   float* dst = obs;
   if (where == RSB_HOST) {
-    size_t need = (size_t)b->N * od;
-    if (b->obs_staging_words < need) {
-      if (b->obs_staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->obs_staging); }
-      b->obs_staging = nullptr; b->obs_staging_words = 0;
-      CK(cudaMalloc((void**)&b->obs_staging, need * 4));
-      b->obs_staging_words = need;
-    }
+    int rc = ensure_obs_staging(b); if (rc) return rc;
     dst = b->obs_staging;
   }
   int threads = 128, blocks = (env_count * 32 + threads - 1) / threads;
@@ -955,18 +929,14 @@ static int observe_impl(rsb_batch* b, float* obs, int env_begin, int env_count, 
                                                          b->gc_stride, b->gv_stride, b->nq, b->nv, b->model->md.floating, env_count, dst, od);
   CK(cudaGetLastError());
   b->launches++;
-  if (where == RSB_HOST) {
-    CK(cudaMemcpyAsync(obs, dst, (size_t)env_count * od * 4, cudaMemcpyDeviceToHost, b->stream));
-    if (sync) CK(cudaStreamSynchronize(b->stream));
-  }
-  return RSB_OK;
+  return where == RSB_HOST ? copy_out(b, obs, dst, (size_t)env_count * od * 4, RSB_HOST) : RSB_OK;
 }
 int rsb_batch_observe(rsb_batch* b, float* obs, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;
   if (!obs) return fail(RSB_ERR_INVALID, "null obs");
   if (env_count == 0) return RSB_OK;
   CK(cudaSetDevice(b->device));
-  return observe_impl(b, obs, env_begin, env_count, where, true);
+  return observe_impl(b, obs, env_begin, env_count, where);
 }
 
 // VectorizedEnvironment::step() for the whole batch in ONE call: PD targets in, `substeps` fused
@@ -996,7 +966,7 @@ int rsb_batch_control_step(rsb_batch* b, const float* ptarget, const float* vtar
   const bool bound_once = b->pt_once || b->vt_once;
   if (!obs || !b->model->md.floating) {
     rc = do_launch(b, substeps, 0, false); if (rc) return rc;
-    if (obs) rc = observe_impl(b, obs, 0, b->N, where_out, true);
+    if (obs) rc = observe_impl(b, obs, 0, b->N, where_out);
     if (bound_once) CK(cudaStreamSynchronize(b->stream));   // the caller may reuse its pinned target buffer on return
     return rc;
   }
@@ -1010,20 +980,12 @@ int rsb_batch_control_step(rsb_batch* b, const float* ptarget, const float* vtar
     return RSB_OK;
   }
   if (where_out == RSB_HOST) {
-    size_t need = (size_t)b->N * od;
-    if (b->obs_staging_words < need) {
-      if (b->obs_staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->obs_staging); }
-      b->obs_staging = nullptr; b->obs_staging_words = 0;
-      CK(cudaMalloc((void**)&b->obs_staging, need * 4));
-      b->obs_staging_words = need;
-    }
+    rc = ensure_obs_staging(b); if (rc) return rc;
     dst = b->obs_staging;
   }
   rc = do_launch(b, substeps, 0, false, dst, where_out == RSB_DEVICE); if (rc) return rc;
-  if (where_out == RSB_HOST) {
-    CK(cudaMemcpyAsync(obs, dst, (size_t)b->N * od * 4, cudaMemcpyDeviceToHost, b->stream));
-    CK(cudaStreamSynchronize(b->stream));
-  } else if (bound_once) CK(cudaStreamSynchronize(b->stream));
+  if (where_out == RSB_HOST) return copy_out(b, obs, dst, (size_t)b->N * od * 4, RSB_HOST);
+  if (bound_once) CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
 
@@ -1150,10 +1112,11 @@ int rsb_batch_set_observation_peers(rsb_batch* b, int world, int rank, void* con
   for (int p = 0; p < world; p++) if (!obs_all[2 * p] || !obs_all[2 * p + 1] || !flags[p]) return fail(RSB_ERR_INVALID, "null peer buffer");
   CK(cudaSetDevice(b->device));
   CK(cudaStreamSynchronize(b->stream));
-  for (int p = 0; p < world; p++) { b->peer_obs[p][0] = (float*)obs_all[2 * p]; b->peer_obs[p][1] = (float*)obs_all[2 * p + 1]; b->peer_flag[p] = (unsigned*)flags[p]; }
-  b->peer_world = world; b->peer_rank = rank; b->peer_epoch = 0;
+  b->peer_world = 0;              // a failure below leaves the batch without peers
   if (!b->peer_done) CK(cudaMalloc(&b->peer_done, sizeof(unsigned)));
   CK(cudaMemsetAsync(b->peer_done, 0, sizeof(unsigned), b->stream));
+  for (int p = 0; p < world; p++) { b->peer_obs[p][0] = (float*)obs_all[2 * p]; b->peer_obs[p][1] = (float*)obs_all[2 * p + 1]; b->peer_flag[p] = (unsigned*)flags[p]; }
+  b->peer_world = world; b->peer_rank = rank; b->peer_epoch = 0;
   return RSB_OK;
 }
 // *buffer_parity (optional) = which of this rank's two buffers holds the rows of the LAST control step of every rank.  The arrival
@@ -1161,12 +1124,6 @@ int rsb_batch_set_observation_peers(rsb_batch* b, int world, int rank, void* con
 // after the step the rows are complete and nothing is enqueued here.
 int rsb_batch_wait_observation_peers(rsb_batch* b, int* buffer_parity) {
   if (!b || b->peer_world <= 0 || b->peer_epoch == 0) return fail(RSB_ERR_INVALID, "no fused observation gather in flight");
-  if (!b->peer_done) {       // (unreachable with rsb_batch_set_observation_peers; kept as the stand-alone form of the wait)
-    CK(cudaSetDevice(b->device));
-    rsb_peer_wait_kernel<<<1, 32, 0, b->stream>>>(b->peer_flag[b->peer_rank], b->peer_world, b->peer_epoch * (unsigned)b->grid, 20000000000ll /* ~10 s of SM clocks */);
-    CK(cudaGetLastError());
-    b->launches++;
-  }
   if (buffer_parity) *buffer_parity = (int)((b->peer_epoch - 1) & 1);
   return RSB_OK;
 }

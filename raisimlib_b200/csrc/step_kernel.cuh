@@ -123,6 +123,10 @@ __host__ __device__ constexpr BlobHeader make_blob_header(Dims d, int npts, int 
 // workspace; allocated only when pairs are enabled (make_ws_layout)
 __host__ __device__ constexpr int self_y_words(int maxdd) { return round_up_c((maxdd + 1) * (3 * RSB_KMAX + RSB_LMAX + 1), 4); }
 
+// stage B's per-warp hit list (stage_b_narrow_phase): HL_CAP rows of HL_WORDS words
+constexpr int HL_WORDS = 9;            // depth (<= 0: dropped), normal, position, pair, candidate index; odd stride: conflict-free by lane
+constexpr int HL_CAP = 64;             // two candidate slots per lane at most
+
 // per-warp workspace layout (word offsets)
 struct WsLayout {
   int o_gc, o_gv, o_tau, o_pt, o_vt, o_L, o_invd, o_rhs, o_z, o_ct, o_Y, o_lam, o_u, o_lim, o_hist, o_sat;   // persistent
@@ -151,8 +155,8 @@ __host__ __device__ constexpr WsLayout make_ws_layout(Dims d, int npairs = 0) {
   L.o_lim = o; o += 4 * LMAX;                                     // joint-limit rows: dof, sign, violation
   L.o_sat = o; o += nvp;                                          // dof driven at its actuator effort limit in this sub-step (stage C -> E)
   L.o_hist = o; o += HIST_WORDS;                                  // Anderson acceleration: u0, x, g, f, dG, dF (one value per constraint row each)
-  if (o - L.o_Y < 9 * 64) o = L.o_Y + 9 * 64;                     // stage B keeps its hit list (HL_CAP rows of HL_WORDS) in [o_Y, here): dead until stage C
-  if (npairs > 0 && o - L.o_Y < 9 * (64 + npairs)) o = L.o_Y + 9 * (64 + npairs);   // ... and one row per self-collision pair
+  if (o - L.o_Y < HL_CAP * HL_WORDS) o = L.o_Y + HL_CAP * HL_WORDS;   // stage B keeps its hit list in [o_Y, here): dead until stage C
+  if (npairs > 0 && o - L.o_Y < (HL_CAP + npairs) * HL_WORDS) o = L.o_Y + (HL_CAP + npairs) * HL_WORDS;   // ... and one row per self-collision pair
   // union: {h, b, poses} (stages A-C) overlaid by G (stages C-D)
   int ua = 0;
   L.o_h = o + ua; ua += nvp;
@@ -189,6 +193,10 @@ struct GymConfig {
   float torque_coeff, forward_vel_coeff, terminal_reward;
 };
 
+// StepArgs::phase_mask bits of the launches that stop early (the host's getters and integrate1())
+constexpr int PHASE_NO_UPDATE = 1;    // stop after stage B (integrate1: no state update)
+constexpr int PHASE_KINEMATICS = 4;   // stop after stage A (stage A + the getters' buffers; the contact records of the last integrate() stay)
+
 struct StepArgs {
   int num_envs, substeps;
   int gc_stride, gv_stride, pt_stride, vt_stride;   // vt_stride likewise for vtarget; pt_stride: row stride of ptarget (own padded buffer or a bound caller buffer)
@@ -224,7 +232,7 @@ struct StepArgs {
   unsigned* peer_flag[MAX_PEERS];  // peer p's arrival counters [world]: += 1 per finished CTA of this rank
   int peer_world, peer_rank;
   unsigned peer_expected;          // arrival count every rank's counter reaches when its rows of THIS step have landed (steps so far x CTAs)
-  unsigned* peer_done;             // CTAs of this launch that finished: the last one waits for the peers (null: the caller enqueues rsb_peer_wait_kernel)
+  unsigned* peer_done;             // CTAs of this launch that finished: the last one waits for the peers (set whenever peer_world > 0)
   // RaisimGym task fused into the step (rsb_batch_gym_step): the launch turns the action rows into PD targets before the first
   // sub-step and, after the last one, computes reward and termination, resets the terminated environments and writes the
   // observation rows of the (possibly reset) state -- VectorizedEnvironment::step() + observe() in ONE launch
@@ -232,9 +240,8 @@ struct StepArgs {
   GymConfig gym;
   float* gym_reward;               // [num_envs]
   unsigned char* gym_done;         // [num_envs]
-  int phase_mask;      // bit0: stop after stage B (integrate1: no state update); bit2: kinematics only (stage A + getters' buffers,
-                       // the contact records of the last integrate() stay as they are)
-  int substep_barrier; // 1: re-align the CTA's warps of one round at every sub-step (2, 3: also before stages C, E)
+  int phase_mask;      // 0 (a full step) or PHASE_NO_UPDATE, optionally with PHASE_KINEMATICS
+  int substep_barrier; // non-zero: re-align the CTA's warps of one round at every sub-step
   int pair_stage_a;    // 1: quadruped instance, CTAs that keep the sub-step barrier: one warp runs stage A of two environments
 };
 
@@ -403,13 +410,11 @@ __device__ __forceinline__ QuadLeg quad_factor_legs(float* s_L, float* s_invd, i
 
 // ------------------------------------------------------------------ stage B: narrow phase ------
 // lane = contact candidate (SLOTS x 32 of them): Ground / HeightMap queries, ballot-compacted contact list in candidate order, the
-// RSB_KMAX deepest kept.  Out of line (one call per sub-step) so that the candidate registers of both slots get an allocation of
-// their own instead of being spilled around the rest of the 72-register kernel body.  Returns the number of contacts written to s_ct.
+// RSB_KMAX deepest kept.  Returns the number of contacts written to s_ct.
 // Stage B writes every penetrating candidate into a per-warp hit list in shared memory (rows of HL_WORDS words, candidate order), keeps
 // the KMAX deepest and emits the contact records.  Nothing per candidate survives in registers across the candidate slots, so the
-// stage needs no register arrays (which ptxas had placed in local memory) and can be compiled out of line.
-constexpr int HL_WORDS = 9;            // depth (<= 0: dropped), normal, position, pair, candidate index; odd stride: conflict-free by lane
-constexpr int HL_CAP = 64;             // two candidate slots per lane at most
+// stage needs no register arrays (which ptxas had placed in local memory).  It is inlined into the kernel (an out-of-line stage B is
+// one of the dead ends of DESIGN §6); the segment / box shape routines it calls stay out of line.
 
 // ---- self-collision pairs (generic instance only): the narrow phase of one pair, the oracle's SelfPair routine in float32
 // (oracle/self_collision.hpp self_pair_geometry: same closest-point rule for parallel and degenerate segments, same face rule inside a box)
@@ -476,14 +481,11 @@ __device__ __noinline__ bool self_pair_contact(const float* pr, const float* s_p
   return true;
 }
 
-#ifndef RSB_STAGE_B_INLINE
-#define RSB_STAGE_B_INLINE __forceinline__
-#endif
 // ter: the kernel parameter itself (constant bank); ter_s: its shared-memory copy, for the out-of-line shape routines
 // SELF: the generic instance, which also runs the self-collision pairs of the blob (lane = pair, after the terrain candidates)
 template <int SLOTS, bool SELF = false>
-__device__ RSB_STAGE_B_INLINE int stage_b_narrow_phase(const TerrainDesc& ter, const TerrainDesc& ter_s, const uint32_t* blob_s, const float* s_pose, float* s_ct, float* s_list,
-                                                 int env, int lane, int nbp, unsigned* prof) {
+__device__ __forceinline__ int stage_b_narrow_phase(const TerrainDesc& ter, const TerrainDesc& ter_s, const uint32_t* blob_s, const float* s_pose, float* s_ct, float* s_list,
+                                              int env, int lane, int nbp, unsigned* prof) {
   const BlobHeader& H = *reinterpret_cast<const BlobHeader*>(blob_s);
   const float* ptsf = reinterpret_cast<const float*>(blob_s + H.off_pts);
   const int* ptsi = reinterpret_cast<const int*>(blob_s + H.off_pts);
@@ -734,10 +736,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
   constexpr bool QUAD = SNB == 13 && SNQ == 19 && SNV == 18 && SFL == 1 && SMAXDEPTH == 3 && SMAXDD == 8;
   // deep trees on few resident warps (the humanoid instance: 14 warps per SM, latency-bound) get their dependent shared-memory loops of
   // stage C unrolled for memory-level parallelism; everything else keeps them rolled (instruction cache)
-#ifndef RSB_DEEP_UNROLL
-#define RSB_DEEP_UNROLL 4
-#endif
-  constexpr int UNR = (ST && !QUAD && SMAXDD >= 12) ? RSB_DEEP_UNROLL : 1;
+  constexpr int UNR = (ST && !QUAD && SMAXDD >= 12) ? 4 : 1;
   constexpr Dims SD{SNB, SNQ, SNV, SFL, SMAXDEPTH, SMAXDD};
   constexpr WsLayout LS = make_ws_layout(SD);
   constexpr BlobHeader HS = make_blob_header(SD, 0, 0);
@@ -838,14 +837,6 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
     }
     __syncthreads();
   }
-  // Sub-step barrier: the warps of this CTA that own an environment in this round (env - warp = the CTA's first one).  Counts of
-  // two rounds never meet on barrier 1: a warp arrives at it only at the sub-steps of its current round, and the last barrier of
-  // round r (its last sub-step) completes only once every warp of round r has arrived, so no round-r warp is still to arrive when
-  // the first warp of round r + 1 does.  A warp without an environment in round r + 1 (environments are dense, so those are the
-  // highest warps of the CTA) leaves the loop and never arrives again.
-#define SUBSTEP_BARRIER(level) \
-  if (args.substep_barrier >= (level) && s_work[0] <= 2 * s_work[1])             \
-    asm volatile("bar.sync 1, %0;" ::"r"(min(WPC, args.num_envs - (env - warp)) * 32))
 #pragma unroll 1
   for (int env = blockIdx.x * WPC + warp; env < args.num_envs; env += warps_total) {
     // ---- load this environment's rows (coalesced: one row per warp) -----------------------------
@@ -885,7 +876,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
     // with a partner, -1 partner, 0 alone (other instances; a leader whose partner has no environment in this round).
     int pair_a = 0;
     if constexpr (QUAD) {
-      if (args.pair_stage_a && args.substep_barrier >= 1 && s_work[0] <= 2 * s_work[1])
+      if (args.pair_stage_a && args.substep_barrier && s_work[0] <= 2 * s_work[1])
         pair_a = (warp & 4) ? -1 : (warp + 4 < min(WPC, args.num_envs - (env - warp)) ? 1 : 0);
     }
     int K = 0, iters = 0;
@@ -895,7 +886,13 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
     for (int sub = 0; sub < args.substeps; sub++) {
       // Re-align the round's warps (instruction-cache locality: warps drifting through a 75 KB kernel miss the instruction
       // cache far more often than warps in the same stage, and the slowest warp of a sub-step finishes its solve alone).
-      SUBSTEP_BARRIER(1);
+      // The barrier counts the warps of this CTA that own an environment in this round (env - warp = the CTA's first one).  Counts
+      // of two rounds never meet on barrier 1: a warp arrives at it only at the sub-steps of its current round, and the last barrier
+      // of round r (its last sub-step) completes only once every warp of round r has arrived, so no round-r warp is still to arrive
+      // when the first warp of round r + 1 does.  A warp without an environment in round r + 1 (environments are dense, so those are
+      // the highest warps of the CTA) leaves the loop and never arrives again.
+      if (args.substep_barrier && s_work[0] <= 2 * s_work[1])
+        asm volatile("bar.sync 1, %0;" ::"r"(min(WPC, args.num_envs - (env - warp)) * 32));
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 0] = (unsigned)clock64();
       // =========================== stage A: FK + RNEA + CRBA =====================================
       f3 O;                                  // base origin: centre of the world-aligned CRBA frame (stages A and C)
@@ -1106,15 +1103,14 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 1] = (unsigned)clock64();
       if (args.dbg_M)   // getters (integrate1): cold path, kept out of line to spare the instruction cache
         write_debug(args, env, lane, nv, nb, nvp, DLP, s_L, s_h, ddepth, danc, bvalid, s_pose, nbp);
-      if (args.phase_mask & 4) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // kinematics for the getters only
+      if (args.phase_mask & PHASE_KINEMATICS) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // kinematics for the getters only
 
       // =========================== stage B: narrow phase ========================================
       K = stage_b_narrow_phase<SLOTS, !ST>(args.ter, s_ter, blob_s, s_pose, s_ct, s_Y, env, lane, nbp, args.prof ? args.prof + ((size_t)env * 4 + (sub & 3)) * 8 : nullptr);
       const int C = 3 * K;
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 2] = (unsigned)clock64();
-      if (args.phase_mask & 1) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // integrate1(): kinematics, collision, M, h only
+      if (args.phase_mask & PHASE_NO_UPDATE) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // integrate1(): kinematics, collision, M, h only
 
-      SUBSTEP_BARRIER(2);
       // =========================== stage C: b, Mhat = L^T L, z, Y, G ==============================
       // a9 joint limits: the first LMAX joints found beyond their URDF limit become unilateral rows sign * qdot >= target
       int Lm = 0;
@@ -1543,7 +1539,6 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       }
       __syncwarp();
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 4] = (unsigned)clock64();
-      SUBSTEP_BARRIER(3);
       // =========================== stage E: v+ = v + L^-1 (dt z + Y lam), integration ============
       if constexpr (QUAD) {
         // w_i = dt z_i + sum over the rows whose chain holds dof i of Y[depth i][row] lam_row, lane = dof
@@ -1710,7 +1705,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       __syncwarp();
     }
     // ---- store state rows and contact records -----------------------------------------------------
-    if (!(args.phase_mask & 1)) {
+    if (!(args.phase_mask & PHASE_NO_UPDATE)) {
       float* g_gc = args.gc + (size_t)env * args.gc_stride;
       float* g_gv = args.gv + (size_t)env * args.gv_stride;
 #pragma unroll 1
@@ -1745,7 +1740,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         }
       }
     }
-    if (args.phase_mask & 4) { __syncwarp(); continue; }   // kinematics only: contact records, iteration counts and flags of the last integrate() stay
+    if (args.phase_mask & PHASE_KINEMATICS) { __syncwarp(); continue; }   // kinematics only: contact records, iteration counts and flags of the last integrate() stay
     {   // failure detection: a non-finite coordinate or velocity marks the environment as diverged
       bool bad = false;
 #pragma unroll 1
@@ -1762,7 +1757,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       if (lane < K) {
         const float* ct = s_ct + lane * CT_WORDS;
         float lx = 0.f, ly = 0.f, lz = 0.f;
-        if (!(args.phase_mask & 1)) { lx = s_lam[3 * lane]; ly = s_lam[3 * lane + 1]; lz = s_lam[3 * lane + 2]; }
+        if (!(args.phase_mask & PHASE_NO_UPDATE)) { lx = s_lam[3 * lane]; ly = s_lam[3 * lane + 1]; lz = s_lam[3 * lane + 2]; }
         rc.local_body = __float_as_int(ct[CF_BODY]); rc.pair_index = __float_as_int(ct[CF_PAIR]);
         pt = __float_as_int(ct[CF_PT]);
 #pragma unroll
@@ -1781,7 +1776,6 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
     }
     __syncwarp();
   }
-#undef SUBSTEP_BARRIER
   if (args.peer_world > 0 && args.obs) {
     // every row this CTA stored must be visible on the peers before they see the arrival count: the CTA barrier orders the warps'
     // stores before the signalling threads, whose release at system scope is cumulative over them (one fence per signalling
@@ -1789,42 +1783,26 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
     __syncthreads();
     if ((int)threadIdx.x < args.peer_world)
       asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(args.peer_flag[threadIdx.x] + args.peer_rank), "r"(1u) : "memory");
-    if (args.peer_done) {
-      // the arrival wait folded into the launch: the last CTA to finish stays until every rank's rows of this step have landed in
-      // THIS GPU's buffer, so the launch completes exactly when the gathered rows do (no separate wait kernel, no launch gap).
-      // Bounded: a dead peer traps instead of hanging the GPU.
-      __shared__ int s_last;
-      if (threadIdx.x == 0) {
-        const unsigned d = atomicAdd(args.peer_done, 1u);
-        s_last = d == gridDim.x - 1 ? 1 : 0;
-        if (s_last) *args.peer_done = 0u;           // every CTA has counted itself: ready for the next launch
-      }
-      __syncthreads();
-      if (s_last && (int)threadIdx.x < args.peer_world) {
-        const unsigned* f = args.peer_flag[args.peer_rank] + threadIdx.x;
-        const long long t0 = clock64();
-        for (;;) {
-          unsigned v;
-          asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-          if ((int)(v - args.peer_expected) >= 0) break;
-          if (clock64() - t0 > 20000000000ll) __trap();
-        }
+    // the arrival wait folded into the launch: the last CTA to finish stays until every rank's rows of this step have landed in
+    // THIS GPU's buffer, so the launch completes exactly when the gathered rows do (no separate wait kernel, no launch gap).
+    // Bounded: a dead peer traps instead of hanging the GPU.
+    __shared__ int s_last;
+    if (threadIdx.x == 0) {
+      const unsigned d = atomicAdd(args.peer_done, 1u);
+      s_last = d == gridDim.x - 1 ? 1 : 0;
+      if (s_last) *args.peer_done = 0u;           // every CTA has counted itself: ready for the next launch
+    }
+    __syncthreads();
+    if (s_last && (int)threadIdx.x < args.peer_world) {
+      const unsigned* f = args.peer_flag[args.peer_rank] + threadIdx.x;
+      const long long t0 = clock64();
+      for (;;) {
+        unsigned v;
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
+        if ((int)(v - args.peer_expected) >= 0) break;
+        if (clock64() - t0 > 20000000000ll) __trap();
       }
     }
-  }
-}
-
-// Arrival wait of the fused observation all-gather: lane r returns when rank r's `expected` CTAs have signalled, i.e. when every
-// row of that rank's step has landed in THIS GPU's gathered buffer.  Bounded: a dead peer traps instead of hanging the GPU.
-__global__ void rsb_peer_wait_kernel(const unsigned* flags, int world, unsigned expected, long long max_cycles) {
-  if ((int)threadIdx.x >= world) return;
-  const volatile unsigned* f = flags + threadIdx.x;
-  const long long t0 = clock64();
-  for (;;) {
-    unsigned v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-    if ((int)(v - expected) >= 0) break;
-    if (clock64() - t0 > max_cycles) __trap();
   }
 }
 

@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 from conftest import RSC
-from helpers import ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, MARGIN, THRESH, setup_batch, index_parity
+from helpers import ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, MARGIN, THRESH, setup_batch, index_parity, launch_config
 from oracle.oracle import Oracle
 from oracle.urdf_tables import load_tables
 
@@ -1050,7 +1050,8 @@ def _peer_worker(rank, world, port, q):
 
 def test_fused_peer_observation_gather_two_gpus(capi):
     """SURVEY 8e without NCCL on the data path: every rank's step kernel stores its observation rows into every rank's buffer over
-    NVLink peer memory (CUDA IPC), counters + a wait kernel close the exchange; rows must equal each rank's own rows, in rank order."""
+    NVLink peer memory (CUDA IPC), arrival counters and a wait at the end of the same launch close the exchange; rows must equal each
+    rank's own rows, in rank order."""
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two GPUs")
@@ -1069,6 +1070,55 @@ def test_fused_peer_observation_gather_two_gpus(capi):
         ref = np.concatenate([got[r][k][0] for r in range(world)])     # every rank's own rows of step k, in rank order
         for r in range(world):
             assert np.array_equal(got[r][k][1], ref), (k, r)
+
+
+def test_fused_peer_observation_gather_one_gpu(capi):
+    """the fused observation gather with world = 1 runs the tail of the step launch that every rank of a multi-GPU job runs (rows
+    stored into the gathered buffer, the arrival counter, the last CTA's wait) on one card: the gathered rows equal the step's own
+    observation rows bit for bit, the two buffers alternate by step, and each control step is one launch (the wait is part of it)."""
+    import ctypes
+    import torch
+    n = 300                                                            # not a multiple of the CTA size
+    bt = capi.Batch(capi.Model(os.path.join(RSC, "anymal_c_like.urdf")), n)
+    bt.set_ground(0.0)
+    rng = np.random.default_rng(501)
+    gc = np.tile(ANYMAL_GC0, (n, 1)); gc[:, 2] = rng.uniform(0.5, 0.7, n); gc[:, 7:] += rng.uniform(-0.2, 0.2, (n, 12))
+    bt.set_state(gc.astype(np.float32), (0.3 * rng.standard_normal((n, 18))).astype(np.float32))
+    od = bt.ob_dim()
+    L = capi.lib()
+    bufs = []                                                          # two gathered-rows buffers (parity 0, 1) and the counter row
+    for nbytes in (n * od * 4, n * od * 4, 256):
+        p = ctypes.c_void_p()
+        capi._ck(L.rsb_peer_buffer_create(0, nbytes, ctypes.byref(p), None))
+        bufs.append(p.value)
+
+    class _Raw:
+        def __init__(self, ptr, shape, typestr):
+            self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "version": 2}
+
+    try:
+        rows = [torch.as_tensor(_Raw(p, (n, od), "<f4"), device="cuda") for p in bufs[:2]]
+        counter = torch.as_tensor(_Raw(bufs[2], (1,), "<i4"), device="cuda")
+        bt.set_observation_peers(1, 0, bufs[:2], bufs[2:])
+        grid = launch_config(capi, bt)["grid"]
+        obs = torch.empty((n, od), dtype=torch.float32, device="cuda")
+        own = []
+        for k in range(3):                                             # three steps: both buffer parities, the counter accumulates
+            launches = bt.launch_count()
+            bt.control_step(None, 2, obs)
+            parity = bt.wait_observation_peers()
+            assert bt.launch_count() == launches + 1                   # no wait launch of its own
+            assert parity == k % 2
+            bt.sync()
+            own.append(obs.cpu().numpy().copy())
+            assert np.array_equal(rows[parity].cpu().numpy(), own[k]), k
+            assert int(counter.cpu()[0]) == (k + 1) * grid             # one arrival per CTA and step
+        assert np.array_equal(rows[1].cpu().numpy(), own[1])           # the other buffer still holds the step before
+        assert not np.array_equal(own[1], own[2])
+    finally:
+        bt.set_observation_peers(0, 0, None, None)
+        for p in bufs:
+            capi._ck(L.rsb_peer_buffer_destroy(ctypes.c_void_p(p)))
 
 
 def test_heightmap_narrow_phase_known_answers_on_gpu(capi):
