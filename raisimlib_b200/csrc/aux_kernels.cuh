@@ -9,7 +9,7 @@
 
 namespace rsb {
 
-// obs_rot_column / obs_dot3: see step_kernel.cuh (shared with the fused observation write)
+// write_obs_row: step_kernel.cuh (shared with the fused observation write)
 __global__ void rsb_observe_kernel(const float* __restrict__ gc, const float* __restrict__ gv, int gc_stride, int gv_stride, int nq, int nv,
                                    int floating, int num_envs, float* __restrict__ obs, int ob_dim) {
   const int lane = threadIdx.x & 31;
@@ -17,25 +17,13 @@ __global__ void rsb_observe_kernel(const float* __restrict__ gc, const float* __
   if (env >= num_envs) return;
   const float* q = gc + (size_t)env * gc_stride;
   const float* v = gv + (size_t)env * gv_stride;
-  float* o = obs + (size_t)env * ob_dim;
   if (!floating) {
+    float* o = obs + (size_t)env * ob_dim;
     for (int i = lane; i < nq; i += 32) o[i] = q[i];
     for (int i = lane; i < nv; i += 32) o[nq + i] = v[i];
     return;
   }
-  float qw = q[3], qx = q[4], qy = q[5], qz = q[6];
-  float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
-  qw *= inv; qx *= inv; qy *= inv; qz *= inv;
-  const int nj = nq - 7;
-  if (lane == 0) o[0] = q[2];
-  if (lane < 3) {
-    float c0, c1, c2;
-    obs_rot_column(qw, qx, qy, qz, lane, c0, c1, c2);
-    o[1 + lane] = c2;
-    o[4 + nj + lane] = obs_dot3(c0, c1, c2, v[0], v[1], v[2]);
-    o[7 + nj + lane] = obs_dot3(c0, c1, c2, v[3], v[4], v[5]);
-  }
-  for (int i = lane; i < nj; i += 32) { o[4 + i] = q[7 + i]; o[10 + nj + i] = v[6 + i]; }
+  write_obs_row(obs, ob_dim, env, q, v, nq, lane);
 }
 
 // external wrench rows for rsb_step_kernel (StepArgs::ext): [body | F(3) | T(3) | point in body frame(3) | pad(2)]

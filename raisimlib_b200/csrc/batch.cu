@@ -238,17 +238,9 @@ static void build_blob(rsb_batch* b) {
 static void build_ws_layout(rsb_batch* b) { b->ws = make_ws_layout(b->dims, (int)b->self_mu.size()); }
 
 // ------------------------------------------------------------------ launches --------------------
-// static specialisations: every 12-joint quadruped (ANYmal, A1, Go1, ...) shares (13,19,18,floating,3,8);
-// the Atlas-like humanoid is (31,37,36,floating,10,15).  Anything else takes the generic kernel.
-constexpr Dims kQuad12{13, 19, 18, 1, 3, 8};
-constexpr Dims kHumanoid30{31, 37, 36, 1, 10, 15};
-static bool same_dims(const Dims& a, const Dims& b) {
-  return a.nb == b.nb && a.nq == b.nq && a.nv == b.nv && a.floating == b.floating && a.maxdepth == b.maxdepth && a.maxdd == b.maxdd;
-}
-
-template <int WPC, int SLOTS, int NB, int NQ, int NV, int FL, int MD, int MDD>
+template <int WPC, int SLOTS, int SPEC>
 static cudaError_t launch_step(const StepArgs& a, int grid, size_t smem, cudaStream_t s) {
-  auto kern = rsb_step_kernel<WPC, SLOTS, NB, NQ, NV, FL, MD, MDD>;
+  auto kern = rsb_step_kernel<WPC, SLOTS, SPEC>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   kern<<<grid, WPC * 32, smem, s>>>(a);
@@ -268,20 +260,22 @@ static int pick_config(rsb_batch* b) {
   const size_t per_warp = (size_t)b->ws.words * 4;
   const int sms = prop.multiProcessorCount;
   b->slots = b->model->md.npts() > 32 ? 2 : 1;
+  // the static instance of the model's dimensions (step_kernel.cuh SPEC_DIMS), if any
+  b->spec = SPEC_GENERIC;
+  for (int s = SPEC_GENERIC + 1; s < SPEC_COUNT; s++)
+    if (b->dims == SPEC_DIMS[s]) b->spec = s;
   // the quadruped instance has the topology compiled in (floating base + 4 serial chains of 3 joints in DFS order): check it
-  bool quad_topology = same_dims(b->dims, kQuad12);
-  if (quad_topology) {
+  if (b->spec == SPEC_QUAD) {
     const Model& md = b->model->md;
     for (int leg = 0; leg < 4; leg++)
       for (int j = 0; j < 3; j++) {
         const int body = 1 + 3 * leg + j;
-        if (md.parent[body] != (j == 0 ? 0 : body - 1) || md.vidx[body] != 5 + body || md.qidx[body] != 6 + body) quad_topology = false;
-        if (md.jtype[body] != 1 && md.jtype[body] != 2) quad_topology = false;
+        if (md.parent[body] != (j == 0 ? 0 : body - 1) || md.vidx[body] != 5 + body || md.qidx[body] != 6 + body) b->spec = SPEC_GENERIC;
+        if (md.jtype[body] != 1 && md.jtype[body] != 2) b->spec = SPEC_GENERIC;
       }
   }
-  b->spec = quad_topology ? 1 : (same_dims(b->dims, kHumanoid30) ? 2 : 0);
-  if (const char* e = getenv("RSB_FORCE_GENERIC")) if (atoi(e)) b->spec = 0;
-  if (!b->self_mu.empty()) b->spec = 0;   // self-collision pairs are compiled into the generic instance only
+  if (const char* e = getenv("RSB_FORCE_GENERIC")) if (atoi(e)) b->spec = SPEC_GENERIC;
+  if (!b->self_mu.empty()) b->spec = SPEC_GENERIC;   // self-collision pairs are compiled into the generic instance only
   // Warps per CTA (= resident environments per CTA).  A round of w resident warps per SM costs ~ max(13, w): latency-bound up to a
   // dozen warps, issue-bound beyond.  Choose the option with the smallest rounds x cost, ties to the larger CTA (one sub-step
   // barrier group, one copy of the model block).  On the 132 SMs of an H100, 4096 ANYmal-like environments (7.5 KB workspaces, at
@@ -312,11 +306,11 @@ static int pick_config(rsb_batch* b) {
 
 template <int WPC>
 static cudaError_t dispatch_spec(const rsb_batch* b, const StepArgs& a) {
-  if (b->spec == 1 && b->slots == 1) return launch_step<WPC, 1, 13, 19, 18, 1, 3, 8>(a, b->grid, b->smem_bytes, b->stream);
-  if (b->spec == 1) return launch_step<WPC, 2, 13, 19, 18, 1, 3, 8>(a, b->grid, b->smem_bytes, b->stream);
-  if (b->spec == 2) return launch_step<WPC, 2, 31, 37, 36, 1, 10, 15>(a, b->grid, b->smem_bytes, b->stream);
-  if (b->slots == 1) return launch_step<WPC, 1, 0, 0, 0, 0, 0, 0>(a, b->grid, b->smem_bytes, b->stream);
-  return launch_step<WPC, 2, 0, 0, 0, 0, 0, 0>(a, b->grid, b->smem_bytes, b->stream);
+  if (b->spec == SPEC_QUAD && b->slots == 1) return launch_step<WPC, 1, SPEC_QUAD>(a, b->grid, b->smem_bytes, b->stream);
+  if (b->spec == SPEC_QUAD) return launch_step<WPC, 2, SPEC_QUAD>(a, b->grid, b->smem_bytes, b->stream);
+  if (b->spec == SPEC_HUMANOID) return launch_step<WPC, 2, SPEC_HUMANOID>(a, b->grid, b->smem_bytes, b->stream);
+  if (b->slots == 1) return launch_step<WPC, 1, SPEC_GENERIC>(a, b->grid, b->smem_bytes, b->stream);
+  return launch_step<WPC, 2, SPEC_GENERIC>(a, b->grid, b->smem_bytes, b->stream);
 }
 
 struct GymLaunch { const float* action; float* reward; unsigned char* done; };   // rsb_batch_gym_step: the task fused into the step launch

@@ -301,8 +301,9 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
                : "memory");
 }
 
-// Observation arithmetic shared by rsb_observe_kernel and the fused write in rsb_step_kernel: explicit
-// round-to-nearest intrinsics, so that both produce bit-identical rows whatever the compiler contracts elsewhere.
+// Observation row of a floating-base robot, written by rsb_observe_kernel and fused into rsb_step_kernel (one warp per row; q, v: the
+// state rows): [z, R^T e_z, q_j, R^T v, R^T w, qdot_j].  Explicit round-to-nearest intrinsics keep the rotation part independent of
+// what the compiler contracts around it.
 // c = column `col` (0..2) of the base rotation matrix of the unit quaternion (qw, qx, qy, qz).
 __device__ __forceinline__ void obs_rot_column(float qw, float qx, float qy, float qz, int col, float& c0, float& c1, float& c2) {
   const float xx = __fmul_rn(qx, qx), yy = __fmul_rn(qy, qy), zz = __fmul_rn(qz, qz);
@@ -317,6 +318,24 @@ __device__ __forceinline__ void obs_rot_column(float qw, float qx, float qy, flo
 }
 __device__ __forceinline__ float obs_dot3(float c0, float c1, float c2, float x, float y, float z) {
   return __fmaf_rn(c2, z, __fmaf_rn(c1, y, __fmul_rn(c0, x)));
+}
+__device__ __forceinline__ float* write_obs_row(float* obs, const int& ob_dim, int env, const float* q, const float* v, int nq, int lane) {
+  float qw = q[3], qx = q[4], qy = q[5], qz = q[6];
+  const float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
+  qw *= inv; qx *= inv; qy *= inv; qz *= inv;
+  float* o = obs + (size_t)env * ob_dim;   // after the quaternion loads: the other order costs the 72-register instances spill reloads
+  const int nj = nq - 7;
+  if (lane == 0) o[0] = q[2];
+  if (lane < 3) {
+    float c0, c1, c2;
+    obs_rot_column(qw, qx, qy, qz, lane, c0, c1, c2);
+    o[1 + lane] = c2;
+    o[4 + nj + lane] = obs_dot3(c0, c1, c2, v[0], v[1], v[2]);
+    o[7 + nj + lane] = obs_dot3(c0, c1, c2, v[3], v[4], v[5]);
+  }
+#pragma unroll 1
+  for (int i = lane; i < nj; i += 32) { o[4 + i] = q[7 + i]; o[10 + nj + i] = v[6 + i]; }
+  return o;
 }
 
 // ------------------------------------------------------------------ terrain --------------------
@@ -561,7 +580,9 @@ __device__ __forceinline__ int stage_b_narrow_phase(const TerrainDesc& ter, cons
         }
       }
     }
-    // ---- this slot's direct hits go to the list at once (nothing of them stays in registers across the sphere groups)
+    // ---- this slot's direct hits go to the list at once (nothing of them stays in registers across the sphere groups).  The three
+    // appends of this function stay written out: one shared helper raised the spill stores of the one-slot 14- and 28-warp instances
+    // from 252-308 to 358-414 bytes (-Xptxas -v)
     {
       const unsigned hmask = __ballot_sync(FULL, hit);
       if (hit) {
@@ -682,62 +703,108 @@ __device__ __forceinline__ int stage_b_narrow_phase(const TerrainDesc& ter, cons
   return total;
 }
 
-// Stage C, generic instance: the second half of a self contact's column (row c) -- the ordinary compact-by-depth column Y = L^-T J^T of
-// the point pos on the chain of dof i0 (the pair's second body; -1 = welded to the world: a zero column), base columns included -- into
-// Y2; jv = J v and yz = Y . z of that half.  The same arithmetic as the first half in the kernel.
-__device__ __forceinline__ void self_second_column(float* Y2, int c, f3 pos, f3 axd, f3 O, int i0, int floating, int nbase, int nvp, int DLP, int nbp,
-                                                   const int* ddepth, const int* danc, const int* dbody, const int* bodyi, const float* s_pose,
-                                                   const float* s_gv, const float* s_L, const float* s_invd, const float* s_z, float& jv, float& yz) {
-  jv = 0.f; yz = 0.f;
-  const int m = i0 >= 0 ? ddepth[i0] : -1;
-  if (m < 0) return;
-  if (floating) {
-    const f3 rc = cross(pos - O, axd);
-    Y2[0 * CP + c] = axd.x; Y2[1 * CP + c] = axd.y; Y2[2 * CP + c] = axd.z;
-    Y2[3 * CP + c] = rc.x; Y2[4 * CP + c] = rc.y; Y2[5 * CP + c] = rc.z;
-    jv = axd.x * s_gv[0] + axd.y * s_gv[1] + axd.z * s_gv[2] + rc.x * s_gv[3] + rc.y * s_gv[4] + rc.z * s_gv[5];
-  }
-#pragma unroll 1
-  for (int t = nbase; t <= m; t++) {
-    const int a_t = danc[t * nvp + i0], j = dbody[a_t];
-    const f3 aj = mk(s_pose[(PF_A + 0) * nbp + j], s_pose[(PF_A + 1) * nbp + j], s_pose[(PF_A + 2) * nbp + j]);
-    f3 col = aj;
-    if (bodyi[BF_JTYPE * nbp + j] == 1) {
-      const f3 pj = mk(s_pose[(PF_P + 0) * nbp + j], s_pose[(PF_P + 1) * nbp + j], s_pose[(PF_P + 2) * nbp + j]);
-      col = cross(aj, pos - pj);
+// Stage C, static humanoid and generic instances: the compact-by-depth column Y = L^-T J^T of constraint row c along the chain of dof i0
+// (depth m; -1 = a body welded to the world: a zero column), into column c of Y, and yz = Y . z.  fill: J is the direction axd at the
+// point pos (base columns included), and jv += J v; otherwise the caller has put J into Y and jv.  The generic instance also computes
+// the second half of a self contact's column with it (the chain of the pair's second body).
+template <int UNR>
+__device__ __forceinline__ void chain_column(float* Y, int c, bool fill, f3 pos, f3 axd, f3 O, int i0, int m, int floating, int nbase, int nvp,
+                                             int DLP, int nbp, const int* danc, const int* dbody, const int* bodyi, const float* s_pose,
+                                             const float* s_gv, const float* s_L, const float* s_invd, const float* s_z, float& jv, float& yz) {
+  if (fill) {
+    if (floating) {
+      const f3 rc = cross(pos - O, axd);
+      Y[0 * CP + c] = axd.x; Y[1 * CP + c] = axd.y; Y[2 * CP + c] = axd.z;
+      Y[3 * CP + c] = rc.x; Y[4 * CP + c] = rc.y; Y[5 * CP + c] = rc.z;
+      jv = axd.x * s_gv[0] + axd.y * s_gv[1] + axd.z * s_gv[2] + rc.x * s_gv[3] + rc.y * s_gv[4] + rc.z * s_gv[5];
     }
-    const float val = dot(col, axd);
-    Y2[t * CP + c] = val;
-    jv += val * s_gv[a_t];
+#pragma unroll (UNR > 1 ? 2 : 1)
+    for (int t = nbase; t <= m; t++) {
+      const int a_t = danc[t * nvp + i0], j = dbody[a_t];
+      const f3 aj = mk(s_pose[(PF_A + 0) * nbp + j], s_pose[(PF_A + 1) * nbp + j], s_pose[(PF_A + 2) * nbp + j]);
+      f3 col = aj;
+      if (bodyi[BF_JTYPE * nbp + j] == 1) {
+        const f3 pj = mk(s_pose[(PF_P + 0) * nbp + j], s_pose[(PF_P + 1) * nbp + j], s_pose[(PF_P + 2) * nbp + j]);
+        col = cross(aj, pos - pj);
+      }
+      const float val = dot(col, axd);
+      Y[t * CP + c] = val;
+      jv += val * s_gv[a_t];
+    }
   }
+  yz = 0.f;
 #pragma unroll 1
   for (int sI = m; sI >= 0; sI--) {
     const int a_s = danc[sI * nvp + i0];
-    const float y = Y2[sI * CP + c] * s_invd[a_s];
-    Y2[sI * CP + c] = y;
+    const float y = Y[sI * CP + c] * s_invd[a_s];
+    Y[sI * CP + c] = y;
     yz += y * s_z[a_s];
-#pragma unroll 1
-    for (int t = 0; t < sI; t++) Y2[t * CP + c] -= s_L[a_s * DLP + t] * y;
+#pragma unroll (UNR)
+    for (int t = 0; t < sI; t++) Y[t * CP + c] -= s_L[a_s * DLP + t] * y;
+  }
+}
+
+// Stage C, static humanoid and generic instances: subtracts the bias of constraint row c from its velocity u_c: ERP on a joint-limit
+// violation (lm) or on a contact's depth (ct, normal rows, d == 2), plus restitution on a normal approach speed jv beyond
+// rest_threshold.  The quadruped instance keeps the same lines inline (see there).
+__device__ __forceinline__ void apply_row_bias(float& u_c, const rsb_params& prm, bool is_lim, int d, const float* lm, const float* ct, float jv) {
+  if (is_lim) u_c -= prm.erp * lm[2] / prm.dt;
+  else if (d == 2) {
+    float target = prm.erp * ct[CF_DEPTH] / prm.dt;
+    if (prm.restitution > 0.f && jv < -prm.rest_threshold) target += -prm.restitution * jv;
+    u_c -= target;
+  }
+}
+
+// Stage E, static humanoid and generic instances: adds Y[di] . lam of the contacts whose column block Y (rows 3k..3k+2) lies on a chain
+// through dof i (depth di) to sacc; SECOND: the self contacts' second halves (the chain of the pair's second body), subtracted
+template <int UNR, bool SECOND>
+__device__ __forceinline__ void chain_gather(float& sacc, const float* Y, const float* s_lam, const float* s_ct, int K, int i, int di, const int* bdof,
+                                             const int* ddepth, const int* danc, int nvp) {
+#pragma unroll (UNR)
+  for (int k = 0; k < K; k++) {
+    int i0;
+    if (SECOND) {
+      const int pr = __float_as_int(s_ct[k * CT_WORDS + CF_PAIR]);
+      i0 = pr < 0 ? bdof[-1 - pr] : -1;
+    } else {
+      i0 = bdof[__float_as_int(s_ct[k * CT_WORDS + CF_BODY])];
+    }
+    if (i0 >= 0 && ddepth[i0] >= di && danc[di * nvp + i0] == i) {
+      const float y = Y[di * CP + 3 * k] * s_lam[3 * k] + Y[di * CP + 3 * k + 1] * s_lam[3 * k + 1] + Y[di * CP + 3 * k + 2] * s_lam[3 * k + 2];
+      if (SECOND) sacc -= y;
+      else sacc += y;
+    }
   }
 }
 
 // ------------------------------------------------------------------ the kernel -----------------
-// SNB > 0: compiled for the model dimensions (SNB, SNQ, SNV, SFL, SMAXDEPTH, SMAXDD) -- every table and
-// workspace offset is an immediate.  SNB == 0: generic, dimensions read from the blob header.
-template <int WPC, int SLOTS, int SNB, int SNQ, int SNV, int SFL, int SMAXDEPTH, int SMAXDD>
+// The compiled instances (SPEC, the value rsb_internal_launch_instance reports).  The generic instance reads the model dimensions from
+// the blob header and is the only one that runs self-collision pairs; the others have the dimensions of SPEC_DIMS compiled in, so every
+// table and workspace offset is an immediate.  pick_config (batch.cu) takes a static instance for a model of exactly its dimensions:
+// every 12-joint quadruped (ANYmal, A1, Go1, ...) whose parent table is base + 4 chains of 3, and the Atlas-like humanoid.
+enum Spec { SPEC_GENERIC = 0, SPEC_QUAD = 1, SPEC_HUMANOID = 2, SPEC_COUNT = 3 };
+constexpr Dims SPEC_DIMS[SPEC_COUNT] = {{0, 0, 0, 0, 0, 0}, {13, 19, 18, 1, 3, 8}, {31, 37, 36, 1, 10, 15}};
+__host__ __device__ constexpr bool operator==(const Dims& a, const Dims& b) {
+  return a.nb == b.nb && a.nq == b.nq && a.nv == b.nv && a.floating == b.floating && a.maxdepth == b.maxdepth && a.maxdd == b.maxdd;
+}
+
+template <int WPC, int SLOTS, int SPEC>
 __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel(const __grid_constant__ StepArgs args) {
   extern __shared__ __align__(128) uint32_t smem[];
   __shared__ __align__(8) uint64_t tma_bar;
   const int lane = threadIdx.x & 31;     // (re-read wherever needed at 72 registers; S2R SR_LANEID instead, with or without a range assumption, measured 12 % slower)
   // the shuffle marks the warp index as warp-uniform for the compiler: the workspace base then lives in a uniform register
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  constexpr bool ST = SNB > 0;
-  // every 12-joint quadruped: the host selects this instance only when the parent table is base + 4 chains of 3 (pick_config)
-  constexpr bool QUAD = SNB == 13 && SNQ == 19 && SNV == 18 && SFL == 1 && SMAXDEPTH == 3 && SMAXDD == 8;
+  constexpr bool SELF = SPEC == SPEC_GENERIC;   // dimensions from the blob header; self-collision pairs
+  constexpr bool ST = !SELF;                    // dimensions compiled in
+  constexpr bool QUAD = SPEC == SPEC_QUAD;      // the 4 x 3-chain topology compiled in as well
   // deep trees on few resident warps (the humanoid instance: 14 warps per SM, latency-bound) get their dependent shared-memory loops of
   // stage C unrolled for memory-level parallelism; everything else keeps them rolled (instruction cache)
-  constexpr int UNR = (ST && !QUAD && SMAXDD >= 12) ? 4 : 1;
-  constexpr Dims SD{SNB, SNQ, SNV, SFL, SMAXDEPTH, SMAXDD};
+  constexpr int UNR = SPEC == SPEC_HUMANOID ? 4 : 1;
+  constexpr Dims SD = SPEC_DIMS[SPEC];
+  // lanes >= nb hold exact zeros in stage A's root sum: with at most 16 bodies its xor-16 butterfly step adds 0 and is skipped
+  constexpr int ROOT_XOR = (ST && SD.nb <= 16) ? 8 : 16;
   constexpr WsLayout LS = make_ws_layout(SD);
   constexpr BlobHeader HS = make_blob_header(SD, 0, 0);
 #define WSO(f) (ST ? LS.f : args.ws.f)
@@ -1040,9 +1107,8 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 #pragma unroll
           for (int k = 0; k < 16; k++) {
             float t = X[k];
-            // lanes >= nb hold exact zeros (zero mass and inertia): with at most 16 bodies the xor-16 step adds 0 and is skipped
 #pragma unroll
-            for (int o = (ST && SNB <= 16) ? 8 : 16; o > 0; o >>= 1) t += __shfl_xor_sync(FULL, t, o);
+            for (int o = ROOT_XOR; o > 0; o >>= 1) t += __shfl_xor_sync(FULL, t, o);
             T[k] = t;
           }
           if (b == 0) {
@@ -1106,7 +1172,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       if (args.phase_mask & PHASE_KINEMATICS) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // kinematics for the getters only
 
       // =========================== stage B: narrow phase ========================================
-      K = stage_b_narrow_phase<SLOTS, !ST>(args.ter, s_ter, blob_s, s_pose, s_ct, s_Y, env, lane, nbp, args.prof ? args.prof + ((size_t)env * 4 + (sub & 3)) * 8 : nullptr);
+      K = stage_b_narrow_phase<SLOTS, SELF>(args.ter, s_ter, blob_s, s_pose, s_ct, s_Y, env, lane, nbp, args.prof ? args.prof + ((size_t)env * 4 + (sub & 3)) * 8 : nullptr);
       const int C = 3 * K;
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 2] = (unsigned)clock64();
       if (args.phase_mask & PHASE_NO_UPDATE) { asm volatile("cp.async.wait_all;" ::: "memory"); __syncwarp(); break; }   // integrate1(): kinematics, collision, M, h only
@@ -1346,6 +1412,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 #pragma unroll
           for (int t = 0; t < 9; t++) if (t <= m) s_Y[t * CP + c] = y[t];
           u_c = jv + args.prm.dt * yz;
+          // apply_row_bias, written out: calling it here changes this instance's code (the headline's) without saving anything
           if (is_lim) u_c -= args.prm.erp * lm[2] / args.prm.dt;
           else if (d == 2) {
             float target = args.prm.erp * ct[CF_DEPTH] / args.prm.dt;
@@ -1365,83 +1432,31 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           const f3 pos = mk(ct[CF_POS], ct[CF_POS + 1], ct[CF_POS + 2]);
           const int i0 = is_lim ? __float_as_int(lm[0]) : bdof[__float_as_int(ct[CF_BODY])];
           const int m = i0 >= 0 ? ddepth[i0] : -1;
-          float jv = 0.f;
+          float jv = 0.f, yz;
           if (is_lim) {   // J = sign * e_dof
   #pragma unroll 1
             for (int t = 0; t < m; t++) s_Y[t * CP + c] = 0.f;
             s_Y[m * CP + c] = lm[1];
             jv = lm[1] * s_gv[i0];
-          } else {
-            if (floating) {
-              f3 rc = cross(pos - O, axd);
-              s_Y[0 * CP + c] = axd.x; s_Y[1 * CP + c] = axd.y; s_Y[2 * CP + c] = axd.z;
-              s_Y[3 * CP + c] = rc.x; s_Y[4 * CP + c] = rc.y; s_Y[5 * CP + c] = rc.z;
-              jv = axd.x * s_gv[0] + axd.y * s_gv[1] + axd.z * s_gv[2] + rc.x * s_gv[3] + rc.y * s_gv[4] + rc.z * s_gv[5];
-            }
-  #pragma unroll (UNR > 1 ? 2 : 1)
-            for (int t = nbase; t <= m; t++) {
-              const int a_t = danc[t * nvp + i0], j = dbody[a_t];
-              f3 aj = mk(s_pose[(PF_A + 0) * nbp + j], s_pose[(PF_A + 1) * nbp + j], s_pose[(PF_A + 2) * nbp + j]);
-              f3 col = aj;
-              if (bodyi[BF_JTYPE * nbp + j] == 1) {
-                f3 pj = mk(s_pose[(PF_P + 0) * nbp + j], s_pose[(PF_P + 1) * nbp + j], s_pose[(PF_P + 2) * nbp + j]);
-                col = cross(aj, pos - pj);
-              }
-              float val = dot(col, axd);
-              s_Y[t * CP + c] = val;
-              jv += val * s_gv[a_t];
-            }
           }
-          float yz = 0.f;
-          if constexpr (ST && SMAXDD + 1 <= 9) {
-            // whole chain in registers (compile-time indices): 2 instructions per multiply-add instead of 4
-            constexpr int DLc = SMAXDD + 1;
-            float y[DLc];
-  #pragma unroll
-            for (int t = 0; t < DLc; t++) y[t] = (t <= m) ? s_Y[t * CP + c] : 0.f;
-  #pragma unroll
-            for (int sI = DLc - 1; sI >= 0; sI--) {
-              if (sI <= m) {
-                const int a_s = danc[sI * nvp + i0];
-                const float ys = y[sI] * s_invd[a_s];
-                y[sI] = ys;
-                yz += ys * s_z[a_s];
-  #pragma unroll
-                for (int t = 0; t < sI; t++) y[t] -= s_L[a_s * DLP + t] * ys;
-              }
-            }
-  #pragma unroll
-            for (int t = 0; t < DLc; t++) if (t <= m) s_Y[t * CP + c] = y[t];
-          } else {
-  #pragma unroll 1
-            for (int sI = m; sI >= 0; sI--) {
-              const int a_s = danc[sI * nvp + i0];
-              float y = s_Y[sI * CP + c] * s_invd[a_s];
-              s_Y[sI * CP + c] = y;
-              yz += y * s_z[a_s];
-  #pragma unroll (UNR)
-              for (int t = 0; t < sI; t++) s_Y[t * CP + c] -= s_L[a_s * DLP + t] * y;
-            }
-          }
+          chain_column<UNR>(s_Y, c, !is_lim, pos, axd, O, i0, m, floating, nbase, nvp, DLP, nbp, danc, dbody, bodyi, s_pose, s_gv, s_L, s_invd, s_z, jv, yz);
           u_c = jv + args.prm.dt * yz;
-          if constexpr (!ST) {
+          if constexpr (SELF) {
             // self contact: the column is Y_first - Y_second; the second half (the second body's chain column at the same point, base
-            // columns included) goes to its own block s_Y2, and u_c, the relative velocity jv, are differences of the two halves
+            // columns included) goes to its own block s_Y2, and u_c, the relative velocity jv, are differences of the two halves.  A body
+            // welded to the world (fixed base only) has no dof: m = -1 and no base columns, a zero column.
             const int pair = __float_as_int(ct[CF_PAIR]);
             if (!is_lim && pair < 0) {
               float* s_Y2 = ws + args.ws.words - self_y_words(maxdd);
-              float jv2 = 0.f, yz2 = 0.f;
-              self_second_column(s_Y2, c, pos, axd, O, bdof[-1 - pair], floating, nbase, nvp, DLP, nbp, ddepth, danc, dbody, bodyi, s_pose, s_gv, s_L, s_invd, s_z, jv2, yz2);
+              const int i2 = bdof[-1 - pair];
+              float jv2 = 0.f, yz2;
+              chain_column<1>(s_Y2, c, true, pos, axd, O, i2, i2 >= 0 ? ddepth[i2] : -1, floating, nbase, nvp, DLP, nbp, danc, dbody, bodyi, s_pose, s_gv,
+                              s_L, s_invd, s_z, jv2, yz2);
               u_c -= jv2 + args.prm.dt * yz2;
               jv -= jv2;
             }
           }
-          if (is_lim) u_c -= args.prm.erp * lm[2] / args.prm.dt;
-          else if (d == 2) {
-            float target = args.prm.erp * ct[CF_DEPTH] / args.prm.dt;
-            if (args.prm.restitution > 0.f && jv < -args.prm.rest_threshold) target += -args.prm.restitution * jv;
-            u_c -= target;
-          }
+          apply_row_bias(u_c, args.prm, is_lim, d, lm, ct, jv);
         }
       }
       iters = 0; resid = 0.f; gs_status = RSB_SOLVER_CONVERGED;
@@ -1483,7 +1498,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
                 float sacc = 0.f;
   #pragma unroll (UNR)
                 for (int t = 0; t <= tmax; t++) sacc += s_Y[t * CP + a] * s_Y[t * CP + bcol];
-                if constexpr (!ST) {
+                if constexpr (SELF) {
                   // self contacts: G_ab = (Y1_a - Y2_a) . (Y1_b - Y2_b), each product along the two chains' common part (lcad)
                   if (H.npairs > 0) {
                     const float* s_Y2 = ws + args.ws.words - self_y_words(maxdd);
@@ -1519,7 +1534,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           float id = 1.0f / (a * c00 + bq * c01 + cc * c02);
           float* o = s_u + CB_WORDS * lane;
           float pm;
-          if constexpr (!ST) {   // a self contact (candidate npts + j) takes the friction of its pair
+          if constexpr (SELF) {   // a self contact (candidate npts + j) takes the friction of its pair
             const int cand = __float_as_int(s_ct[lane * CT_WORDS + CF_PT]);
             pm = cand < H.npts ? ptsf[5 * H.nptp + cand] : reinterpret_cast<const float*>(blob_s + H.off_pair)[PAIR_WORDS * (cand - H.npts) + PR_MU];
           } else {
@@ -1582,24 +1597,10 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         for (int i = lane; i < nv; i += 32) {   // w = dt z + Y lam, gathered per dof over the contacts whose chain holds it
           float sacc = args.prm.dt * s_z[i];
           const int di = ddepth[i];
-  #pragma unroll (UNR)
-          for (int k = 0; k < K; k++) {
-            const int i0 = bdof[__float_as_int(s_ct[k * CT_WORDS + CF_BODY])];
-            if (i0 >= 0 && ddepth[i0] >= di && danc[di * nvp + i0] == i)
-              sacc += s_Y[di * CP + 3 * k] * s_lam[3 * k] + s_Y[di * CP + 3 * k + 1] * s_lam[3 * k + 1] + s_Y[di * CP + 3 * k + 2] * s_lam[3 * k + 2];
-          }
-          if constexpr (!ST) {
+          chain_gather<UNR, false>(sacc, s_Y, s_lam, s_ct, K, i, di, bdof, ddepth, danc, nvp);
+          if constexpr (SELF) {
             // self contacts: the second body's half of the column with -lambda
-            if (H.npairs > 0) {
-              const float* s_Y2 = ws + args.ws.words - self_y_words(maxdd);
-  #pragma unroll 1
-              for (int k = 0; k < K; k++) {
-                const int pr = __float_as_int(s_ct[k * CT_WORDS + CF_PAIR]);
-                const int i2 = pr < 0 ? bdof[-1 - pr] : -1;
-                if (i2 >= 0 && ddepth[i2] >= di && danc[di * nvp + i2] == i)
-                  sacc -= s_Y2[di * CP + 3 * k] * s_lam[3 * k] + s_Y2[di * CP + 3 * k + 1] * s_lam[3 * k + 1] + s_Y2[di * CP + 3 * k + 2] * s_lam[3 * k + 2];
-              }
-            }
+            if (H.npairs > 0) chain_gather<1, true>(sacc, ws + args.ws.words - self_y_words(maxdd), s_lam, s_ct, K, i, di, bdof, ddepth, danc, nvp);
           }
   #pragma unroll 1
           for (int l = 0; l < Lm; l++) {
@@ -1713,22 +1714,8 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 #pragma unroll 1
       for (int i = lane; i < nv; i += 32) { g_gv[i] = s_gv[i]; args.tau_applied[(size_t)env * args.gv_stride + i] = s_b[i]; }
     }
-    if (args.obs && floating) {   // VectorizedEnvironment::observe() fused into the step: [z, R^T e_z, q_j, R^T v, R^T w, qdot_j]
-      float qw = s_gc[3], qx = s_gc[4], qy = s_gc[5], qz = s_gc[6];
-      const float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
-      qw *= inv; qx *= inv; qy *= inv; qz *= inv;
-      float* o = args.obs + (size_t)env * args.ob_dim;
-      const int nj = nq - 7;
-      if (lane == 0) o[0] = s_gc[2];
-      if (lane < 3) {   // same arithmetic as rsb_observe_kernel (aux_kernels.cuh)
-        float c0, c1, c2;
-        obs_rot_column(qw, qx, qy, qz, lane, c0, c1, c2);
-        o[1 + lane] = c2;
-        o[4 + nj + lane] = obs_dot3(c0, c1, c2, s_gv[0], s_gv[1], s_gv[2]);
-        o[7 + nj + lane] = obs_dot3(c0, c1, c2, s_gv[3], s_gv[4], s_gv[5]);
-      }
-#pragma unroll 1
-      for (int i = lane; i < nj; i += 32) { o[4 + i] = s_gc[7 + i]; o[10 + nj + i] = s_gv[6 + i]; }
+    if (args.obs && floating) {   // VectorizedEnvironment::observe() fused into the step
+      const float* o = write_obs_row(args.obs, args.ob_dim, env, s_gc, s_gv, nq, lane);
       if (args.peer_world > 0) {   // fused all-gather: the finished row goes to every GPU of the job (this one included) over NVLink
         __syncwarp();
         const size_t row = ((size_t)args.peer_rank * args.num_envs + env) * args.ob_dim;

@@ -329,6 +329,41 @@ def setup_batch(capi, urdf, n, seed, terrain="ground", base_z=0.45, vel=0.5, tau
     return t, bt, o64, o32, gc32.astype(np.float64), gv32.astype(np.float64), tau32.astype(np.float64)
 
 
+# Contact row bias on: ERP pushes penetrations and joint-limit violations out, restitution reflects approach speeds beyond
+# rest_threshold.  The tests that run with it check that the threshold splits the contacts (normal_speeds).
+ROW_BIAS = dict(erp=0.02, restitution=0.4, rest_threshold=0.2)
+
+
+def normal_speeds(t, gc, gv, d):
+    """J_n v of every terrain contact of the oracle's debug output d at the state (gc, gv) it stepped from (nan elsewhere): the approach
+    speed that the restitution switch compares with -rest_threshold"""
+    n, K = d["c_pt"].shape
+    out = np.full((n, K), np.nan)
+    for e in range(n):
+        R, p, a = fk_numpy(t, gc[e])
+        for k in range(d["ncontacts"][e]):
+            if d["c_pair"][e, k] < 0:
+                continue
+            x = d["c_pos"][e, k]
+            v = gv[e, 0:3] + np.cross(gv[e, 3:6], x - p[0]) if t["floating"] else np.zeros(3)
+            j = d["c_body"][e, k]
+            while t["parent"][j] >= 0:
+                v = v + gv[e, t["vidx"][j]] * (np.cross(a[j], x - p[j]) if t["jtype"][j] == 1 else a[j])
+                j = t["parent"][j]
+            out[e, k] = d["c_normal"][e, k] @ v
+    return out
+
+
+def check_restitution_split(vn, rest_threshold):
+    """the restitution switch is taken for some contacts and not for others, and no approach speed lies so close to the threshold that
+    float32 rounding of the state could flip the switch"""
+    vn = vn[np.isfinite(vn)]
+    print(f"approach speeds beyond the restitution threshold: {int((vn < -rest_threshold).sum())} of {vn.size}, closest "
+          f"{np.abs(vn + rest_threshold).min():.1e} m/s")
+    assert (vn < -rest_threshold).sum() > 10 and (vn > -rest_threshold).sum() > 10
+    assert np.abs(vn + rest_threshold).min() > 1e-4
+
+
 def index_parity(pts_gpu, cnt_gpu, d_ref, label):
     """bit-exact contact lists, excluding environments that hold a candidate inside the margin."""
     n = len(cnt_gpu)

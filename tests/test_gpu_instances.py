@@ -12,8 +12,8 @@ import os
 import numpy as np
 import pytest
 
-from helpers import (ANYMAL_GC0, QUAD_FEET, QUAD_PRISMATIC, QUAD_BRANCHED, HEXAPOD, MAX32, MARGIN, THRESH, setup_batch, index_parity,
-                     launch_config)
+from helpers import (ANYMAL_GC0, QUAD_FEET, QUAD_PRISMATIC, QUAD_BRANCHED, HEXAPOD, MAX32, MARGIN, THRESH, ROW_BIAS, setup_batch, index_parity,
+                     launch_config, normal_speeds, check_restitution_split)
 from oracle.oracle import Oracle
 from oracle.urdf_tables import load_tables
 
@@ -93,14 +93,14 @@ def _pd(t, n, gc0, rng):
     return kp, kd, pt.astype(np.float32)
 
 
-def _batch(capi, monkeypatch, name, n, terrain, seed, wpc=None):
+def _batch(capi, monkeypatch, name, n, terrain, seed, wpc=None, params=None):
     urdf, generic, inst, base_z, q = CASES[name]
     monkeypatch.setenv("RSB_FORCE_GENERIC", "1" if generic else "0")
     if wpc is None:
         monkeypatch.delenv("RSB_FORCE_WPC", raising=False)
     else:
         monkeypatch.setenv("RSB_FORCE_WPC", str(wpc))
-    t, bt, o64, o32, _, _, _ = setup_batch(capi, urdf, n, seed, terrain=terrain, tau_scale=0.0)
+    t, bt, o64, o32, _, _, _ = setup_batch(capi, urdf, n, seed, terrain=terrain, tau_scale=0.0, params=params)
     cfg = launch_config(capi, bt)
     assert (cfg["spec"], cfg["slots"]) == inst, f"{name}: runs instance {cfg}, expected (spec, slots) = {inst}"
     rng = np.random.default_rng(seed + 1)
@@ -151,13 +151,17 @@ def test_instance_stage_outputs(capi, monkeypatch, name):
     assert np.allclose(M, np.transpose(M, (0, 2, 1)))
 
 
-@pytest.mark.parametrize("terrain", ["ground", "hm"])
-@pytest.mark.parametrize("name", list(CASES))
-def test_instance_step_and_trajectory(capi, monkeypatch, name, terrain):
+# every case on both terrains, and the row bias of stage C (ERP, restitution) on the humanoid and a generic instance
+STEP_CASES = [pytest.param(name, terrain, None, id=f"{name}-{terrain}") for name in CASES for terrain in ("ground", "hm")] + [
+    pytest.param("atlas", "ground", ROW_BIAS, id="atlas-ground-bias"), pytest.param("anymal_generic", "hm", ROW_BIAS, id="anymal_generic-hm-bias")]
+
+
+@pytest.mark.parametrize("name,terrain,bias", STEP_CASES)
+def test_instance_step_and_trajectory(capi, monkeypatch, name, terrain, bias):
     """one step (contact lists, state, impulses, complementarity) and 10 steps (state) against the oracle, PD targets on, joints at
     their stops and actuators at their effort limits"""
     n = 256
-    t, bt, o64, o32, gc, gv, kp, kd, pt, cfg = _batch(capi, monkeypatch, name, n, terrain, seed=1000 + 17 * len(name) + (terrain == "hm"))
+    t, bt, o64, o32, gc, gv, kp, kd, pt, cfg = _batch(capi, monkeypatch, name, n, terrain, seed=1000 + 17 * len(name) + (terrain == "hm"), params=bias)
     ptd, vt = pt.astype(np.float64), np.zeros((n, t["nv"]))
     bt.integrate(1)
     g1, v1 = bt.get_state(); ct, cnt = bt.contacts(); pts = bt.contact_points(); st = bt.solver_status()
@@ -168,6 +172,8 @@ def test_instance_step_and_trajectory(capi, monkeypatch, name, terrain):
     assert np.isfinite(g1).all() and np.isfinite(v1).all()
     # the edges this test is meant to reach: contacts, joint-limit rows, saturated actuators
     assert cnt.sum() > n // 4 and d["nlimits"].sum() > 0 and _at_effort_limit(t, d["tau_applied"]).any()
+    if bias:
+        check_restitution_split(normal_speeds(t, gc, gv, d), bias["rest_threshold"])
     hard = index_parity(pts, cnt, d32, f"{name} {terrain}")
     # on the rough map two triangles sharing an edge can tie to 1e-6 m under different rounding
     # (test_heightmap_narrow_phase_matches_oracle_on_rough_terrain): at most one environment in 256

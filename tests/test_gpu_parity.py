@@ -14,7 +14,8 @@ import numpy as np
 import pytest
 
 from conftest import RSC
-from helpers import ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, MARGIN, THRESH, setup_batch, index_parity, launch_config
+from helpers import (ANYMAL_GC0, PENDULUM_URDF, SPHERE_URDF, BOX_URDF, MARGIN, THRESH, ROW_BIAS, setup_batch, index_parity, launch_config,
+                     normal_speeds, check_restitution_split)
 from oracle.oracle import Oracle
 from oracle.urdf_tables import load_tables
 
@@ -79,15 +80,16 @@ def test_contact_indices_bit_exact(capi, terrain):
         assert len(np.unique(ct["pair_index"][live])) > 100   # many different cells / both triangles
 
 
-@pytest.mark.parametrize("urdf,terrain,base_z,tau_scale", [
-    ("anymal_c_like.urdf", "ground", 0.45, 20.0),
-    ("anymal_c_like.urdf", "hm", 0.45, 20.0),
-    ("atlas_like.urdf", "ground", 0.9, 2.0),
+@pytest.mark.parametrize("urdf,terrain,base_z,tau_scale,bias", [
+    pytest.param("anymal_c_like.urdf", "ground", 0.45, 20.0, None, id="anymal_c_like.urdf-ground-0.45-20.0"),
+    pytest.param("anymal_c_like.urdf", "hm", 0.45, 20.0, None, id="anymal_c_like.urdf-hm-0.45-20.0"),
+    pytest.param("atlas_like.urdf", "ground", 0.9, 2.0, None, id="atlas_like.urdf-ground-0.9-2.0"),
+    pytest.param("anymal_c_like.urdf", "ground", 0.45, 20.0, ROW_BIAS, id="anymal_c_like.urdf-ground-0.45-20.0-bias"),
 ])
-def test_one_step_state_and_impulses(capi, urdf, terrain, base_z, tau_scale):
-    """a1 whole step from the same state: gc+, gv+ and contact impulses."""
+def test_one_step_state_and_impulses(capi, urdf, terrain, base_z, tau_scale, bias):
+    """a1 whole step from the same state: gc+, gv+ and contact impulses (bias: with ERP and restitution, on the quadruped instance)."""
     n = 512
-    t, bt, o64, o32, gc, gv, tau = _setup(capi, urdf, n, seed=31, terrain=terrain, base_z=base_z, tau_scale=tau_scale)
+    t, bt, o64, o32, gc, gv, tau = _setup(capi, urdf, n, seed=31, terrain=terrain, base_z=base_z, tau_scale=tau_scale, params=bias)
     bt.integrate(1)
     g1, v1 = bt.get_state()
     ct, cnt = bt.contacts()
@@ -95,6 +97,10 @@ def test_one_step_state_and_impulses(capi, urdf, terrain, base_z, tau_scale):
     it = bt.solver_iterations()
     a, b = gc.copy(), gv.copy()
     d = o64.step(a, b, tau_ff=tau, debug=True)
+    if bias:
+        assert launch_config(capi, bt)["spec"] == 1
+        assert d["nlimits"].sum() > 10                    # ERP on joint-limit rows as well
+        check_restitution_split(normal_speeds(t, gc, gv, d), bias["rest_threshold"])
     assert np.isfinite(g1).all() and np.isfinite(v1).all()
     # compare where both solvers converged on the same contact set; cycling Gauss-Seidel cases
     # (both sides hit max_iter; see DESIGN.md "solver convergence") have no unique answer

@@ -8,7 +8,7 @@ import subprocess
 import numpy as np
 import pytest
 
-from helpers import ANYMAL_GC0, MAX32, THRESH, setup_batch, index_parity, launch_config
+from helpers import ANYMAL_GC0, MAX32, THRESH, ROW_BIAS, setup_batch, index_parity, launch_config, check_restitution_split
 from test_self_collision_oracle import anymal_leg_pairs, crossed_anymal
 from oracle.self_oracle import SelfOracle, self_pair_tables
 from oracle.urdf_tables import load_tables
@@ -72,7 +72,7 @@ def _crossed(name, t, n, rng, z):
 CASES = {"anymal": ("anymal_c_like.urdf", anymal_leg_pairs(), 0.45), "atlas": ("atlas_like.urdf", ATLAS_PAIRS, 0.75)}
 
 
-def _setup(capi, monkeypatch, name, terrain, n, seed):
+def _setup(capi, monkeypatch, name, terrain, n, seed, params=None):
     """a batch with the case's pairs and the float64 / float32 self-collision oracles on the same terrain (a random 65 x 49 map for
     "hm"), the robots crossed (_crossed), joint torques zero"""
     urdf, pairs, z = CASES[name]
@@ -80,7 +80,7 @@ def _setup(capi, monkeypatch, name, terrain, n, seed):
     path = os.path.join(RSC, urdf)
     t = load_tables(path)
     bt = capi.Batch(capi.Model(path), n)
-    prm = dict(threshold=THRESH)
+    prm = dict(threshold=THRESH, **(params or {}))
     o64, o32 = SelfOracle(t, params=prm), SelfOracle(t, precision="f32", params=prm)
     bt.set_params(**prm)
     rng = np.random.default_rng(seed)
@@ -212,13 +212,13 @@ def _complementarity(t, ct, cnt, pts, d64, Jt, v_after, conv, mu=0.8):
     return worst_cone, worst_sig
 
 
-@pytest.mark.parametrize("terrain", ["ground", "hm"])
-@pytest.mark.parametrize("name", list(CASES))
-def test_self_collision_step_and_trajectory(capi, monkeypatch, name, terrain):
+@pytest.mark.parametrize("name,terrain,bias", [pytest.param(name, terrain, None, id=f"{name}-{terrain}") for name in CASES for terrain in ("ground", "hm")] +
+                         [pytest.param("atlas", "ground", dict(ROW_BIAS, rest_threshold=0.1), id="atlas-ground-bias")])   # some self contacts beyond it
+def test_self_collision_step_and_trajectory(capi, monkeypatch, name, terrain, bias):
     """one step and 10 steps against the float64 oracle within the bounds of tests/test_gpu_instances.py, Signorini and Coulomb on every
-    self contact"""
+    self contact (bias: with ERP and restitution, which a self contact takes on the difference of its two halves)"""
     n = 256
-    t, bt, o64, o32, gc, gv, cfg = _setup(capi, monkeypatch, name, terrain, n, seed=400 + (terrain == "hm"))
+    t, bt, o64, o32, gc, gv, cfg = _setup(capi, monkeypatch, name, terrain, n, seed=400 + (terrain == "hm"), params=bias)
     bt.set_control_mode(capi.FORCE_AND_TORQUE)
     bt.set_generalized_force(np.zeros((n, t["nv"]), np.float32))
     zero = np.zeros((n, t["nv"]))
@@ -235,6 +235,10 @@ def test_self_collision_step_and_trajectory(capi, monkeypatch, name, terrain):
     scale_v = 1.0 + np.abs(b[conv])
     _, pj, Jt = o64.contact_jacobians(gc)
     assert np.array_equal(pj, d["c_pt"])
+    if bias:
+        vn = np.where(d["c_pt"] >= 0, np.einsum("evk,ev->ek", Jt[:, :, 2::3], gv), np.nan)       # terrain and self contacts
+        check_restitution_split(vn, bias["rest_threshold"])
+        assert (np.isfinite(vn) & (d["c_pair"] < 0) & (vn < -bias["rest_threshold"])).sum() >= 5
     worst_cone, worst_sig = _complementarity(t, ct, cnt, pts, d, Jt, v1.astype(np.float64), conv)
     bt.integrate(9)
     gN, _ = bt.get_state()
