@@ -209,6 +209,28 @@ int rsb_batch_get_diverged(rsb_batch* b, int32_t* flags, int env_begin, int env_
 #define RSB_SOLVER_MAXITER 3             /* max_iter sweeps without reaching the threshold                              */
 int rsb_batch_get_solver_status(rsb_batch* b, int32_t* status, int env_begin, int env_count, int where);
 int rsb_batch_get_solver_residual(rsb_batch* b, float* resid, int env_begin, int env_count, int where);              /* largest impulse update of the last sweep (< threshold: converged) */
+/* ---- frame kinematics (ArticulatedSystem::getFramePosition / getFrameOrientation / getFrameVelocity / getFrameAngularVelocity /
+ *      getDenseFrameJacobian for every environment at once).  The getters are lazy like rsb_batch_get_body_poses: they describe the
+ *      current state and run the kinematics pass only when the state changed through this API since the last one (one launch, plus
+ *      that pass when it is due).  They leave the contact records, solver outputs, diverged flags and applied torques of the last
+ *      integrate() as they were and have no effect on any later step.  After rsb_batch_integrate2() the getters' buffers hold the
+ *      poses from before that step (M and h stay those of integrate1()); the frame getters then run the kinematics pass for the
+ *      stepped state first, so poses and velocities always belong to one state, and M, h and the body poses describe it too from
+ *      then on.  Device buffers are tight rows, written in stream order.  Host buffers are written when the call returns; they are
+ *      staged through a device buffer of the batch sized to the largest host read so far (env_count * F floats times 18 for the
+ *      states, times 6 * nv for the Jacobians), kept until the batch is destroyed: device buffers avoid it. */
+#define RSB_MAX_FRAMES 64
+/* Frames rigidly attached to bodies, shared by all environments: body[n] (rsb_model_body_index order), pos[n][3] in the body frame,
+ * rot[n][9] row-major orientation in the body frame (NULL = identity).  rsb_model_frame() returns exactly (body, pos, rot) for the
+ * URDF's link frames.  n = 0 clears.  A refused call (n < 0 or > RSB_MAX_FRAMES, a body out of range, NULL body or pos with n > 0)
+ * changes nothing. */
+int rsb_batch_set_frames(rsb_batch* b, const int32_t* body, const float* pos, const float* rot, int n);
+/* World frame, current state: pos [n][F][3], rot [n][F][9] (R_body * rot), lin_vel [n][F][3] (velocity of the frame's point),
+ * ang_vel [n][F][3] (angular velocity of its body).  A NULL output is skipped.  RSB_ERR_INVALID when no frames are set. */
+int rsb_batch_get_frame_states(rsb_batch* b, int env_begin, int env_count, float* pos, float* rot, float* lin_vel, float* ang_vel, int where);
+/* [n][F][6][nv] row-major: rows 0-2 translational (v_point = Jp gv), rows 3-5 rotational (omega = Jr gv).
+ * Columns follow the batch's gv order; for a floating base that is [v_world | omega_world | joints].  Non-ancestor columns are 0. */
+int rsb_batch_get_frame_jacobians(rsb_batch* b, int env_begin, int env_count, float* jac, int where);
 /* FK, M and h of the CURRENT state for the getters above, without touching the contact records of the last integrate()
  * (upstream's getters are lazy the same way).  The getters call it themselves when the state changed through this API;
  * call it explicitly after writing the state through rsb_batch_device_ptrs() views. */

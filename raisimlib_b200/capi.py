@@ -100,6 +100,7 @@ EXPORTED = [
     "rsb_batch_integrate1", "rsb_batch_integrate2", "rsb_batch_integrate",
     "rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities", "rsb_batch_get_body_poses", "rsb_batch_get_contacts",
     "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
+    "rsb_batch_set_frames", "rsb_batch_get_frame_states", "rsb_batch_get_frame_jacobians",
     "rsb_batch_ob_dim", "rsb_batch_observe", "rsb_batch_control_step",
     "rsb_batch_gym_configure", "rsb_batch_gym_reset", "rsb_batch_gym_step",
     "rsb_peer_buffer_create", "rsb_peer_buffer_open", "rsb_peer_buffer_close", "rsb_peer_buffer_destroy", "rsb_batch_set_observation_peers", "rsb_batch_wait_observation_peers",
@@ -171,6 +172,9 @@ def lib():
         L.rsb_batch_get_solver_residual.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
         L.rsb_batch_get_solver_status.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
         L.rsb_batch_update_kinematics.argtypes = [C.c_void_p]
+        L.rsb_batch_set_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        L.rsb_batch_get_frame_states.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_int]
+        L.rsb_batch_get_frame_jacobians.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
         L.rsb_batch_device_ptrs.argtypes = [C.c_void_p, C.POINTER(DeviceView)]
         L.rsb_batch_launch_count.argtypes = [C.c_void_p]
         L.rsb_batch_ob_dim.argtypes = [C.c_void_p]
@@ -276,6 +280,7 @@ class Batch:
         h = C.c_void_p()
         _ck(lib().rsb_batch_create(model.h, num_envs, device, C.byref(h)))
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
+        self.device, self.nframes = device, 0
 
     def __del__(self):
         if getattr(self, "h", None) and lib is not None and _lib is not None:
@@ -440,6 +445,64 @@ class Batch:
 
     def update_kinematics(self):
         _ck(lib().rsb_batch_update_kinematics(self.h))
+
+    # frame kinematics
+    def set_frames(self, body, pos, rot=None):
+        """frames rigidly attached to bodies, shared by all environments: body [F] indices, pos [F, 3] and rot [F, 3, 3] (None:
+        identity) in the body frame.  An empty list clears them; a refused call keeps the frames set before."""
+        bd = np.ascontiguousarray(body, np.int32).reshape(-1)
+        p = np.ascontiguousarray(pos, np.float32).reshape(-1, 3)
+        r = None if rot is None else np.ascontiguousarray(rot, np.float32).reshape(-1, 9)
+        if len(p) != len(bd) or (r is not None and len(r) != len(bd)):
+            raise ValueError(f"set_frames: {len(bd)} bodies, {len(p)} positions, {'no' if r is None else len(r)} rotations")
+        _ck(lib().rsb_batch_set_frames(self.h, bd.ctypes.data_as(C.c_void_p), p.ctypes.data_as(C.c_void_p),
+                                       None if r is None else r.ctypes.data_as(C.c_void_p), len(bd)))
+        self.nframes = len(bd)
+
+    def set_frames_by_name(self, names):
+        """the URDF link frames (or joint names) `names`, as rsb_model_frame gives them"""
+        L = lib()
+        body, pos, rot = [], np.zeros((len(names), 3)), np.zeros((len(names), 9))
+        for k, name in enumerate(names):
+            f, b = _ck(L.rsb_model_frame_index(self.model.h, name.encode())), C.c_int()
+            _ck(L.rsb_model_frame(self.model.h, f, C.byref(b), pos[k].ctypes.data_as(C.c_void_p), rot[k].ctypes.data_as(C.c_void_p)))
+            body.append(b.value)
+        self.set_frames(body, pos, rot)
+
+    def frame_states(self, env_begin=0, env_count=None):
+        """world-frame (pos [n, F, 3], rot [n, F, 3, 3], lin_vel [n, F, 3], ang_vel [n, F, 3]) of the frames at the current state"""
+        n = self._count(env_begin, env_count)
+        out = (np.empty((n, self.nframes, 3), np.float32), np.empty((n, self.nframes, 3, 3), np.float32),
+               np.empty((n, self.nframes, 3), np.float32), np.empty((n, self.nframes, 3), np.float32))
+        _ck(lib().rsb_batch_get_frame_states(self.h, env_begin, n, *[a.ctypes.data_as(C.c_void_p) for a in out], HOST))
+        return out
+
+    def frame_jacobians(self, env_begin=0, env_count=None):
+        """[n, F, 6, nv]: rows 0-2 the frame point's velocity, rows 3-5 its body's angular velocity per unit gv"""
+        return self._read(lib().rsb_batch_get_frame_jacobians, (self.nframes, 6, self.nv), np.float32, env_begin, env_count, range_first=True)
+
+    def _device_out(self, t, shape, name):
+        """device address of a caller-given output tensor (None: skip it)"""
+        if t is None:
+            return None
+        import torch
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+            raise ValueError(f"{name}: need a torch tensor on cuda:{self.device}")
+        if t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError(f"{name}: need a contiguous float32 tensor of shape {shape}, got {t.dtype} {tuple(t.shape)}")
+        return C.c_void_p(t.data_ptr())
+
+    def frame_states_into(self, pos=None, rot=None, lin_vel=None, ang_vel=None, env_begin=0, env_count=None):
+        """frame_states() written into torch CUDA tensors (None skips one), in the batch's stream order"""
+        n, F = self._count(env_begin, env_count), self.nframes
+        ptrs = [self._device_out(pos, (n, F, 3), "pos"), self._device_out(rot, (n, F, 3, 3), "rot"),
+                self._device_out(lin_vel, (n, F, 3), "lin_vel"), self._device_out(ang_vel, (n, F, 3), "ang_vel")]
+        _ck(lib().rsb_batch_get_frame_states(self.h, env_begin, n, *ptrs, DEVICE))
+
+    def frame_jacobians_into(self, jac, env_begin=0, env_count=None):
+        """frame_jacobians() written into a torch CUDA tensor [n, F, 6, nv], in the batch's stream order"""
+        n = self._count(env_begin, env_count)
+        _ck(lib().rsb_batch_get_frame_jacobians(self.h, env_begin, n, self._device_out(jac, (n, self.nframes, 6, self.nv), "jac"), DEVICE))
 
     def diverged(self, env_begin=0, env_count=None):
         return self._read(lib().rsb_batch_get_diverged, (), np.int32, env_begin, env_count)

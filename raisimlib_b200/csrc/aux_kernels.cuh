@@ -37,6 +37,92 @@ __global__ void rsb_ext_pack_kernel(float* rows, int body, const float* __restri
   r[7] = px; r[8] = py; r[9] = pz; r[10] = 0.f; r[11] = 0.f;
 }
 
+// ---- frame kinematics (rsb_batch_set_frames / get_frame_states / get_frame_jacobians) ----------------------------------------------
+// Frames rigidly attached to bodies and, per dof, what its Jacobian column needs; device arrays uploaded by rsb_batch_set_frames.
+// A dof turns or slides along the axis a of its body k (a = R_k axis: the joint frame's rotation about its own axis leaves the axis
+// where it is); the six dofs of a floating base are three slides and three turns about the world axes through the base origin, so
+// one column rule serves both: revolute (a x (x - p_k), a), prismatic (a, 0).
+enum FrameFlag { FRAME_AT_ORIGIN = 1, FRAME_IDENTITY = 2 };   // pos == 0 / rot == I exactly: the body pose is copied, bit for bit
+enum DofKind { DOF_WORLD_AXIS = 4 };                          // added to JT_REVOLUTE / JT_PRISMATIC: dof_axis is in the world frame
+struct FrameTable {
+  int nf, nb, nv;
+  const int* body;          // [nf] body index
+  const int* flags;         // [nf] FrameFlag bits
+  const float* pos;         // [nf][3] origin in the body frame
+  const float* rot;         // [nf][9] row-major orientation in the body frame
+  const int* dof_body;      // [nv] body whose joint carries the dof (the base for the base dofs)
+  const int* dof_kind;      // [nv] JT_REVOLUTE / JT_PRISMATIC (+ DOF_WORLD_AXIS)
+  const float* dof_axis;    // [nv][3] unit axis in the frame of dof_body (world frame with DOF_WORLD_AXIS)
+  const unsigned* anc;      // [nb] bit k: body k is the body itself or one of its ancestors
+};
+
+// One warp per (environment, frame), lanes over the dof columns: the Jacobian rows are written coalesced, and the frame velocity is
+// the warp sum of the same columns times gv, so lin_vel / ang_vel and J gv come from one routine.  Poses are the kinematics pass's
+// (R [N][nb][9], P [N][nb][3]); outputs are tight rows of the environments [env_begin, env_begin + count) in (environment, frame)
+// order; a null output is skipped.
+__global__ void __launch_bounds__(128) rsb_frame_kernel(FrameTable ft, const float* __restrict__ R, const float* __restrict__ P,
+                                                        const float* __restrict__ gv, int gv_stride, int env_begin, int count,
+                                                        float* pos_out, float* rot_out, float* lin_out, float* ang_out, float* jac_out) {
+  const int lane = threadIdx.x & 31;
+  const long w = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // output row: (environment - env_begin) * nf + frame
+  if (w >= (long)count * ft.nf) return;
+  const int f = (int)(w % ft.nf);
+  const long e = env_begin + w / ft.nf;
+  const int b = ft.body[f], flags = ft.flags[f];
+  const float* Rb = R + (e * ft.nb + b) * 9;
+  const float* pb = P + (e * ft.nb + b) * 3;
+  const float* fp = ft.pos + 3 * f;
+  float x[3];
+  #pragma unroll
+  for (int k = 0; k < 3; k++) x[k] = (flags & FRAME_AT_ORIGIN) ? pb[k] : pb[k] + (Rb[3 * k] * fp[0] + Rb[3 * k + 1] * fp[1] + Rb[3 * k + 2] * fp[2]);
+  if (pos_out && lane < 3) pos_out[w * 3 + lane] = lane == 0 ? x[0] : lane == 1 ? x[1] : x[2];
+  if (rot_out && lane < 9) {
+    const int i = lane / 3, j = lane % 3;
+    const float* fr = ft.rot + 9 * f;
+    rot_out[w * 9 + lane] = (flags & FRAME_IDENTITY) ? Rb[lane] : Rb[3 * i] * fr[j] + Rb[3 * i + 1] * fr[3 + j] + Rb[3 * i + 2] * fr[6 + j];
+  }
+  const unsigned anc = ft.anc[b];
+  const float* v = gv + e * gv_stride;
+  float lin[3] = {0.f, 0.f, 0.f}, ang[3] = {0.f, 0.f, 0.f};
+  for (int c = lane; c < ft.nv; c += 32) {
+    float jt[3] = {0.f, 0.f, 0.f}, jr[3] = {0.f, 0.f, 0.f};
+    const int k = ft.dof_body[c];
+    if ((anc >> k) & 1u) {
+      const int kind = ft.dof_kind[c];
+      const float* ax = ft.dof_axis + 3 * c;
+      const float* Rk = R + (e * ft.nb + k) * 9;
+      float a[3];
+      #pragma unroll
+      for (int q = 0; q < 3; q++) a[q] = (kind & DOF_WORLD_AXIS) ? ax[q] : Rk[3 * q] * ax[0] + Rk[3 * q + 1] * ax[1] + Rk[3 * q + 2] * ax[2];
+      if ((kind & 3) == JT_REVOLUTE) {
+        const float* pk = P + (e * ft.nb + k) * 3;
+        const float d0 = x[0] - pk[0], d1 = x[1] - pk[1], d2 = x[2] - pk[2];
+        jt[0] = a[1] * d2 - a[2] * d1; jt[1] = a[2] * d0 - a[0] * d2; jt[2] = a[0] * d1 - a[1] * d0;
+        jr[0] = a[0]; jr[1] = a[1]; jr[2] = a[2];
+      } else {
+        jt[0] = a[0]; jt[1] = a[1]; jt[2] = a[2];
+      }
+    }
+    const float vc = v[c];
+    #pragma unroll
+    for (int q = 0; q < 3; q++) { lin[q] += jt[q] * vc; ang[q] += jr[q] * vc; }
+    if (jac_out) {
+      float* J = jac_out + w * 6 * ft.nv + c;
+      #pragma unroll
+      for (int q = 0; q < 3; q++) { J[q * ft.nv] = jt[q]; J[(3 + q) * ft.nv] = jr[q]; }
+    }
+  }
+  if (!lin_out && !ang_out) return;
+  #pragma unroll
+  for (int s = 16; s > 0; s >>= 1)
+    #pragma unroll
+    for (int q = 0; q < 3; q++) { lin[q] += __shfl_xor_sync(0xffffffffu, lin[q], s); ang[q] += __shfl_xor_sync(0xffffffffu, ang[q], s); }
+  if (lane < 3) {
+    if (lin_out) lin_out[w * 3 + lane] = lane == 0 ? lin[0] : lane == 1 ? lin[1] : lin[2];
+    if (ang_out) ang_out[w * 3 + lane] = lane == 0 ? ang[0] : lane == 1 ? ang[1] : ang[2];
+  }
+}
+
 }  // namespace rsb
 
 // ---- RaisimGym ANYmal locomotion task on the device (SURVEY.md 8f N1; [RECALL] raisimGymTorch

@@ -48,6 +48,7 @@ struct rsb_batch {
   unsigned peer_epoch = 0;                // control steps signalled so far
   unsigned* peer_done = nullptr;          // device counter of finished CTAs (in-kernel arrival wait)
   bool kin_dirty = true;             // the getters' buffers (M, h, poses) do not describe the current state
+  bool kin_prestep = false;          // they were written by a full step (integrate2()) and hold stage A of the state before it
   unsigned* prof = nullptr;          // rsb_internal_set_profile
   unsigned* prof_a = nullptr;        // rsb_internal_set_profile_stage_a
   int* hmap_index = nullptr;         // terrain atlas: map index per environment
@@ -85,6 +86,11 @@ struct rsb_batch {
   bool gym_ready = false;
   float *gym_action = nullptr, *gym_obs = nullptr, *gym_reward = nullptr;
   unsigned char* gym_done = nullptr;
+  // frames of rsb_batch_set_frames (ftab.nf = 0: none): their table and the model's dof columns, in one device allocation
+  FrameTable ftab{};
+  int* frame_tab = nullptr;
+  float* frame_staging = nullptr;    // device rows of the frame getters for a host destination (the largest read so far)
+  size_t frame_staging_words = 0;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
@@ -360,8 +366,8 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   }
   if (e != cudaSuccess) return fail(RSB_ERR_CUDA, std::string("step kernel launch: ") + cudaGetErrorString(e));
   b->launches++;
-  if (!(phase_mask & PHASE_NO_UPDATE)) b->kin_dirty = !debug;   // the state advanced: M, h and poses are stale unless this launch refreshed them
-  else if (debug) b->kin_dirty = false;
+  if (!(phase_mask & PHASE_NO_UPDATE)) { b->kin_dirty = !debug; b->kin_prestep = debug; }   // the state advanced: M, h and poses are stale unless this launch refreshed them
+  else if (debug) { b->kin_dirty = false; b->kin_prestep = false; }
   if (phase_mask == 0) b->ext_active = false;   // an external wrench lasts for one integrate() call (upstream semantics)
   return RSB_OK;
 }
@@ -388,16 +394,17 @@ static int copy_out(rsb_batch* b, void* dst, const void* src, size_t bytes, int 
   if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
-// device rows of observations for a host destination
-static int ensure_obs_staging(rsb_batch* b) {
-  const size_t need = (size_t)b->N * rsb_batch_ob_dim(b);
-  if (b->obs_staging_words >= need) return RSB_OK;
-  if (b->obs_staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->obs_staging); }
-  b->obs_staging = nullptr; b->obs_staging_words = 0;
-  CK(cudaMalloc((void**)&b->obs_staging, need * 4));
-  b->obs_staging_words = need;
+// a device buffer of the batch that only grows: *buf holds at least `need` floats on return
+static int ensure_scratch(rsb_batch* b, float** buf, size_t* words, size_t need) {
+  if (*words >= need) return RSB_OK;
+  if (*buf) { CK(cudaStreamSynchronize(b->stream)); cudaFree(*buf); }
+  *buf = nullptr; *words = 0;
+  CK(cudaMalloc((void**)buf, need * 4));
+  *words = need;
   return RSB_OK;
 }
+// device rows of observations for a host destination
+static int ensure_obs_staging(rsb_batch* b) { return ensure_scratch(b, &b->obs_staging, &b->obs_staging_words, (size_t)b->N * rsb_batch_ob_dim(b)); }
 // device-side alias of a pinned, mapped host allocation (cudaHostAlloc / cudaHostRegister / torch pin_memory); null otherwise
 static const float* mapped_alias(const void* host) {
   cudaPointerAttributes at{};
@@ -576,7 +583,8 @@ void rsb_batch_destroy(rsb_batch* b) {
   if (b->stream) cudaStreamSynchronize(b->stream);
   for (void* p : {(void*)b->solver_status, (void*)b->resid, (void*)b->diverged, (void*)b->tau_applied, (void*)b->gc, (void*)b->gv, (void*)b->tau, (void*)b->pt, (void*)b->vt, (void*)b->ncontacts, (void*)b->contact_pt, (void*)b->iters,
                   (void*)b->contacts, (void*)b->dbg_M, (void*)b->dbg_h, (void*)b->dbg_R, (void*)b->dbg_p, (void*)b->hmap, (void*)b->staging, (void*)b->obs_staging, (void*)b->blob, (void*)b->gym_const, (void*)b->gym_action,
-                  (void*)b->gym_obs, (void*)b->gym_reward, (void*)b->gym_done, (void*)b->ext, (void*)b->hmap_index, (void*)b->peer_done})
+                  (void*)b->gym_obs, (void*)b->gym_reward, (void*)b->gym_done, (void*)b->ext, (void*)b->hmap_index, (void*)b->peer_done,
+                  (void*)b->frame_tab, (void*)b->frame_staging})
     if (p) cudaFree(p);
   if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
   delete b;
@@ -867,6 +875,95 @@ int rsb_batch_get_body_poses(rsb_batch* b, int env_begin, int env_count, float* 
   rc = ensure_kinematics(b); if (rc) return rc;
   rc = rot ? copy_out(b, rot, b->dbg_R + (size_t)env_begin * b->nb * 9, (size_t)env_count * b->nb * 9 * 4, where) : RSB_OK; if (rc) return rc;
   return pos ? copy_out(b, pos, b->dbg_p + (size_t)env_begin * b->nb * 3, (size_t)env_count * b->nb * 3 * 4, where) : RSB_OK;
+}
+
+// ---- frame kinematics: pose, velocity and Jacobian of frames rigidly attached to bodies, from the kinematics pass's poses ----------
+int rsb_batch_set_frames(rsb_batch* b, const int32_t* body, const float* pos, const float* rot, int n) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (n < 0 || n > RSB_MAX_FRAMES) return fail(RSB_ERR_INVALID, "at most " + std::to_string(RSB_MAX_FRAMES) + " frames per batch (got " + std::to_string(n) + ")");
+  if (n > 0 && (!body || !pos)) return fail(RSB_ERR_INVALID, "null frame body or position list");
+  for (int f = 0; f < n; f++)
+    if (body[f] < 0 || body[f] >= b->nb) return fail(RSB_ERR_INVALID, "frame " + std::to_string(f) + ": body index out of range (the model has " + std::to_string(b->nb) + ")");
+  if (n == 0) { b->ftab.nf = 0; return RSB_OK; }
+  const Model& md = b->model->md;
+  const int nb = md.nb, nv = md.nv, F = RSB_MAX_FRAMES;
+  // int words: body[F] | flags[F] | dof_body[nv] | dof_kind[nv] | anc[nb] | float words: pos[F][3] | rot[F][9] | dof_axis[nv][3]
+  const int o_flags = F, o_dbody = 2 * F, o_dkind = o_dbody + nv, o_anc = o_dkind + nv, o_pos = o_anc + nb, o_rot = o_pos + 3 * F, o_axis = o_rot + 9 * F;
+  const int words = o_axis + 3 * nv;
+  std::vector<int32_t> W(words, 0);
+  auto Fw = [&](int o, float v) { std::memcpy(&W[o], &v, 4); };
+  for (int f = 0; f < n; f++) {
+    W[f] = body[f];
+    int flags = (pos[3 * f] == 0.f && pos[3 * f + 1] == 0.f && pos[3 * f + 2] == 0.f) ? FRAME_AT_ORIGIN : 0;
+    bool ident = true;
+    for (int k = 0; k < 9; k++) {
+      const float r = rot ? rot[9 * f + k] : (k % 4 == 0 ? 1.f : 0.f);
+      ident = ident && r == (k % 4 == 0 ? 1.f : 0.f);
+      Fw(o_rot + 9 * f + k, r);
+    }
+    W[o_flags + f] = flags | (ident ? FRAME_IDENTITY : 0);
+    for (int k = 0; k < 3; k++) Fw(o_pos + 3 * f + k, pos[3 * f + k]);
+  }
+  if (md.floating)
+    for (int c = 0; c < 6; c++) {   // base: slides along, then turns about, the world axes through the base origin
+      W[o_dbody + c] = 0; W[o_dkind + c] = (c < 3 ? JT_PRISMATIC : JT_REVOLUTE) | DOF_WORLD_AXIS;
+      Fw(o_axis + 3 * c + c % 3, 1.f);
+    }
+  for (int i = 1; i < nb; i++) {
+    const int c = md.vidx[i];
+    W[o_dbody + c] = i; W[o_dkind + c] = md.jtype[i];
+    for (int k = 0; k < 3; k++) Fw(o_axis + 3 * c + k, (float)md.axis[3 * i + k]);
+  }
+  for (int i = 0; i < nb; i++) {
+    uint32_t m = 0;
+    for (int j = i; j >= 0; j = md.parent[j]) m |= 1u << j;
+    W[o_anc + i] = (int32_t)m;
+  }
+  CK(cudaSetDevice(b->device));
+  if (!b->frame_tab) CK(cudaMalloc((void**)&b->frame_tab, (size_t)words * 4));   // sized for RSB_MAX_FRAMES: the layout never moves
+  CK(cudaMemcpyAsync(b->frame_tab, W.data(), (size_t)words * 4, cudaMemcpyHostToDevice, b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  const int* T = b->frame_tab;
+  b->ftab = FrameTable{n, nb, nv, T, T + o_flags, (const float*)(T + o_pos), (const float*)(T + o_rot), T + o_dbody, T + o_dkind,
+                       (const float*)(T + o_axis), (const unsigned*)(T + o_anc)};
+  return RSB_OK;
+}
+// one launch of rsb_frame_kernel (after the kinematics pass when the poses are stale); out = {pos, rot, lin_vel, ang_vel, jac}
+static int frame_outputs(rsb_batch* b, int env_begin, int env_count, float* const out[5], int where) {
+  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  if (b->ftab.nf == 0) return fail(RSB_ERR_INVALID, "no frames: call rsb_batch_set_frames() first");
+  if (env_count == 0 || !(out[0] || out[1] || out[2] || out[3] || out[4])) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  // after integrate2() the getters' buffers hold the poses from before the step: the frame kernel pairs them with the current gv
+  rc = b->kin_prestep ? rsb_batch_update_kinematics(b) : ensure_kinematics(b); if (rc) return rc;
+  const size_t rows = (size_t)env_count * b->ftab.nf;
+  const size_t per[5] = {3, 9, 3, 3, (size_t)6 * b->nv};
+  float* dst[5] = {out[0], out[1], out[2], out[3], out[4]};
+  if (where == RSB_HOST) {
+    size_t need = 0;
+    for (int k = 0; k < 5; k++) if (out[k]) need += rows * per[k];
+    rc = ensure_scratch(b, &b->frame_staging, &b->frame_staging_words, need); if (rc) return rc;
+    float* s = b->frame_staging;
+    for (int k = 0; k < 5; k++) if (out[k]) { dst[k] = s; s += rows * per[k]; }
+  }
+  const int threads = 128;
+  const unsigned blocks = (unsigned)((rows * 32 + threads - 1) / threads);
+  rsb_frame_kernel<<<blocks, threads, 0, b->stream>>>(b->ftab, b->dbg_R, b->dbg_p, b->gv, b->gv_stride, env_begin, env_count, dst[0], dst[1], dst[2], dst[3], dst[4]);
+  CK(cudaGetLastError());
+  b->launches++;
+  if (where != RSB_HOST) return RSB_OK;
+  for (int k = 0; k < 5; k++) if (out[k]) { rc = copy_out(b, out[k], dst[k], rows * per[k] * 4, RSB_HOST); if (rc) return rc; }
+  return RSB_OK;
+}
+int rsb_batch_get_frame_states(rsb_batch* b, int env_begin, int env_count, float* pos, float* rot, float* lin_vel, float* ang_vel, int where) {
+  float* const out[5] = {pos, rot, lin_vel, ang_vel, nullptr};
+  return frame_outputs(b, env_begin, env_count, out, where);
+}
+int rsb_batch_get_frame_jacobians(rsb_batch* b, int env_begin, int env_count, float* jac, int where) {
+  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  if (!jac) return fail(RSB_ERR_INVALID, "null output buffer");
+  float* const out[5] = {nullptr, nullptr, nullptr, nullptr, jac};
+  return frame_outputs(b, env_begin, env_count, out, where);
 }
 int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;

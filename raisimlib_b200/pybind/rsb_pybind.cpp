@@ -90,6 +90,20 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void control_step(uintptr_t ptarget_dev, int substeps, uintptr_t obs_dev) {
     check(rsb_batch_control_step(b_, reinterpret_cast<const float*>(ptarget_dev), nullptr, RSB_DEVICE, substeps, reinterpret_cast<float*>(obs_dev), RSB_DEVICE), "control_step");
   }
+  // frames rigidly attached to bodies: body [F], pos [F*3], rot [F*9] row-major in the body frame (empty = identity)
+  void set_frames(const std::vector<int32_t>& body, const std::vector<float>& pos, const std::vector<float>& rot) {
+    if (pos.size() != 3 * body.size() || (!rot.empty() && rot.size() != 9 * body.size())) throw std::runtime_error("set_frames: need 3 positions and 0 or 9 rotation entries per frame");
+    check(rsb_batch_set_frames(b_, body.data(), pos.data(), rot.empty() ? nullptr : rot.data(), (int)body.size()), "set_frames");
+  }
+  // frame states of every environment into tensor addresses ([num_envs, F, 3 | 9] float32, contiguous); 0 skips an output
+  void frame_states(uintptr_t pos_dev, uintptr_t rot_dev, uintptr_t lin_dev, uintptr_t ang_dev) {
+    check(rsb_batch_get_frame_states(b_, 0, view_.num_envs, reinterpret_cast<float*>(pos_dev), reinterpret_cast<float*>(rot_dev), reinterpret_cast<float*>(lin_dev),
+                                     reinterpret_cast<float*>(ang_dev), RSB_DEVICE), "frame_states");
+  }
+  // frame Jacobians of every environment into a tensor address ([num_envs, F, 6, nv] float32, contiguous)
+  void frame_jacobians(uintptr_t jac_dev) {
+    check(rsb_batch_get_frame_jacobians(b_, 0, view_.num_envs, reinterpret_cast<float*>(jac_dev), RSB_DEVICE), "frame_jacobians");
+  }
   int num_envs() const { return view_.num_envs; }
   int nq() const { return view_.nq; }
   int nv() const { return view_.nv; }
@@ -121,6 +135,9 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("integrate", &Batch::integrate, py::arg("substeps") = 1)
       .def("update_kinematics", &Batch::update_kinematics)
       .def("control_step", &Batch::control_step)
+      .def("set_frames", &Batch::set_frames, py::arg("body"), py::arg("pos"), py::arg("rot") = std::vector<float>())
+      .def("frame_states", &Batch::frame_states, py::arg("pos_dev"), py::arg("rot_dev"), py::arg("lin_dev"), py::arg("ang_dev"))
+      .def("frame_jacobians", &Batch::frame_jacobians, py::arg("jac_dev"))
       .def("sync", &Batch::sync)
       .def_property_readonly("num_envs", &Batch::num_envs)
       .def_property_readonly("nq", &Batch::nq)
