@@ -20,12 +20,14 @@ DEFAULT_PARAMS = dict(dt=0.0025, gx=0.0, gy=0.0, gz=-9.81, erp=0.0, alpha_init=1
                       max_iter=150, threshold=1e-7, mu=0.8, restitution=0.0, rest_threshold=0.01, stall_window=8, stall_ratio=0.5, warm_start=0, slip_bisect=0, joint_limits=1, slip_local=1, accel_m=2, accel_start=6, stall_reg=0.02)
 
 
+def make(target, force=False):
+    """oracle/<target> rebuilt when it is older than one of its sources (the dependencies and flags are oracle/Makefile's)"""
+    subprocess.check_call(["make", "-C", _HERE, "-B" if force else "-s", target])
+    return os.path.join(_HERE, target)
+
+
 def build(force=False):
-    if force or not os.path.exists(_LIB_PATH) or any(
-            os.path.getmtime(os.path.join(_HERE, f)) > os.path.getmtime(_LIB_PATH)
-            for f in ("oracle_capi.cpp", "rbd_oracle.hpp")):
-        subprocess.check_call(["make", "-C", _HERE, "-B" if force else "-s", "liboracle.so"])
-    return _LIB_PATH
+    return make("liboracle.so", force)
 
 
 class _ModelDesc(C.Structure):

@@ -211,6 +211,7 @@ template <typename T> class Sim {
       }
     }
   }
+  virtual ~Sim() = default;
 
   void set_terrain(const Terrain& t) {
     ter = t;
@@ -565,8 +566,9 @@ template <typename T> class Sim {
     }
   }
 
-  void collide(Workspace<T>& ws) const {
-    ws.contacts.clear();
+  // every terrain hit into ws.all in candidate order, ranked into ws.contacts.  Virtual, like jacobians(): the two stages of step()
+  // that the self-collision restatement (self_collision.hpp) replaces
+  virtual void collide(Workspace<T>& ws) const {
     std::vector<Contact<T>>& all = ws.all;
     all.clear();
     const bool hm = ter.type == 2;
@@ -602,17 +604,27 @@ template <typename T> class Sim {
       if (!best.hit) continue;
       Contact<T> c;
       c.pt = k; c.body = b; c.pair = best.pair; c.n = best.n; c.depth = best.depth; c.pos = best.pos;
-      // tangent basis: t1 = normalised projection of e_x (or e_y when n is nearly along x)
-      V3<T> e = (std::fabs(c.n.x) < T(0.9)) ? V3<T>{1, 0, 0} : V3<T>{0, 1, 0};
-      V3<T> t = e - dot(e, c.n) * c.n;
-      T inv = T(1) / std::sqrt(dot(t, t));
-      c.t1 = inv * t; c.t2 = cross(c.n, c.t1);
+      tangent_frame(c);
       c.lam = {0, 0, 0};
       c.sdir = SlipDir<T>();
       all.push_back(c);
     }
+    rank_contacts(ws);
+  }
+
+  // tangent basis: t1 = normalised projection of e_x (or e_y when n is nearly along x)
+  static void tangent_frame(Contact<T>& c) {
+    V3<T> e = (std::fabs(c.n.x) < T(0.9)) ? V3<T>{1, 0, 0} : V3<T>{0, 1, 0};
+    V3<T> t = e - dot(e, c.n) * c.n;
+    T inv = T(1) / std::sqrt(dot(t, t));
+    c.t1 = inv * t; c.t2 = cross(c.n, c.t1);
+  }
+
+  // ws.contacts = the KMAX deepest of ws.all (ties: lower candidate index wins), emitted in candidate order
+  static void rank_contacts(Workspace<T>& ws) {
+    const std::vector<Contact<T>>& all = ws.all;
+    ws.contacts.clear();
     if ((int)all.size() > KMAX) {
-      // keep the KMAX deepest (ties: lower candidate index wins), emitted in candidate order
       std::vector<int> idx(all.size());
       for (size_t i = 0; i < idx.size(); i++) idx[i] = int(i);
       std::stable_sort(idx.begin(), idx.end(), [&](int a, int b) { return all[a].depth > all[b].depth; });
@@ -653,7 +665,7 @@ template <typename T> class Sim {
   }
 
   // ---- a7: contact Jacobian rows in the contact frame; Jt is nv x 3K (row r of Jt = dof r) -------
-  void jacobians(Workspace<T>& ws) const {
+  virtual void jacobians(Workspace<T>& ws) const {
     int K = int(ws.contacts.size()), C = 3 * K + int(ws.limits.size());
     std::fill(ws.Jt.begin(), ws.Jt.begin() + nv * C, T(0));
     for (size_t l = 0; l < ws.limits.size(); l++) ws.Jt[ws.limits[l].dof * C + 3 * K + int(l)] = ws.limits[l].sign;

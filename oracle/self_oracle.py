@@ -2,31 +2,19 @@
 product.  SelfOracle is oracle.Oracle on the library whose Sim also collides enabled pairs of the robot's own collision bodies
 (self_collision.hpp); without pairs it computes exactly what Oracle computes.  The same import rules as oracle.oracle hold."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from oracle import oracle as _o
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB_PATH = os.path.join(_HERE, "liboracle_self.so")
-_SOURCES = ("self_collision_capi.cpp", "self_collision.hpp", "oracle_capi.cpp", "rbd_oracle.hpp", "counting_scalar.hpp")
-# the parity build's flags (oracle/Makefile): no FMA contraction, portable ISA, so that the float32 instance evaluates the
-# narrow-phase predicates exactly as written
-_CXXFLAGS = ["-O3", "-march=x86-64-v3", "-ffp-contract=off", "-fopenmp", "-fPIC", "-std=c++17", "-Wall", "-Wno-unused-variable"]
-
 
 def build(force=False):
-    if force or not os.path.exists(_LIB_PATH) or any(os.path.getmtime(os.path.join(_HERE, f)) > os.path.getmtime(_LIB_PATH) for f in _SOURCES):
-        subprocess.check_call(["/usr/bin/g++", *_CXXFLAGS, "-shared", "-o", _LIB_PATH, os.path.join(_HERE, "self_collision_capi.cpp")])
-    return _LIB_PATH
+    return _o.make("liboracle_self.so", force)
 
 
 def lib():
     if "self" not in _o._libs:
-        build()
-        L = _o._declare(C.CDLL(_LIB_PATH))
+        L = _o._declare(C.CDLL(build()))
         L.orc_set_self_pairs.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.orc_self_pair_geometry.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
         L.orc_self_contact_jacobians.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 4

@@ -5,8 +5,8 @@ import os
 import numpy as np
 import pytest
 
-from helpers import ANYMAL_GC0, _urdf, fk_numpy, integrate_gc
-from oracle.oracle import Oracle
+from helpers import ANYMAL_GC0, ROW_BIAS, _urdf, fk_numpy, integrate_gc, normal_speeds
+from oracle.oracle import DEFAULT_PARAMS, Oracle
 from oracle.self_oracle import SelfOracle, self_pair_tables
 from oracle.urdf_tables import load_tables
 
@@ -32,33 +32,65 @@ def _sliders(m1, m2, gap):
                        '<link name="world"/>')
 
 
+@pytest.mark.parametrize("branch", ["feedforward", "pd_limits", "wrench", "row_bias", "plain"])
 @pytest.mark.parametrize("precision", ["f64", "f32"])
 @pytest.mark.parametrize("terrain", ["ground", "hm"])
-def test_without_pairs_self_oracle_is_the_oracle(terrain, precision):
+def test_without_pairs_self_oracle_is_the_oracle(terrain, precision, branch):
     """the self-collision restatement without pairs computes what the oracle computes, bit for bit: state, contact lists, impulses,
-    solver counters over 5 steps of robots dropped in random poses"""
+    solver counters over 5 steps of robots dropped in random poses, under feed-forward torques and on each branch of the step: stiff PD
+    with joints past their stops and actuators at their effort limits, an external wrench, ERP with restitution, the plain loop"""
     from helpers import random_state
     t = load_tables(os.path.join(RSC, "anymal_c_like.urdf"))
     rng = np.random.default_rng(11)
-    gc, gv = random_state(t, rng, 64, pos_scale=2.0, vel_scale=0.5, base_z=0.45)
-    tau = rng.uniform(-20, 20, (64, t["nv"])); tau[:, :6] = 0
-    out = []
-    for O in (Oracle, SelfOracle):
-        o = O(t, precision=precision)
+    n = 64
+    gc, gv = random_state(t, rng, n, pos_scale=2.0, vel_scale=0.5, base_z=0.45)
+    tau = rng.uniform(-20, 20, (n, t["nv"])); tau[:, :6] = 0
+    ctrl, params, ext = dict(tau_ff=tau), {"row_bias": ROW_BIAS, "plain": dict(accel_m=0, stall_window=0)}.get(branch), None
+    if branch == "pd_limits":        # two HAA joints of every robot start 0.05 rad past a stop; PD towards targets up to 1 rad away
+        haa = np.where(t["jlimit"][1:, 1] - t["jlimit"][1:, 0] < 3.0)[0] + 1
+        for e in range(n):
+            for body in rng.choice(haa, 2, replace=False):
+                lo, hi = t["jlimit"][body]
+                gc[e, t["qidx"][body]] = hi + 0.05 if rng.uniform() < 0.5 else lo - 0.05
+        pt = gc.copy(); pt[:, 7:] += rng.uniform(-1, 1, (n, t["nq"] - 7))
+        ctrl.update(ptarget=pt, vtarget=np.zeros((n, t["nv"])), kp=np.r_[np.zeros(6), 300.0 * np.ones(t["nv"] - 6)],
+                    kd=np.r_[np.zeros(6), 4.0 * np.ones(t["nv"] - 6)])
+    elif branch == "wrench":         # on a shank: the base rows and the leg's joint rows
+        ext = (3, rng.uniform(-40, 40, (n, 3)), rng.uniform(-4, 4, (n, 3)), (0.02, -0.01, 0.03))
+    runs = []
+    for O, e in [(Oracle, ext), (SelfOracle, ext)] + ([(Oracle, None)] if ext else []):   # the last: the oracle without the wrench
+        o = O(t, precision=precision, params=params)
         if terrain == "ground":
             o.set_ground(0.0)
         else:
             o.set_heightmap(65, 49, 12.8, 9.6, 0.1, -0.2, 0.1 * np.random.default_rng(12).uniform(-1, 1, (49, 65)))
         o.set_collision_friction(4, 0.5)
         a, b = gc.copy(), gv.copy()
-        o.step(a, b, n_steps=4, tau_ff=tau)
-        d = o.step(a, b, tau_ff=tau, debug=True)
-        out.append((a, b, d))
-    (a0, b0, d0), (a1, b1, d1) = out
-    assert d0["ncontacts"].sum() > 64
-    assert a0.tobytes() == a1.tobytes() and b0.tobytes() == b1.tobytes()
-    for k in d0:
-        assert d0[k].tobytes() == d1[k].tobytes(), k
+        steps = []
+        for _ in range(5):
+            d = o.step(a, b, ext=e, debug=True, **ctrl)
+            steps.append((a.copy(), b.copy(), d))
+        runs.append(steps)
+    for (a0, b0, d0), (a1, b1, d1) in zip(runs[0], runs[1]):
+        assert a0.tobytes() == a1.tobytes() and b0.tobytes() == b1.tobytes()
+        for k in d0:
+            assert d0[k].tobytes() == d1[k].tobytes(), k
+    # the branch was taken
+    a0, b0, d0 = runs[0][-1]
+    assert d0["ncontacts"].sum() > n
+    saturated = int((np.abs(d0["tau_applied"][:, 6:]) == t["jeffort"][1:]).sum())
+    starts = [(gc, gv)] + [(a, b) for a, b, _ in runs[0][:-1]]              # the state each step starts from
+    bounced = sum(int((normal_speeds(t, a, b, d) < -ROW_BIAS["rest_threshold"]).sum()) for (a, b), (_, _, d) in zip(starts, runs[0]))
+    print(f"{branch}: last step: contacts {d0['ncontacts'].sum()}, limit rows {d0['nlimits'].sum()}, dofs at their effort limit {saturated}, "
+          f"most sweeps {d0['iters'].max()}; 5 steps: approach speeds beyond the restitution threshold {bounced}")
+    if branch == "pd_limits":
+        assert d0["nlimits"].sum() > n // 2 and saturated > n
+    elif branch == "wrench":
+        assert not np.array_equal(b0, runs[2][-1][1])
+    elif branch == "row_bias":
+        assert bounced > 0
+    elif branch == "plain":          # solves long enough that the default loop would have extrapolated
+        assert d0["iters"].max() > DEFAULT_PARAMS["accel_start"]
 
 
 @pytest.mark.parametrize("e", [0.0, 0.5])
