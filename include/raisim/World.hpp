@@ -100,6 +100,10 @@ struct LockStep {
   std::vector<float> gc, gv, pt, vt, tau, tauApplied;
   std::vector<rsb_contact> contacts;
   std::vector<int32_t> ncontacts;
+  std::vector<float> cfForce;               // [n][S][3], [n][S] of the contact bodies (ArticulatedSystem::setContactBodies), S = cfBodies
+  std::vector<int32_t> cfSteps;
+  int cfBodies = 0;
+  bool cfValid = false;
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
   bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
@@ -132,6 +136,12 @@ struct LockStep {
     rsbCheck(rsb_batch_get_contacts(batch, contacts.data(), ncontacts.data(), 0, n, RSB_HOST), "getContacts");
     contactsValid = true;
   }
+  void needContactForces() {
+    if (cfValid) return;
+    cfForce.resize(size_t(n) * cfBodies * 3); cfSteps.resize(size_t(n) * cfBodies);
+    rsbCheck(rsb_batch_get_body_contact_forces(batch, 0, n, cfForce.data(), cfSteps.data(), RSB_HOST), "getBodyContactForce");
+    cfValid = true;
+  }
   // every environment is parked (or finished) with the same number of integrate() calls pending: upload, one launch, invalidate
   void flush() {
     int k = 0;
@@ -146,7 +156,7 @@ struct LockStep {
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
-    stateValid = tauAppliedValid = contactsValid = false;
+    stateValid = tauAppliedValid = contactsValid = cfValid = false;
   }
   // rows written outside a step (reset(), init()): push them before anything else reads the device
   void pushWrites() {
@@ -185,11 +195,25 @@ class BatchedWorld {
   void advanceTime(double t) { worldTime_ += t; }
   // lock-step mode (VectorizedEnvironment<ENVIRONMENT>): per-environment views work on host mirrors, integrate() is deferred
   LockStep* lockStep() { return ls_.get(); }
-  void enableLockStep() { if (!ls_) { ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); } }
+  void enableLockStep() { if (!ls_) { ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); ls_->cfBodies = int(contactBodies_.size()); } }
+  // bodies whose contact force every integrate() gathers (ArticulatedSystem::setContactBodies): one list for all environments
+  void setContactBodies(const std::vector<size_t>& bodies) {
+    if (bodies == contactBodies_) return;      // every environment of a VectorizedEnvironment sets the same list in its constructor
+    std::vector<int32_t> b(bodies.begin(), bodies.end());
+    rsbCheck(rsb_batch_set_contact_bodies(batch_, b.data(), int(b.size())), "setContactBodies");
+    contactBodies_ = bodies;
+    if (ls_) { ls_->cfBodies = int(bodies.size()); ls_->cfValid = false; }
+  }
+  size_t contactBodySlot(size_t bodyIdx) const {
+    for (size_t s = 0; s < contactBodies_.size(); s++) if (contactBodies_[s] == bodyIdx) return s;
+    throw std::runtime_error("getBodyContactForce: body " + std::to_string(bodyIdx) + " is not among the bodies given to setContactBodies()");
+  }
+  size_t numContactBodies() const { return contactBodies_.size(); }
   const std::string& urdf() const { return urdf_; }
   void rememberUrdf(const std::string& u) { urdf_ = u; }
  private:
   std::unique_ptr<LockStep> ls_;
+  std::vector<size_t> contactBodies_;
   std::string urdf_;
   rsb_model* model_ = nullptr;
   rsb_batch* batch_ = nullptr;
@@ -687,6 +711,36 @@ class ArticulatedSystem {
     contacts_.clear();
     for (int i = 0; i < n; i++) contacts_.emplace_back(c[i]);
     return contacts_;
+  }
+  // ---- Extensions upstream does not have.  Under upstream an ENVIRONMENT calls World::integrate() once per simulation step and sees
+  // every step's getContacts() in between; here the integrate() calls of a control step run as one fused launch and getContacts()
+  // shows the last of them only, so the launch gathers for the caller what that loop would have gathered.
+  // setContactBodies: the bodies (getBodyIdx order, at most RSB_MAX_CONTACT_BODIES) to gather for.  The list belongs to the batch: every
+  // environment shares it, and each environment of a VectorizedEnvironment may set the same list in its constructor.
+  void setContactBodies(const std::vector<size_t>& bodies) { w_->setContactBodies(bodies); }
+  // mean contact force on the body [N, world frame] over the integrate() calls since the last state access (the fused launch); over
+  // the one step of a stand-alone integrate()
+  void getBodyContactForce(size_t bodyIdx, Vec<3>& out) {
+    const size_t S = w_->numContactBodies(), s = w_->contactBodySlot(bodyIdx);
+    if (LockStep* ls = w_->lockStep()) {
+      ls->sync(env_); ls->needContactForces();
+      for (int k = 0; k < 3; k++) out[k] = ls->cfForce[(size_t(env_) * S + s) * 3 + k];
+      return;
+    }
+    std::vector<float> f(S * 3);
+    rsbCheck(rsb_batch_get_body_contact_forces(w_->batch(), env_, 1, f.data(), nullptr, RSB_HOST), "getBodyContactForce");
+    for (int k = 0; k < 3; k++) out[k] = f[s * 3 + k];
+  }
+  // the number of those integrate() calls in which the body had a contact (> 0: it touched something during the control step)
+  int getBodyContactSteps(size_t bodyIdx) {
+    const size_t S = w_->numContactBodies(), s = w_->contactBodySlot(bodyIdx);
+    if (LockStep* ls = w_->lockStep()) {
+      ls->sync(env_); ls->needContactForces();
+      return ls->cfSteps[size_t(env_) * S + s];
+    }
+    std::vector<int32_t> n(S);
+    rsbCheck(rsb_batch_get_body_contact_forces(w_->batch(), env_, 1, nullptr, n.data(), RSB_HOST), "getBodyContactSteps");
+    return n[s];
   }
   int env() const { return env_; }
  private:

@@ -231,6 +231,33 @@ int rsb_batch_get_frame_states(rsb_batch* b, int env_begin, int env_count, float
 /* [n][F][6][nv] row-major: rows 0-2 translational (v_point = Jp gv), rows 3-5 rotational (omega = Jr gv).
  * Columns follow the batch's gv order; for a floating base that is [v_world | omega_world | joints].  Non-ancestor columns are 0. */
 int rsb_batch_get_frame_jacobians(rsb_batch* b, int env_begin, int env_count, float* jac, int where);
+/* ---- contact forces per body over a whole launch.  A launch that advances the state (rsb_batch_integrate, rsb_batch_integrate2,
+ *      rsb_batch_control_step, rsb_batch_gym_step) runs `substeps` sub-steps, and the contact records above are those of the last one
+ *      only.  For up to RSB_MAX_CONTACT_BODIES chosen bodies, shared by all environments, the step kernel also gathers, as the
+ *      sub-steps go by:
+ *        force[env][s][3]         world frame, newtons: the sum over all sub-steps of the launch and over all contacts acting on body s
+ *                                 in each of them of the contact impulse on the body, times the float32 reciprocal of substeps * dt: the
+ *                                 mean contact force on the body over the launch.  A terrain contact acts on its local_body with the
+ *                                 impulse rsb_contact::impulse would show; a self contact with +impulse on its first body (local_body)
+ *                                 and -impulse on its second (-1 - pair_index), on both when both are listed.  Joint-limit rows and
+ *                                 external wrenches do not enter.
+ *        steps_in_contact[env][s] the number of sub-steps of the launch in which the body had at least one contact in the environment's
+ *                                 contact list (as first or second body), whatever the impulse: > 0 = touched during the launch,
+ *                                 == substeps = in contact throughout.
+ *      Contacts are summed in contact-list order and sub-steps in time order, one lane per body: results are bit-identical from run to
+ *      run and for every launch shape.  A candidate cut by the RSB_KMAX cap carries no impulse in the solve and none here.  Each
+ *      advancing launch overwrites both outputs; every other launch (rsb_batch_integrate1, the kinematics pass of the lazy getters,
+ *      rsb_batch_update_kinematics, the frame getters) leaves them as they are, like the contact records.  They read zero from
+ *      rsb_batch_set_contact_bodies() until the first advancing launch.  In rsb_batch_gym_step an environment that terminates and is
+ *      reset keeps the forces of the step that ended it.  With no bodies set the step computes and stores nothing for this.  Upstream
+ *      has no such call: there, user code sees every sub-step's getContacts() between its own World::integrate() calls. */
+#define RSB_MAX_CONTACT_BODIES 32
+/* body[n] in rsb_model_body_index order; a body may be listed twice.  n = 0 clears.  Refused with RSB_ERR_INVALID, changing nothing:
+ * n < 0 or > RSB_MAX_CONTACT_BODIES, NULL with n > 0, a body out of range. */
+int rsb_batch_set_contact_bodies(rsb_batch* b, const int32_t* body, int n);
+/* force [n][S][3] float32, steps_in_contact [n][S] int32, S = the number of bodies set; a NULL output is skipped; RSB_ERR_INVALID when
+ * no bodies are set.  A plain copy of a contiguous slice of the batch's rows in stream order: no launch, host or device destination. */
+int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count, float* force, int32_t* steps_in_contact, int where);
 /* FK, M and h of the CURRENT state for the getters above, without touching the contact records of the last integrate()
  * (upstream's getters are lazy the same way).  The getters call it themselves when the state changed through this API;
  * call it explicitly after writing the state through rsb_batch_device_ptrs() views. */

@@ -101,6 +101,7 @@ EXPORTED = [
     "rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities", "rsb_batch_get_body_poses", "rsb_batch_get_contacts",
     "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
     "rsb_batch_set_frames", "rsb_batch_get_frame_states", "rsb_batch_get_frame_jacobians",
+    "rsb_batch_set_contact_bodies", "rsb_batch_get_body_contact_forces",
     "rsb_batch_ob_dim", "rsb_batch_observe", "rsb_batch_control_step",
     "rsb_batch_gym_configure", "rsb_batch_gym_reset", "rsb_batch_gym_step",
     "rsb_peer_buffer_create", "rsb_peer_buffer_open", "rsb_peer_buffer_close", "rsb_peer_buffer_destroy", "rsb_batch_set_observation_peers", "rsb_batch_wait_observation_peers",
@@ -175,6 +176,9 @@ def lib():
         L.rsb_batch_set_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.rsb_batch_get_frame_states.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_int]
         L.rsb_batch_get_frame_jacobians.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
+        if hasattr(L, "rsb_batch_set_contact_bodies"):     # absent from an older build loaded through RSB_LIB_PATH (tools/contact_force_probe.py)
+            L.rsb_batch_set_contact_bodies.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+            L.rsb_batch_get_body_contact_forces.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
         L.rsb_batch_device_ptrs.argtypes = [C.c_void_p, C.POINTER(DeviceView)]
         L.rsb_batch_launch_count.argtypes = [C.c_void_p]
         L.rsb_batch_ob_dim.argtypes = [C.c_void_p]
@@ -280,7 +284,7 @@ class Batch:
         h = C.c_void_p()
         _ck(lib().rsb_batch_create(model.h, num_envs, device, C.byref(h)))
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
-        self.device, self.nframes = device, 0
+        self.device, self.nframes, self.ncontact_bodies = device, 0, 0
 
     def __del__(self):
         if getattr(self, "h", None) and lib is not None and _lib is not None:
@@ -481,15 +485,15 @@ class Batch:
         """[n, F, 6, nv]: rows 0-2 the frame point's velocity, rows 3-5 its body's angular velocity per unit gv"""
         return self._read(lib().rsb_batch_get_frame_jacobians, (self.nframes, 6, self.nv), np.float32, env_begin, env_count, range_first=True)
 
-    def _device_out(self, t, shape, name):
+    def _device_out(self, t, shape, name, dtype="float32"):
         """device address of a caller-given output tensor (None: skip it)"""
         if t is None:
             return None
         import torch
         if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
             raise ValueError(f"{name}: need a torch tensor on cuda:{self.device}")
-        if t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous():
-            raise ValueError(f"{name}: need a contiguous float32 tensor of shape {shape}, got {t.dtype} {tuple(t.shape)}")
+        if t.dtype != getattr(torch, dtype) or tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError(f"{name}: need a contiguous {dtype} tensor of shape {shape}, got {t.dtype} {tuple(t.shape)}")
         return C.c_void_p(t.data_ptr())
 
     def frame_states_into(self, pos=None, rot=None, lin_vel=None, ang_vel=None, env_begin=0, env_count=None):
@@ -503,6 +507,32 @@ class Batch:
         """frame_jacobians() written into a torch CUDA tensor [n, F, 6, nv], in the batch's stream order"""
         n = self._count(env_begin, env_count)
         _ck(lib().rsb_batch_get_frame_jacobians(self.h, env_begin, n, self._device_out(jac, (n, self.nframes, 6, self.nv), "jac"), DEVICE))
+
+    # contact forces per body over a whole launch
+    def set_contact_bodies(self, bodies):
+        """bodies [S] (at most 32 body indices, shared by all environments) whose mean contact force and sub-steps in contact every
+        launch that advances the state gathers over all its sub-steps.  An empty list clears them; a refused call keeps the list
+        set before."""
+        bd = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        _ck(lib().rsb_batch_set_contact_bodies(self.h, bd.ctypes.data_as(C.c_void_p), len(bd)))
+        self.ncontact_bodies = len(bd)
+
+    def set_contact_bodies_by_name(self, names):
+        self.set_contact_bodies([self.model.body_index(n) for n in names])
+
+    def body_contact_forces(self, env_begin=0, env_count=None):
+        """(force [n, S, 3] float32: world-frame mean contact force on each listed body over the last advancing launch;
+        steps [n, S] int32: its sub-steps in which the body had a contact)"""
+        n = self._count(env_begin, env_count)
+        force, steps = np.empty((n, self.ncontact_bodies, 3), np.float32), np.empty((n, self.ncontact_bodies), np.int32)
+        _ck(lib().rsb_batch_get_body_contact_forces(self.h, env_begin, n, force.ctypes.data_as(C.c_void_p), steps.ctypes.data_as(C.c_void_p), HOST))
+        return force, steps
+
+    def body_contact_forces_into(self, force=None, steps=None, env_begin=0, env_count=None):
+        """body_contact_forces() copied into torch CUDA tensors (float32 / int32; None skips one), in the batch's stream order: no launch"""
+        n, S = self._count(env_begin, env_count), self.ncontact_bodies
+        _ck(lib().rsb_batch_get_body_contact_forces(self.h, env_begin, n, self._device_out(force, (n, S, 3), "force"),
+                                                    self._device_out(steps, (n, S), "steps", "int32"), DEVICE))
 
     def diverged(self, env_begin=0, env_count=None):
         return self._read(lib().rsb_batch_get_diverged, (), np.int32, env_begin, env_count)

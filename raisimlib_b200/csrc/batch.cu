@@ -91,6 +91,11 @@ struct rsb_batch {
   int* frame_tab = nullptr;
   float* frame_staging = nullptr;    // device rows of the frame getters for a host destination (the largest read so far)
   size_t frame_staging_words = 0;
+  // contact bodies of rsb_batch_set_contact_bodies (none: empty) and the rows the step kernel fills for them, tight for the current
+  // list: cf_force [N][S][3], cf_steps [N][S]; allocated once, for RSB_MAX_CONTACT_BODIES
+  std::vector<uint8_t> contact_bodies;
+  float* cf_force = nullptr;
+  int* cf_steps = nullptr;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
@@ -334,6 +339,10 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   a.prm = b->prm; a.ter = b->ter; a.ws = b->ws;
   a.blob_words = (int)b->blob_host.size(); a.blob = b->blob;
   a.tau_applied = b->tau_applied;
+  if (phase_mask == 0 && !b->contact_bodies.empty()) {   // only a launch that advances the state accumulates (and overwrites) the contact forces
+    a.cf_force = b->cf_force; a.cf_steps = b->cf_steps; a.cf_n = (int)b->contact_bodies.size();
+    std::memcpy(a.cf_body, b->contact_bodies.data(), b->contact_bodies.size());
+  }
   a.ncontacts = b->ncontacts; a.contacts = b->contacts; a.contact_pt = b->contact_pt; a.iters = b->iters; a.diverged = b->diverged; a.resid = b->resid; a.solver_status = b->solver_status;
   if (debug) { a.dbg_M = b->dbg_M; a.dbg_h = b->dbg_h; a.dbg_R = b->dbg_R; a.dbg_p = b->dbg_p; }
   a.phase_mask = phase_mask; a.prof = b->prof; a.prof_a = b->prof_a;
@@ -584,7 +593,7 @@ void rsb_batch_destroy(rsb_batch* b) {
   for (void* p : {(void*)b->solver_status, (void*)b->resid, (void*)b->diverged, (void*)b->tau_applied, (void*)b->gc, (void*)b->gv, (void*)b->tau, (void*)b->pt, (void*)b->vt, (void*)b->ncontacts, (void*)b->contact_pt, (void*)b->iters,
                   (void*)b->contacts, (void*)b->dbg_M, (void*)b->dbg_h, (void*)b->dbg_R, (void*)b->dbg_p, (void*)b->hmap, (void*)b->staging, (void*)b->obs_staging, (void*)b->blob, (void*)b->gym_const, (void*)b->gym_action,
                   (void*)b->gym_obs, (void*)b->gym_reward, (void*)b->gym_done, (void*)b->ext, (void*)b->hmap_index, (void*)b->peer_done,
-                  (void*)b->frame_tab, (void*)b->frame_staging})
+                  (void*)b->frame_tab, (void*)b->frame_staging, (void*)b->cf_force, (void*)b->cf_steps})
     if (p) cudaFree(p);
   if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
   delete b;
@@ -964,6 +973,33 @@ int rsb_batch_get_frame_jacobians(rsb_batch* b, int env_begin, int env_count, fl
   if (!jac) return fail(RSB_ERR_INVALID, "null output buffer");
   float* const out[5] = {nullptr, nullptr, nullptr, nullptr, jac};
   return frame_outputs(b, env_begin, env_count, out, where);
+}
+// ---- contact forces per body over a whole launch: the step kernel accumulates them sub-step by sub-step into the batch's rows --------
+int rsb_batch_set_contact_bodies(rsb_batch* b, const int32_t* body, int n) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (n < 0 || n > RSB_MAX_CONTACT_BODIES) return fail(RSB_ERR_INVALID, "at most " + std::to_string(RSB_MAX_CONTACT_BODIES) + " contact bodies per batch (got " + std::to_string(n) + ")");
+  if (n > 0 && !body) return fail(RSB_ERR_INVALID, "null contact body list");
+  for (int s = 0; s < n; s++)
+    if (body[s] < 0 || body[s] >= b->nb) return fail(RSB_ERR_INVALID, "contact body " + std::to_string(s) + ": body index out of range (the model has " + std::to_string(b->nb) + ")");
+  if (n == 0) { b->contact_bodies.clear(); return RSB_OK; }
+  CK(cudaSetDevice(b->device));
+  const size_t rows = (size_t)b->N * RSB_MAX_CONTACT_BODIES;
+  if (!b->cf_force) CK(cudaMalloc((void**)&b->cf_force, rows * 3 * 4));
+  if (!b->cf_steps) CK(cudaMalloc((void**)&b->cf_steps, rows * 4));
+  // the rows of a new list read zero until a launch advances the state (in stream order: a step enqueued before this call still wrote the old layout)
+  CK(cudaMemsetAsync(b->cf_force, 0, rows * 3 * 4, b->stream));
+  CK(cudaMemsetAsync(b->cf_steps, 0, rows * 4, b->stream));
+  b->contact_bodies.assign(body, body + n);
+  return RSB_OK;
+}
+int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count, float* force, int32_t* steps_in_contact, int where) {
+  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  if (b->contact_bodies.empty()) return fail(RSB_ERR_INVALID, "no contact bodies: call rsb_batch_set_contact_bodies() first");
+  if (env_count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const size_t S = b->contact_bodies.size();
+  rc = force ? copy_out(b, force, b->cf_force + (size_t)env_begin * S * 3, (size_t)env_count * S * 3 * 4, where) : RSB_OK; if (rc) return rc;
+  return steps_in_contact ? copy_out(b, steps_in_contact, b->cf_steps + (size_t)env_begin * S, (size_t)env_count * S * 4, where) : RSB_OK;
 }
 int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count); if (rc) return rc;

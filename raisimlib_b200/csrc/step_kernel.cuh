@@ -219,6 +219,12 @@ struct StepArgs {
   float* resid;        // [N] largest impulse update of the last Gauss-Seidel sweep (< threshold: the solve converged)
   int* solver_status;  // [N] RSB_SOLVER_* of the last sub-step's solve
   float* tau_applied;  // [N][gv_stride] generalized force actually applied in the last sub-step (getGeneralizedForce)
+  // contact forces per body over the whole launch (rsb_batch_set_contact_bodies); cf_force null = none listed or the launch does not
+  // advance the state.  The list sits in the kernel parameters: lane s reads its body with one constant-bank load at its own index
+  float* cf_force;     // [N][cf_n][3] mean world force on body cf_body[s]: the row itself is the accumulator over the sub-steps
+  int* cf_steps;       // [N][cf_n] sub-steps in which the body had a contact in the list
+  int cf_n;
+  uint8_t cf_body[RSB_MAX_CONTACT_BODIES];
   float *dbg_M, *dbg_h, *dbg_R, *dbg_p;   // optional (integrate1 / getters)
   float* obs;          // optional [N][ob_dim]: RaisimGym observation row of the final state, written by this kernel
   int ob_dim;
@@ -1674,6 +1680,35 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         if (qi >= (floating ? 7 : 0)) s_gc[qi] += args.prm.dt * s_gv[i];
       }
       __syncwarp();
+      if (args.cf_force && lane < args.cf_n) {
+        // contact forces per body: lane s adds this sub-step's world impulses on body cf_body[s], formed as the contact records form
+        // them, in list order (+ on a contact's own body, - on the second body of a self contact).  The accumulator is the
+        // environment's own output row, which only this lane touches: stored at the first sub-step, read back and added to at the
+        // later ones, turned into the mean force at the last.  Nothing is carried in a register across the sub-step loop.
+        const int body = args.cf_body[lane];
+        float* fo = args.cf_force + ((size_t)env * args.cf_n + lane) * 3;
+        int* so = args.cf_steps + (size_t)env * args.cf_n + lane;
+        float ax = 0.f, ay = 0.f, az = 0.f;
+        int hit = 0;
+        if (sub > 0) { ax = fo[0]; ay = fo[1]; az = fo[2]; hit = *so; }   // issued before the walk over the contacts, which hides the L2 round trip
+        float fx = 0.f, fy = 0.f, fz = 0.f;
+        bool any = false;
+#pragma unroll 2
+        for (int k = 0; k < K; k++) {
+          const float* ct = s_ct + k * CT_WORDS;
+          const int pr = __float_as_int(ct[CF_PAIR]);
+          const bool first = __float_as_int(ct[CF_BODY]) == body, second = pr < 0 && -1 - pr == body;
+          const float lx = s_lam[3 * k], ly = s_lam[3 * k + 1], lz = s_lam[3 * k + 2];
+          const float ix = ct[CF_T1] * lx + ct[CF_T2] * ly + ct[CF_N] * lz;
+          const float iy = ct[CF_T1 + 1] * lx + ct[CF_T2 + 1] * ly + ct[CF_N + 1] * lz;
+          const float iz = ct[CF_T1 + 2] * lx + ct[CF_T2 + 2] * ly + ct[CF_N + 2] * lz;
+          fx += first ? ix : (second ? -ix : 0.f); fy += first ? iy : (second ? -iy : 0.f); fz += first ? iz : (second ? -iz : 0.f);
+          any |= first || second;
+        }
+        fx = ax + fx; fy = ay + fy; fz = az + fz; hit += any ? 1 : 0;
+        if (sub == args.substeps - 1) { const float s = 1.0f / ((float)args.substeps * args.prm.dt); fx *= s; fy *= s; fz *= s; }
+        fo[0] = fx; fo[1] = fy; fo[2] = fz; *so = hit;
+      }
       if (args.prof && lane == 0) args.prof[((size_t)env * 4 + (sub & 3)) * 8 + 5] = (unsigned)clock64();
     }   // substeps
 

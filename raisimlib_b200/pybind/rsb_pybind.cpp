@@ -104,6 +104,13 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void frame_jacobians(uintptr_t jac_dev) {
     check(rsb_batch_get_frame_jacobians(b_, 0, view_.num_envs, reinterpret_cast<float*>(jac_dev), RSB_DEVICE), "frame_jacobians");
   }
+  // bodies whose contact force every stepping launch gathers over all its sub-steps (empty clears)
+  void set_contact_bodies(const std::vector<int32_t>& body) { check(rsb_batch_set_contact_bodies(b_, body.data(), (int)body.size()), "set_contact_bodies"); }
+  // their mean contact force and sub-steps in contact over the last stepping launch into tensor addresses ([num_envs, S, 3] float32,
+  // [num_envs, S] int32, contiguous); 0 skips an output.  A copy in the batch's stream order: no launch
+  void body_contact_forces(uintptr_t force_dev, uintptr_t steps_dev) {
+    check(rsb_batch_get_body_contact_forces(b_, 0, view_.num_envs, reinterpret_cast<float*>(force_dev), reinterpret_cast<int32_t*>(steps_dev), RSB_DEVICE), "body_contact_forces");
+  }
   int num_envs() const { return view_.num_envs; }
   int nq() const { return view_.nq; }
   int nv() const { return view_.nv; }
@@ -138,6 +145,8 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("set_frames", &Batch::set_frames, py::arg("body"), py::arg("pos"), py::arg("rot") = std::vector<float>())
       .def("frame_states", &Batch::frame_states, py::arg("pos_dev"), py::arg("rot_dev"), py::arg("lin_dev"), py::arg("ang_dev"))
       .def("frame_jacobians", &Batch::frame_jacobians, py::arg("jac_dev"))
+      .def("set_contact_bodies", &Batch::set_contact_bodies, py::arg("body"))
+      .def("body_contact_forces", &Batch::body_contact_forces, py::arg("force_dev"), py::arg("steps_dev"))
       .def("sync", &Batch::sync)
       .def_property_readonly("num_envs", &Batch::num_envs)
       .def_property_readonly("nq", &Batch::nq)

@@ -31,6 +31,8 @@ def main():
     stream = torch.cuda.current_stream()
     wl = bench.Workload(key, 0, n)
     sim = bench.GpuSim(wl, 0, stream)
+    if os.environ.get("RSB_PROBE_CONTACT_BODIES"):     # e.g. 3,6,9,12: per-body contact forces on (their cost shows in stage E)
+        sim.bt.set_contact_bodies([int(x) for x in os.environ["RSB_PROBE_CONTACT_BODIES"].split(",")])
     for k in range(wl.settle + 8):
         sim.step_resident(k)
     torch.cuda.synchronize()
