@@ -104,6 +104,8 @@ struct LockStep {
   std::vector<int32_t> cfSteps;
   int cfBodies = 0;
   bool cfValid = false;
+  std::vector<float> bodyInertia;           // [n][nb][10] inertial rows (ArticulatedSystem::updateMassInfo); empty until the first one
+  bool bodyInertiaDirty = false;
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
   bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
@@ -152,7 +154,8 @@ struct LockStep {
     if (stateDirty) rsbCheck(rsb_batch_set_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "setState");
     if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
-    stateDirty = ptDirty = vtDirty = tauDirty = false;
+    if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
+    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = false;
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
@@ -163,7 +166,8 @@ struct LockStep {
     if (stateDirty) rsbCheck(rsb_batch_set_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "setState");
     if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
-    stateDirty = ptDirty = vtDirty = tauDirty = false;
+    if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
+    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = false;
   }
 };
 
@@ -446,7 +450,7 @@ class ArticulatedSystem {
   // One wrench (force + torque on the same body) per environment.
   void setExternalForce(size_t localIdx, const Vec<3>& force) {
     rsb_model_tables t; rsbCheck(rsb_model_get_tables(w_->model(), &t), "getTables");
-    Vec<3> c{t.com[localIdx * 3], t.com[localIdx * 3 + 1], t.com[localIdx * 3 + 2]};
+    Vec<3> c{comOf(t, int(localIdx), 0), comOf(t, int(localIdx), 1), comOf(t, int(localIdx), 2)};
     setExternalForce(localIdx, c, force);
   }
   void setExternalForce(size_t localIdx, const Vec<3>& posInBody, const Vec<3>& force) {
@@ -596,13 +600,55 @@ class ArticulatedSystem {
     return r;
   }
   VecDyn getActuationLowerLimits() const { VecDyn r = getActuationUpperLimits(); for (size_t i = 0; i < r.size(); i++) r[i] = -r[i]; return r; }
-  double getMass(size_t localIdx) const { return tables().mass[localIdx]; }
-  double getTotalMass() const { const rsb_model_tables t = tables(); double m = 0; for (int b = 0; b < t.nb; b++) m += t.mass[b]; return m; }
+  // the whole-body getters below read this environment's inertial parameters: the model's until updateMassInfo(), then the last ones
+  // it pushed
+  double getMass(size_t localIdx) const { return massOf(tables(), int(localIdx)); }
+  double getTotalMass() const { const rsb_model_tables t = tables(); double m = 0; for (int b = 0; b < t.nb; b++) m += massOf(t, b); return m; }
   std::vector<Vec<3>> getBodyCOM_B() const {
     const rsb_model_tables t = tables();
     std::vector<Vec<3>> r(size_t(t.nb));
-    for (int b = 0; b < t.nb; b++) for (int k = 0; k < 3; k++) r[size_t(b)][size_t(k)] = t.com[3 * b + k];
+    for (int b = 0; b < t.nb; b++) for (int k = 0; k < 3; k++) r[size_t(b)][size_t(k)] = comOf(t, b, k);
     return r;
+  }
+  // Upstream's idiom for changing a robot's inertial parameters: edit getMass()[i], getBodyCOM_B()[i] (body frame) and getInertia()[i]
+  // (about the centre of mass, body frame; symmetric), then updateMassInfo().  The vectors are this environment's editable copy,
+  // filled from the model on first use.  updateMassInfo() makes them the parameters this environment integrates: a stand-alone World
+  // uploads them at once; in a VectorizedEnvironment they go to the host mirror and up before the next launch (no launch of their
+  // own).  The batch refuses a copy that is not finite, has a negative mass or an inertia that is not positive semidefinite
+  // (include/rsb.h) when it arrives: at once stand-alone, at the upload in a VectorizedEnvironment.
+  std::vector<double>& getMass() { initMassInfo(); return mass_; }
+  std::vector<Vec<3>>& getBodyCOM_B() { initMassInfo(); return com_; }
+  std::vector<Mat<3, 3>>& getInertia() { initMassInfo(); return inertia_; }
+  void updateMassInfo() {
+    initMassInfo();
+    const size_t nb = mass_.size();
+    std::vector<float> row(nb * 10);
+    for (size_t b = 0; b < nb; b++) {
+      float* r = &row[b * 10];
+      const Mat<3, 3>& I = inertia_[b];
+      r[0] = float(mass_[b]);
+      for (size_t k = 0; k < 3; k++) r[1 + k] = float(com_[b][k]);
+      r[4] = float(I(0, 0)); r[5] = float(I(0, 1)); r[6] = float(I(0, 2)); r[7] = float(I(1, 1)); r[8] = float(I(1, 2)); r[9] = float(I(2, 2));
+    }
+    if (LockStep* ls = w_->lockStep()) {
+      ls->sync(env_);
+      if (ls->bodyInertia.empty()) {             // every environment starts from the model's rows
+        std::vector<float> model(nb * 10);
+        const rsb_model_tables t = tables();
+        for (size_t b = 0; b < nb; b++) {
+          model[b * 10] = float(t.mass[b]);
+          for (size_t k = 0; k < 3; k++) model[b * 10 + 1 + k] = float(t.com[3 * b + k]);
+          for (size_t k = 0; k < 6; k++) model[b * 10 + 4 + k] = float(t.inertia[6 * b + k]);
+        }
+        ls->bodyInertia.resize(size_t(ls->n) * nb * 10);
+        for (int e = 0; e < ls->n; e++) std::copy(model.begin(), model.end(), ls->bodyInertia.begin() + size_t(e) * nb * 10);
+      }
+      std::copy(row.begin(), row.end(), ls->bodyInertia.begin() + size_t(env_) * nb * 10);
+      ls->bodyInertiaDirty = true;
+    } else {
+      rsbCheck(rsb_batch_set_body_inertia(w_->batch(), row.data(), env_, 1, RSB_HOST), "updateMassInfo");
+    }
+    appliedMass_ = mass_; appliedCom_ = com_;
   }
   std::vector<Vec<3>> getBodyCOM_W() const {
     const rsb_model_tables t = tables(); const Poses P = poses();
@@ -613,7 +659,7 @@ class ArticulatedSystem {
   Vec<3> getCOM() const {      // centre of mass of the whole robot, world frame
     const rsb_model_tables t = tables(); const Poses P = poses();
     Vec<3> c; double m = 0;
-    for (int b = 0; b < t.nb; b++) { const Vec<3> cb = comWorld(t, P, b); for (int k = 0; k < 3; k++) c[size_t(k)] += t.mass[b] * cb[size_t(k)]; m += t.mass[b]; }
+    for (int b = 0; b < t.nb; b++) { const Vec<3> cb = comWorld(t, P, b); for (int k = 0; k < 3; k++) c[size_t(k)] += massOf(t, b) * cb[size_t(k)]; m += massOf(t, b); }
     for (int k = 0; k < 3; k++) c[size_t(k)] /= m;
     return c;
   }
@@ -632,7 +678,7 @@ class ArticulatedSystem {
   double getPotentialEnergy(const Vec<3>& gravity) const {
     const rsb_model_tables t = tables(); const Poses P = poses();
     double e = 0;
-    for (int b = 0; b < t.nb; b++) { const Vec<3> c = comWorld(t, P, b); e -= t.mass[b] * (gravity[0] * c[0] + gravity[1] * c[1] + gravity[2] * c[2]); }
+    for (int b = 0; b < t.nb; b++) { const Vec<3> c = comWorld(t, P, b); e -= massOf(t, b) * (gravity[0] * c[0] + gravity[1] * c[1] + gravity[2] * c[2]); }
     return e;
   }
   double getEnergy(const Vec<3>& gravity) const { return getKineticEnergy() + getPotentialEnergy(gravity); }
@@ -641,7 +687,7 @@ class ArticulatedSystem {
     Vec<3> p;
     for (int b = 0; b < t.nb; b++) {
       MatDyn J; jacobian(P, size_t(b), comWorld(t, P, b), &J, nullptr);
-      for (int r = 0; r < 3; r++) { double s = 0; for (size_t c = 0; c < J.cols(); c++) s += J(size_t(r), c) * gv[c]; p[size_t(r)] += t.mass[b] * s; }
+      for (int r = 0; r < 3; r++) { double s = 0; for (size_t c = 0; c < J.cols(); c++) s += J(size_t(r), c) * gv[c]; p[size_t(r)] += massOf(t, b) * s; }
     }
     return p;
   }
@@ -818,11 +864,30 @@ class ArticulatedSystem {
   }
   rsb_model_tables tables() const { rsb_model_tables t; rsbCheck(rsb_model_get_tables(w_->model(), &t), "getTables"); return t; }
   Vec<3> comWorld(const rsb_model_tables& t, const Poses& P, int b) const {
-    const float* R = &P.R[size_t(b) * 9]; const float* o = &P.p[size_t(b) * 3]; const double* c = &t.com[size_t(b) * 3];
+    const float* R = &P.R[size_t(b) * 9]; const float* o = &P.p[size_t(b) * 3];
+    const double c[3] = {comOf(t, b, 0), comOf(t, b, 1), comOf(t, b, 2)};
     Vec<3> r;
     for (int k = 0; k < 3; k++) r[size_t(k)] = o[k] + R[3 * k] * c[0] + R[3 * k + 1] * c[1] + R[3 * k + 2] * c[2];
     return r;
   }
+  // this environment's inertial parameters: the model's until updateMassInfo() pushed its own
+  double massOf(const rsb_model_tables& t, int b) const { return appliedMass_.empty() ? t.mass[b] : appliedMass_[size_t(b)]; }
+  double comOf(const rsb_model_tables& t, int b, int k) const { return appliedCom_.empty() ? t.com[3 * b + k] : appliedCom_[size_t(b)][size_t(k)]; }
+  void initMassInfo() {
+    if (!mass_.empty()) return;
+    const rsb_model_tables t = tables();
+    mass_.resize(size_t(t.nb)); com_.resize(size_t(t.nb)); inertia_.resize(size_t(t.nb));
+    for (int b = 0; b < t.nb; b++) {
+      mass_[size_t(b)] = t.mass[b];
+      for (int k = 0; k < 3; k++) com_[size_t(b)][size_t(k)] = t.com[3 * b + k];
+      const double* I = &t.inertia[6 * b];
+      const double full[9] = {I[0], I[1], I[2], I[1], I[3], I[4], I[2], I[4], I[5]};
+      for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) inertia_[size_t(b)](size_t(r), size_t(c)) = full[3 * r + c];
+    }
+  }
+  std::vector<double> mass_, appliedMass_;            // editable copy (getMass()) and the values last pushed by updateMassInfo()
+  std::vector<Vec<3>> com_, appliedCom_;
+  std::vector<Mat<3, 3>> inertia_;
   VecDyn lastP_, lastD_, kpLast_, kdLast_;
   std::vector<int> qmap_, vmap_;
   BatchedWorld* w_;

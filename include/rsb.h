@@ -186,6 +186,21 @@ int rsb_batch_set_control_mode(rsb_batch* b, int mode);
  * sub-steps of that call) and is cleared afterwards. */
 int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, const float* torque, const float* point_body,
                                   int env_begin, int env_count, int where);
+/* Per-environment inertial parameters of every body (ArticulatedSystem::getMass / getBodyCOM_B / getInertia + updateMassInfo, per
+ * World upstream).  rows [env_count][nb][10] float32: mass, centre of mass in the body frame (3), inertia about the centre of mass in
+ * the body frame (xx, xy, xz, yy, yz, zz) -- the order of rsb_model_tables mass / com / inertia.  rows == NULL resets those
+ * environments to the model's values.  Host or device source (`where`).
+ * The first call (and the first after rsb_batch_clear_body_inertia) gives every environment the model's float32 values, the ones the
+ * step uses without rows, then writes the range: rows equal to the model's values give results bit-identical to no rows.  Every later
+ * launch of the step kernel uses the rows: integrate, integrate1, integrate2, control_step, gym_step and the kinematics pass of the
+ * lazy getters (gym resets keep them).  M, h and the poses describe the new parameters from the next getter on.
+ * Refused with RSB_ERR_INVALID, changing nothing: a bad range or `where`, a value that is not finite, a negative mass, or an inertia
+ * that is not positive semidefinite.  The inertia test, in double precision with t = xx + yy + zz: every diagonal entry >= -1e-6 t,
+ * every 2 x 2 principal minor >= -1e-6 t^2 and the determinant >= -1e-6 t^3.  The rows are checked on the device in a staging buffer
+ * before any of them is committed; the call waits for that check.  Gains, effort limits, friction and collision shapes stay per batch. */
+int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
+/* drop all per-environment rows: every later launch runs exactly as if none had ever been set */
+int rsb_batch_clear_body_inertia(rsb_batch* b);
 /* ArticulatedSystem::getGeneralizedForce(): feed-forward + PD force applied over the last integrate() */
 int rsb_batch_get_generalized_force(rsb_batch* b, float* tau, int env_begin, int env_count, int where);
 

@@ -37,6 +37,28 @@ __global__ void rsb_ext_pack_kernel(float* rows, int body, const float* __restri
   r[7] = px; r[8] = py; r[9] = pz; r[10] = 0.f; r[11] = 0.f;
 }
 
+// per-environment inertial rows (rsb_batch_set_body_inertia, StepArgs::body_inertia): `rows` tight rows of the caller [mass | com(3) |
+// inertia xx xy xz yy yz zz] checked and repacked to BI_WORDS.  A refused row lowers *bad to row * 4 + reason (1 not finite, 2 negative
+// mass, 3 inertia not positive semidefinite); *bad is left alone when every row is accepted.  PSD within a tolerance relative to the
+// trace t: every principal minor of order k >= -eps t^k (double precision)
+enum BodyInertiaFault { BI_NOT_FINITE = 1, BI_NEGATIVE_MASS = 2, BI_NOT_PSD = 3 };
+__global__ void rsb_body_inertia_pack_kernel(float* __restrict__ out, const float* __restrict__ src, int rows, double eps, int* bad) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  float v[10];
+  bool finite = true;
+  for (int k = 0; k < 10; k++) { v[k] = src[(size_t)r * 10 + k]; finite = finite && isfinite(v[k]); }
+  float* o = out + (size_t)r * BI_WORDS;
+  for (int k = 0; k < 10; k++) o[k] = v[k];
+  o[10] = 0.f; o[11] = 0.f;
+  const double xx = v[4], xy = v[5], xz = v[6], yy = v[7], yz = v[8], zz = v[9], t = xx + yy + zz;
+  const double m2 = eps * t * t;
+  const bool psd = xx >= -eps * t && yy >= -eps * t && zz >= -eps * t && xx * yy - xy * xy >= -m2 && xx * zz - xz * xz >= -m2 && yy * zz - yz * yz >= -m2 &&
+                   xx * (yy * zz - yz * yz) - xy * (xy * zz - yz * xz) + xz * (xy * yz - yy * xz) >= -m2 * t;
+  const int fault = !finite ? BI_NOT_FINITE : !(v[0] >= 0.f) ? BI_NEGATIVE_MASS : !psd ? BI_NOT_PSD : 0;
+  if (fault) atomicMin(bad, r * 4 + fault);
+}
+
 // ---- frame kinematics (rsb_batch_set_frames / get_frame_states / get_frame_jacobians) ----------------------------------------------
 // Frames rigidly attached to bodies and, per dof, what its Jacobian column needs; device arrays uploaded by rsb_batch_set_frames.
 // A dof turns or slides along the axis a of its body k (a = R_k axis: the joint frame's rotation about its own axis leaves the axis

@@ -96,6 +96,14 @@ struct rsb_batch {
   std::vector<uint8_t> contact_bodies;
   float* cf_force = nullptr;
   int* cf_steps = nullptr;
+  // per-environment inertial rows of rsb_batch_set_body_inertia: bi_rows [N][nb][BI_WORDS], read by every step launch while bi_active.
+  // bi_stage: the same layout, where a call's rows are checked before they replace any of bi_rows; bi_src: a host source's tight rows
+  // on the device; bi_bad: the check's verdict
+  float* bi_rows = nullptr;
+  float* bi_stage = nullptr;
+  float* bi_src = nullptr;
+  int* bi_bad = nullptr;
+  bool bi_active = false;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
@@ -347,6 +355,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   if (debug) { a.dbg_M = b->dbg_M; a.dbg_h = b->dbg_h; a.dbg_R = b->dbg_R; a.dbg_p = b->dbg_p; }
   a.phase_mask = phase_mask; a.prof = b->prof; a.prof_a = b->prof_a;
   a.ext = b->ext_active ? b->ext : nullptr;
+  a.body_inertia = b->bi_active ? b->bi_rows : nullptr;
   a.obs = obs_dev; a.ob_dim = rsb_batch_ob_dim(b);
   if (gym) {       // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
     a.gym_action = gym->action; a.gym = b->gym; a.gym_reward = gym->reward; a.gym_done = gym->done;
@@ -593,7 +602,8 @@ void rsb_batch_destroy(rsb_batch* b) {
   for (void* p : {(void*)b->solver_status, (void*)b->resid, (void*)b->diverged, (void*)b->tau_applied, (void*)b->gc, (void*)b->gv, (void*)b->tau, (void*)b->pt, (void*)b->vt, (void*)b->ncontacts, (void*)b->contact_pt, (void*)b->iters,
                   (void*)b->contacts, (void*)b->dbg_M, (void*)b->dbg_h, (void*)b->dbg_R, (void*)b->dbg_p, (void*)b->hmap, (void*)b->staging, (void*)b->obs_staging, (void*)b->blob, (void*)b->gym_const, (void*)b->gym_action,
                   (void*)b->gym_obs, (void*)b->gym_reward, (void*)b->gym_done, (void*)b->ext, (void*)b->hmap_index, (void*)b->peer_done,
-                  (void*)b->frame_tab, (void*)b->frame_staging, (void*)b->cf_force, (void*)b->cf_steps})
+                  (void*)b->frame_tab, (void*)b->frame_staging, (void*)b->cf_force, (void*)b->cf_steps, (void*)b->bi_rows, (void*)b->bi_stage,
+                  (void*)b->bi_src, (void*)b->bi_bad})
     if (p) cudaFree(p);
   if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
   delete b;
@@ -815,6 +825,79 @@ int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, co
   const int threads = 128, blocks = (env_count + threads - 1) / threads;
   rsb_ext_pack_kernel<<<blocks, threads, 0, b->stream>>>(b->ext + (size_t)env_begin * EXT_WORDS, body, df, dtq, px, py, pz, env_count);
   CK(cudaGetLastError());
+  return RSB_OK;
+}
+// ---- per-environment inertial parameters (ArticulatedSystem::getMass / getBodyCOM_B / getInertia + updateMassInfo per World upstream) ----
+// the model's row of every body, in float32 exactly as build_blob writes BF_MASS / BF_COM / BF_INERTIA, repeated for n environments
+static std::vector<float> model_inertia_rows(const Model& md, int n) {
+  std::vector<float> r((size_t)n * md.nb * BI_WORDS, 0.f);
+  for (int e = 0; e < n; e++)
+    for (int i = 0; i < md.nb; i++) {
+      float* o = &r[((size_t)e * md.nb + i) * BI_WORDS];
+      o[0] = (float)md.mass[i];
+      for (int k = 0; k < 3; k++) o[1 + k] = (float)md.com[3 * i + k];
+      for (int k = 0; k < 6; k++) o[4 + k] = (float)md.inertia[6 * i + k];
+    }
+  return r;
+}
+int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {
+  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  if (where != RSB_HOST && where != RSB_DEVICE) return fail(RSB_ERR_INVALID, "body inertia: `where` must be RSB_HOST or RSB_DEVICE");
+  if (env_count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const Model& md = b->model->md;
+  const size_t per_env = (size_t)md.nb * BI_WORDS, all = (size_t)b->N * per_env;
+  const float* staged = nullptr;
+  std::vector<float> model_rows;
+  if (rows) {   // check the caller's rows in bi_stage; nothing of bi_rows changes unless every value is accepted
+    if (!b->bi_stage) CK(cudaMalloc((void**)&b->bi_stage, all * 4));
+    if (!b->bi_bad) CK(cudaMalloc((void**)&b->bi_bad, 4));
+    const float* src = rows;
+    const size_t nrows = (size_t)env_count * md.nb;
+    if (where == RSB_HOST) {
+      if (!b->bi_src) CK(cudaMalloc((void**)&b->bi_src, (size_t)b->N * md.nb * 10 * 4));
+      CK(cudaMemcpyAsync(b->bi_src, rows, nrows * 10 * 4, cudaMemcpyHostToDevice, b->stream));
+      src = b->bi_src;
+    }
+    const int ok = 0x7fffffff;
+    CK(cudaMemcpyAsync(b->bi_bad, &ok, 4, cudaMemcpyHostToDevice, b->stream));
+    const int threads = 128;
+    rsb_body_inertia_pack_kernel<<<(unsigned)((nrows + threads - 1) / threads), threads, 0, b->stream>>>(b->bi_stage, src, (int)nrows, 1e-6, b->bi_bad);
+    CK(cudaGetLastError());
+    int bad = ok;
+    CK(cudaMemcpyAsync(&bad, b->bi_bad, 4, cudaMemcpyDeviceToHost, b->stream));
+    CK(cudaStreamSynchronize(b->stream));
+    if (bad != ok) {
+      static const char* what[] = {"", "a value that is not finite", "a negative mass", "an inertia that is not symmetric positive semidefinite"};
+      const int r = bad / 4, env = env_begin + r / md.nb, body = r % md.nb;
+      return fail(RSB_ERR_INVALID, "body inertia: environment " + std::to_string(env) + ", body " + std::to_string(body) + " (" + md.body_names[body] + ") has " + what[bad & 3] +
+                                   "; no row changed");
+    }
+    staged = b->bi_stage;
+  } else {
+    model_rows = model_inertia_rows(md, env_count);
+  }
+  // commit: the first call after creation or rsb_batch_clear_body_inertia starts every environment from the model's rows
+  if (!b->bi_rows) CK(cudaMalloc((void**)&b->bi_rows, all * 4));
+  if (!b->bi_active) {
+    const std::vector<float> init = model_inertia_rows(md, b->N);
+    CK(cudaMemcpyAsync(b->bi_rows, init.data(), all * 4, cudaMemcpyHostToDevice, b->stream));
+    CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
+  }
+  float* const at = b->bi_rows + (size_t)env_begin * per_env;
+  if (staged) CK(cudaMemcpyAsync(at, staged, (size_t)env_count * per_env * 4, cudaMemcpyDeviceToDevice, b->stream));
+  else {
+    CK(cudaMemcpyAsync(at, model_rows.data(), model_rows.size() * 4, cudaMemcpyHostToDevice, b->stream));
+    CK(cudaStreamSynchronize(b->stream));
+  }
+  b->bi_active = true;
+  b->kin_dirty = true;   // M, h and the poses of the getters describe the new parameters from the next getter on
+  return RSB_OK;
+}
+int rsb_batch_clear_body_inertia(rsb_batch* b) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (b->bi_active) b->kin_dirty = true;
+  b->bi_active = false;
   return RSB_OK;
 }
 int rsb_batch_set_control_mode(rsb_batch* b, int mode) {

@@ -41,6 +41,7 @@ constexpr int NROUNDS = 2;         // 32-section rounds of the slip search: brac
 constexpr int SEC_STRIDE = 36;      // (NSEC+1) padded
 constexpr int CT_WORDS = 16;        // per-contact shared record
 constexpr int EXT_WORDS = 12;       // external wrench row: body (int bits), force(3), torque(3), point in the body frame(3), 2 pad
+constexpr int BI_WORDS = 12;        // per-environment inertial row of one body: mass, com(3), inertia xx xy xz yy yz zz, 2 pad (three float4)
 constexpr int MAX_PT_SLOTS = 2;     // candidate points per lane (npts <= 64)
 constexpr int HIST_WORDS = 6 * 32;  // Anderson history of the Gauss-Seidel sweep map (stage D)
 constexpr int MAX_PEERS = 8;        // GPUs of one NVSwitch domain that receive this GPU's observation rows (fused all-gather)
@@ -229,6 +230,8 @@ struct StepArgs {
   float* obs;          // optional [N][ob_dim]: RaisimGym observation row of the final state, written by this kernel
   int ob_dim;
   const float* ext;    // optional [num_envs][EXT_WORDS] external wrench rows (body, F world, T world, point in body frame); null = none
+  const float* body_inertia;   // optional [num_envs][nb][BI_WORDS] inertial rows (rsb_batch_set_body_inertia) read by stage A in place
+                               // of the blob's BF_MASS / BF_COM / BF_INERTIA; null = the model's values for every environment
   unsigned* prof;      // optional [num_envs][4 sub-steps][8] SM-clock stamps at the stage boundaries (tools/balance_probe.py)
   unsigned* prof_a;    // optional [num_envs][4 sub-steps][4] SM-clock stamps inside stage A: after the FK walk, the per-body terms, the
                        // subtree sums, the M columns (tools/stage_probe.py)
@@ -1055,15 +1058,25 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         // per-body force and inertia terms about O
         float X[16];   // F(3) N_O(3) m h(3) I_O(6)
         {
-          float m = bvalid ? bodyf[BF_MASS * nbp + bb] : 0.f;
-          f3 cl = mk(bodyf[(BF_COM + 0) * nbp + bb], bodyf[(BF_COM + 1) * nbp + bb], bodyf[(BF_COM + 2) * nbp + bb]);
+          // inertial parameters: the model's (blob) or this environment's own row (envA: a leader's upper lanes read the partner's),
+          // the same floats into the same expressions either way
+          float m; f3 cl; float I0, I1, I2, I3, I4, I5;
+          if (args.body_inertia) {
+            const float4* row = reinterpret_cast<const float4*>(args.body_inertia + ((size_t)envA * nb + bb) * BI_WORDS);
+            const float4 r0 = __ldg(row), r1 = __ldg(row + 1), r2 = __ldg(row + 2);
+            m = r0.x; cl = mk(r0.y, r0.z, r0.w);
+            I0 = r1.x; I1 = r1.y; I2 = r1.z; I3 = r1.w; I4 = r2.x; I5 = r2.y;
+          } else {
+            m = bodyf[BF_MASS * nbp + bb];
+            cl = mk(bodyf[(BF_COM + 0) * nbp + bb], bodyf[(BF_COM + 1) * nbp + bb], bodyf[(BF_COM + 2) * nbp + bb]);
+            I0 = bodyf[(BF_INERTIA + 0) * nbp + bb]; I1 = bodyf[(BF_INERTIA + 1) * nbp + bb]; I2 = bodyf[(BF_INERTIA + 2) * nbp + bb];
+            I3 = bodyf[(BF_INERTIA + 3) * nbp + bb]; I4 = bodyf[(BF_INERTIA + 4) * nbp + bb]; I5 = bodyf[(BF_INERTIA + 5) * nbp + bb];
+          }
+          if (!bvalid) { m = 0.f; I0 = I1 = I2 = I3 = I4 = I5 = 0.f; }
           f3 c = mulR(R, cl);
           f3 cO = (p - O) + c;
           f3 ac = vd + cross(wd, c) + cross(w, cross(w, c));
           f3 f = m * ac;
-          float I0 = bodyf[(BF_INERTIA + 0) * nbp + bb], I1 = bodyf[(BF_INERTIA + 1) * nbp + bb], I2 = bodyf[(BF_INERTIA + 2) * nbp + bb];
-          float I3 = bodyf[(BF_INERTIA + 3) * nbp + bb], I4 = bodyf[(BF_INERTIA + 4) * nbp + bb], I5 = bodyf[(BF_INERTIA + 5) * nbp + bb];
-          if (!bvalid) { I0 = I1 = I2 = I3 = I4 = I5 = 0.f; }
           // Iw = R I R^T
           float RI[9];
 #pragma unroll

@@ -111,6 +111,10 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void body_contact_forces(uintptr_t force_dev, uintptr_t steps_dev) {
     check(rsb_batch_get_body_contact_forces(b_, 0, view_.num_envs, reinterpret_cast<float*>(force_dev), reinterpret_cast<int32_t*>(steps_dev), RSB_DEVICE), "body_contact_forces");
   }
+  // per-environment inertial rows [env_count, nb, 10] float32 (mass, com, inertia xx xy xz yy yz zz) from a device address
+  void set_body_inertia(uintptr_t rows_dev, int env_begin, int env_count) {
+    check(rsb_batch_set_body_inertia(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_body_inertia");
+  }
   int num_envs() const { return view_.num_envs; }
   int nq() const { return view_.nq; }
   int nv() const { return view_.nv; }
@@ -147,6 +151,7 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("frame_jacobians", &Batch::frame_jacobians, py::arg("jac_dev"))
       .def("set_contact_bodies", &Batch::set_contact_bodies, py::arg("body"))
       .def("body_contact_forces", &Batch::body_contact_forces, py::arg("force_dev"), py::arg("steps_dev"))
+      .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("sync", &Batch::sync)
       .def_property_readonly("num_envs", &Batch::num_envs)
       .def_property_readonly("nq", &Batch::nq)

@@ -33,6 +33,10 @@ def main():
     sim = bench.GpuSim(wl, 0, stream)
     if os.environ.get("RSB_PROBE_CONTACT_BODIES"):     # e.g. 3,6,9,12: per-body contact forces on (their cost shows in stage E)
         sim.bt.set_contact_bodies([int(x) for x in os.environ["RSB_PROBE_CONTACT_BODIES"].split(",")])
+    if os.environ.get("RSB_PROBE_BODY_INERTIA"):       # 1: a distinct inertial row in every environment (their cost shows in stage A)
+        rows = np.tile(sim.bt.model_body_inertia(), (n, 1, 1))
+        rows[:, :, :1] *= np.random.default_rng(1).uniform(0.98, 1.02, (n, rows.shape[1], 1)).astype(np.float32)
+        sim.bt.set_body_inertia(rows)
     for k in range(wl.settle + 8):
         sim.step_resident(k)
     torch.cuda.synchronize()
