@@ -12,6 +12,9 @@
  * Rules: plain C, opaque handles, int status (0 = OK, negative = error, text via rsb_last_error()),
  * no exceptions across the boundary, all buffers caller-owned.  One handle <-> one host thread.
  * All batched arrays are float32; `where` says whether a caller buffer is host or device memory.
+ * `where`, `where_in` and `where_out` are RSB_HOST or RSB_DEVICE: any other value is refused with
+ * RSB_ERR_INVALID before anything is enqueued.  Pageable host rows pass through a device staging
+ * buffer of the batch that grows to the largest such transfer and is kept until the batch is destroyed.
  * Device work is enqueued on the batch's stream (rsb_batch_set_stream) and is asynchronous unless a
  * host buffer is read back.
  */
@@ -196,8 +199,8 @@ int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, co
  * lazy getters (gym resets keep them).  M, h and the poses describe the new parameters from the next getter on.
  * Refused with RSB_ERR_INVALID, changing nothing: a bad range or `where`, a value that is not finite, a negative mass, or an inertia
  * that is not positive semidefinite.  The inertia test, in double precision with t = xx + yy + zz: every diagonal entry >= -1e-6 t,
- * every 2 x 2 principal minor >= -1e-6 t^2 and the determinant >= -1e-6 t^3.  The rows are checked on the device in a staging buffer
- * before any of them is committed; the call waits for that check.  Gains, effort limits, friction and collision shapes stay per batch. */
+ * every 2 x 2 principal minor >= -1e-6 t^2 and the determinant >= -1e-6 t^3.  The rows are checked on the device in the batch's
+ * staging buffer before any of them is committed; the call waits for that check.  Gains, effort limits, friction and collision shapes stay per batch. */
 int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
 /* drop all per-environment rows: every later launch runs exactly as if none had ever been set */
 int rsb_batch_clear_body_inertia(rsb_batch* b);
@@ -232,8 +235,8 @@ int rsb_batch_get_solver_residual(rsb_batch* b, float* resid, int env_begin, int
  *      poses from before that step (M and h stay those of integrate1()); the frame getters then run the kinematics pass for the
  *      stepped state first, so poses and velocities always belong to one state, and M, h and the body poses describe it too from
  *      then on.  Device buffers are tight rows, written in stream order.  Host buffers are written when the call returns; they are
- *      staged through a device buffer of the batch sized to the largest host read so far (env_count * F floats times 18 for the
- *      states, times 6 * nv for the Jacobians), kept until the batch is destroyed: device buffers avoid it. */
+ *      staged through the batch's staging buffer (env_count * F floats times 18 for the states, times 6 * nv for the Jacobians):
+ *      device buffers avoid it. */
 #define RSB_MAX_FRAMES 64
 /* Frames rigidly attached to bodies, shared by all environments: body[n] (rsb_model_body_index order), pos[n][3] in the body frame,
  * rot[n][9] row-major orientation in the body frame (NULL = identity).  rsb_model_frame() returns exactly (body, pos, rot) for the

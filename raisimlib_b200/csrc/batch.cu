@@ -26,6 +26,50 @@ static int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
 struct rsb_model { Model md; };
 
+// A device allocation of the batch: it grows on demand, never shrinks, and is freed with its owner.  A failed ensure() leaves the
+// buffer as it was; a successful one that grows it does not keep the contents.
+template <class T>
+struct DevBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+  T* get() const { return static_cast<T*>(p); }
+  cudaError_t ensure(size_t need, cudaStream_t s) {
+    if (bytes >= need) return cudaSuccess;
+    void* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, need);
+    if (e != cudaSuccess) return e;
+    if (p && (e = cudaStreamSynchronize(s)) != cudaSuccess) { cudaFree(q); return e; }   // work enqueued on s may still use the old one
+    if (p) cudaFree(p);
+    p = q; bytes = need;
+    return cudaSuccess;
+  }
+};
+
+// what the batch's model and overrides decide about the step launch, built whole by rebuild() and taken by the batch only when all of
+// it succeeded: the model blob (the kernel's copy is uploaded from this one), the per-warp workspace, the compiled instance and the shape
+struct LaunchConfig {
+  std::vector<uint32_t> blob;
+  BlobHeader hdr{};
+  Dims dims{};
+  WsLayout ws{};
+  int spec = 0;                  // 0 generic, 1 quadruped-12 static dims, 2 humanoid-30 static dims
+  int slots = 1;
+  int wpc = 0, grid = 0;
+  size_t smem_bytes = 0;
+};
+
+// the per-batch settings the blob is built from
+struct Overrides {
+  std::vector<float> kp, kd;         // [nv] PD gains
+  std::vector<float> pt_mu;          // [npts] terrain friction of every contact candidate (< 0: default material)
+  std::vector<int32_t> self_pairs;   // [n][2] collision bodies of the enabled self-collision pairs (rsb_batch_set_self_collision)
+  std::vector<float> self_mu;        // [n] their friction (< 0: default material)
+};
+
 struct rsb_batch {
   const rsb_model* model = nullptr;
   int N = 0, device = 0;
@@ -40,78 +84,57 @@ struct rsb_batch {
   int pt_bound_stride = 0;
   const float* vt_bound = nullptr;   // same for the velocity targets
   int vt_bound_stride = 0;
-  bool pt_once = false, vt_once = false;   // zero-copy control step: the kernel copies the rows it read into pt / vt, then THAT binding ends
   // fused observation all-gather over NVLink peer memory (rsb_batch_set_observation_peers)
   int peer_world = 0, peer_rank = 0;
   float* peer_obs[MAX_PEERS][2] = {};     // [peer][buffer parity]: gathered-rows buffers, double-buffered by control step
   unsigned* peer_flag[MAX_PEERS] = {};    // [peer]: arrival counters [world]
   unsigned peer_epoch = 0;                // control steps signalled so far
-  unsigned* peer_done = nullptr;          // device counter of finished CTAs (in-kernel arrival wait)
+  DevBuf<unsigned> peer_done;             // device counter of finished CTAs (in-kernel arrival wait)
   bool kin_dirty = true;             // the getters' buffers (M, h, poses) do not describe the current state
   bool kin_prestep = false;          // they were written by a full step (integrate2()) and hold stage A of the state before it
   unsigned* prof = nullptr;          // rsb_internal_set_profile
   unsigned* prof_a = nullptr;        // rsb_internal_set_profile_stage_a
-  int* hmap_index = nullptr;         // terrain atlas: map index per environment
-  float* ext = nullptr;              // [N][EXT_WORDS] external wrench rows; ext_active: rows hold a wrench for the next launch
-  bool ext_active = false;
-  // device buffers
-  float *gc = nullptr, *gv = nullptr, *tau = nullptr, *pt = nullptr, *vt = nullptr, *tau_applied = nullptr;
-  int *ncontacts = nullptr, *contact_pt = nullptr, *iters = nullptr, *diverged = nullptr;
-  float* resid = nullptr;
-  int* solver_status = nullptr;
-  rsb_contact* contacts = nullptr;
-  float *dbg_M = nullptr, *dbg_h = nullptr, *dbg_R = nullptr, *dbg_p = nullptr;
-  float* hmap = nullptr;
-  float* staging = nullptr;      // tight-row staging for host<->device repacking
-  float* obs_staging = nullptr;
-  size_t obs_staging_words = 0;
-  size_t staging_words = 0, staging_cursor = 0;
-  uint32_t* blob = nullptr;
-  std::vector<uint32_t> blob_host;
-  BlobHeader hdr{};
-  Dims dims{};
-  WsLayout ws{};
-  int spec = 0;                  // 0 generic, 1 quadruped-12 static dims, 2 humanoid-30 static dims
-  int slots = 1;
   TerrainDesc ter{};
-  std::vector<float> kp, kd;
-  std::vector<int32_t> self_pairs;   // [n][2] collision bodies of the enabled self-collision pairs (rsb_batch_set_self_collision)
-  std::vector<float> self_mu;        // [n] their friction (< 0: default material)
-  int wpc = 0, grid = 0;
-  size_t smem_bytes = 0;
+  DevBuf<float> hmap;
+  DevBuf<int> hmap_index;            // terrain atlas: map index per environment
+  DevBuf<float> ext;                 // [N][EXT_WORDS] external wrench rows; ext_active: rows hold a wrench for the next launch
+  bool ext_active = false;
+  // state and solver outputs, allocated and zeroed by rsb_batch_create
+  DevBuf<float> gc, gv, tau, pt, vt, tau_applied, resid;
+  DevBuf<int> ncontacts, contact_pt, iters, diverged, solver_status;
+  DevBuf<rsb_contact> contacts;
+  DevBuf<float> dbg_M, dbg_h, dbg_R, dbg_p;   // the getters' M, h and poses (ensure_debug)
+  DevBuf<float> stage;               // staging()
+  Overrides ovr;
+  LaunchConfig cfg;
+  DevBuf<uint32_t> blob;
   int64_t launches = 0;
   // RaisimGym task state (rsb_batch_gym_*)
-  float* gym_const = nullptr;     // device: gc_init | gv_init | action_mean | action_std
+  DevBuf<float> gym_const;           // gc_init | gv_init | action_mean | action_std
   GymConfig gym{};
   bool gym_ready = false;
-  float *gym_action = nullptr, *gym_obs = nullptr, *gym_reward = nullptr;
-  unsigned char* gym_done = nullptr;
+  DevBuf<float> gym_action, gym_obs, gym_reward;
+  DevBuf<unsigned char> gym_done;
   // frames of rsb_batch_set_frames (ftab.nf = 0: none): their table and the model's dof columns, in one device allocation
   FrameTable ftab{};
-  int* frame_tab = nullptr;
-  float* frame_staging = nullptr;    // device rows of the frame getters for a host destination (the largest read so far)
-  size_t frame_staging_words = 0;
+  DevBuf<int> frame_tab;
   // contact bodies of rsb_batch_set_contact_bodies (none: empty) and the rows the step kernel fills for them, tight for the current
   // list: cf_force [N][S][3], cf_steps [N][S]; allocated once, for RSB_MAX_CONTACT_BODIES
   std::vector<uint8_t> contact_bodies;
-  float* cf_force = nullptr;
-  int* cf_steps = nullptr;
-  // per-environment inertial rows of rsb_batch_set_body_inertia: bi_rows [N][nb][BI_WORDS], read by every step launch while bi_active.
-  // bi_stage: the same layout, where a call's rows are checked before they replace any of bi_rows; bi_src: a host source's tight rows
-  // on the device; bi_bad: the check's verdict
-  float* bi_rows = nullptr;
-  float* bi_stage = nullptr;
-  float* bi_src = nullptr;
-  int* bi_bad = nullptr;
+  DevBuf<float> cf_force;
+  DevBuf<int> cf_steps;
+  // per-environment inertial rows of rsb_batch_set_body_inertia: bi_rows [N][nb][BI_WORDS], read by every step launch while bi_active;
+  // bi_bad: the verdict of the check a call's rows pass before they replace any of bi_rows
+  DevBuf<float> bi_rows;
+  DevBuf<int> bi_bad;
   bool bi_active = false;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 // ------------------------------------------------------------------ blob ------------------------
-static void build_blob(rsb_batch* b) {
-  const Model& md = b->model->md;
-  BlobHeader& H = b->hdr;
+static void build_blob(const Model& md, const Overrides& ov, LaunchConfig& cfg) {
+  BlobHeader& H = cfg.hdr;
   // dof tree: a floating base is a chain of 6 dofs; dof order is DFS pre-order so subtrees are contiguous
   const int nv = md.nv;
   std::vector<int> dparent(std::max(1, nv), -1), ddepth(std::max(1, nv), 0), dsub(std::max(1, nv), 1), dbody(std::max(1, nv), 0), bdof(md.nb, -1);
@@ -132,9 +155,9 @@ static void build_blob(rsb_batch* b) {
     for (int i = 0; i < nv; i++) if (ddepth[i] == d) { lvldofs.push_back(i); for (int t = 0; t <= d; t++) ent.push_back(i | (t << 8)); }
   }
   lvl[DL] = (int)lvldofs.size(); entstart[DL] = (int)ent.size();
-  b->dims = Dims{md.nb, md.nq, md.nv, md.floating, md.maxdepth, maxdd};
-  const int npairs = (int)b->self_mu.size();
-  H = make_blob_header(b->dims, md.npts(), (int)ent.size(), md.ncoll(), npairs);
+  cfg.dims = Dims{md.nb, md.nq, md.nv, md.floating, md.maxdepth, maxdd};
+  const int npairs = (int)ov.self_mu.size();
+  H = make_blob_header(cfg.dims, md.npts(), (int)ent.size(), md.ncoll(), npairs);
   {
     bool ident = true;
     for (int i = 1; i < md.nb; i++) for (int k = 0; k < 9; k++) if (std::fabs(md.jrot[9 * i + k] - ((k % 4 == 0) ? 1.0 : 0.0)) > 0.0) ident = false;
@@ -143,7 +166,7 @@ static void build_blob(rsb_batch* b) {
     H.flags = (ident ? 1 : 0) | (max_inner << 8);
   }
   const int words = H.words;
-  std::vector<uint32_t>& B = b->blob_host;
+  std::vector<uint32_t>& B = cfg.blob;
   B.assign(words, 0u);
   auto F = [&](int o, float v) { std::memcpy(&B[o], &v, 4); };
   auto I = [&](int o, int v) { std::memcpy(&B[o], &v, 4); };
@@ -167,7 +190,7 @@ static void build_blob(rsb_batch* b) {
     I(H.off_pts + 0 * H.nptp + k, md.pt_body[k]);
     for (int q = 0; q < 3; q++) F(H.off_pts + (1 + q) * H.nptp + k, (float)md.pt_pos[3 * k + q]);
     F(H.off_pts + 4 * H.nptp + k, (float)md.pt_rad[k]);
-    F(H.off_pts + 5 * H.nptp + k, -1.0f);
+    F(H.off_pts + 5 * H.nptp + k, ov.pt_mu[k]);
     I(H.off_pts + 6 * H.nptp + k, md.pt_type[k]);
     for (int q = 0; q < 3; q++) F(H.off_pts + (7 + q) * H.nptp + k, (float)md.pt_pos2[3 * k + q]);
     I(H.off_pts + 10 * H.nptp + k, md.pt_coll[k]);
@@ -190,7 +213,7 @@ static void build_blob(rsb_batch* b) {
     for (int q = 0; q < 9; q++) F(H.off_coll + COLL_WORDS * c + 6 + q, (float)md.crot[9 * c + q]);
   }
   for (int i = 0; i < md.nv; i++) {
-    F(H.off_gain + i, b->kp[i]); F(H.off_gain + H.nvp + i, b->kd[i]); F(H.off_gain + 2 * H.nvp + i, 3.0e38f);
+    F(H.off_gain + i, ov.kp[i]); F(H.off_gain + H.nvp + i, ov.kd[i]); F(H.off_gain + 2 * H.nvp + i, 3.0e38f);
     I(H.off_dofq + i, -1);
   }
   for (int i = 1; i < md.nb; i++) F(H.off_gain + 2 * H.nvp + md.vidx[i], (float)std::min(md.jeffort[i], 3.0e38));   // actuator effort limit per dof
@@ -220,7 +243,7 @@ static void build_blob(rsb_batch* b) {
     }
   }
   for (int j = 0; j < npairs; j++) {   // self-collision pairs (PairField): spheres and capsules as swept segments, sphere-box with the sphere in A
-    const int c1 = b->self_pairs[2 * j], c2 = b->self_pairs[2 * j + 1];
+    const int c1 = ov.self_pairs[2 * j], c2 = ov.self_pairs[2 * j + 1];
     const bool box = md.ctype[c1] == CT_BOX || md.ctype[c2] == CT_BOX, flip = md.ctype[c1] == CT_BOX;
     const int ca = flip ? c2 : c1, cb = flip ? c1 : c2;
     const int o = H.off_pair + PAIR_WORDS * j;
@@ -247,14 +270,12 @@ static void build_blob(rsb_batch* b) {
       F(o + PR_RB, (float)md.csize[3 * cb]);
       cull_b = md.csize[3 * cb] + hb;
     }
-    F(o + PR_MU, b->self_mu[j]);
+    F(o + PR_MU, ov.self_mu[j]);
     // bounding spheres of the stage-B cull, widened so that float32 rounding never culls a touching pair
     F(o + PR_CULL_A, (float)((md.csize[3 * ca] + ha) * 1.0001 + 1e-6)); F(o + PR_CULL_B, (float)(cull_b * 1.0001 + 1e-6));
   }
   std::memcpy(B.data(), &H, sizeof(H));
 }
-
-static void build_ws_layout(rsb_batch* b) { b->ws = make_ws_layout(b->dims, (int)b->self_mu.size()); }
 
 // ------------------------------------------------------------------ launches --------------------
 template <int WPC, int SLOTS, int SPEC>
@@ -268,33 +289,33 @@ static cudaError_t launch_step(const StepArgs& a, int grid, size_t smem, cudaStr
 
 extern "C" int rsb_batch_ob_dim(const rsb_batch* b);
 
-static int pick_config(rsb_batch* b) {
+static int pick_config(const rsb_batch* b, LaunchConfig& c) {
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, b->device));
   // sm_90a code runs on compute capability 9.0 only (arch-specific features are not forward compatible)
   if (prop.major != 9 || prop.minor != 0)
     return fail(RSB_ERR_UNSUPPORTED, "raisimlib_b200 is compiled for sm_90a and needs an H100-class device (compute capability 9.0); found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
   const size_t budget = prop.sharedMemPerBlockOptin;   // 227 KB on H100
-  const size_t blob_bytes = (size_t)b->blob_host.size() * 4;
-  const size_t per_warp = (size_t)b->ws.words * 4;
+  const size_t blob_bytes = (size_t)c.blob.size() * 4;
+  const size_t per_warp = (size_t)c.ws.words * 4;
   const int sms = prop.multiProcessorCount;
-  b->slots = b->model->md.npts() > 32 ? 2 : 1;
+  c.slots = b->model->md.npts() > 32 ? 2 : 1;
   // the static instance of the model's dimensions (step_kernel.cuh SPEC_DIMS), if any
-  b->spec = SPEC_GENERIC;
+  c.spec = SPEC_GENERIC;
   for (int s = SPEC_GENERIC + 1; s < SPEC_COUNT; s++)
-    if (b->dims == SPEC_DIMS[s]) b->spec = s;
+    if (c.dims == SPEC_DIMS[s]) c.spec = s;
   // the quadruped instance has the topology compiled in (floating base + 4 serial chains of 3 joints in DFS order): check it
-  if (b->spec == SPEC_QUAD) {
+  if (c.spec == SPEC_QUAD) {
     const Model& md = b->model->md;
     for (int leg = 0; leg < 4; leg++)
       for (int j = 0; j < 3; j++) {
         const int body = 1 + 3 * leg + j;
-        if (md.parent[body] != (j == 0 ? 0 : body - 1) || md.vidx[body] != 5 + body || md.qidx[body] != 6 + body) b->spec = SPEC_GENERIC;
-        if (md.jtype[body] != 1 && md.jtype[body] != 2) b->spec = SPEC_GENERIC;
+        if (md.parent[body] != (j == 0 ? 0 : body - 1) || md.vidx[body] != 5 + body || md.qidx[body] != 6 + body) c.spec = SPEC_GENERIC;
+        if (md.jtype[body] != 1 && md.jtype[body] != 2) c.spec = SPEC_GENERIC;
       }
   }
-  if (const char* e = getenv("RSB_FORCE_GENERIC")) if (atoi(e)) b->spec = SPEC_GENERIC;
-  if (!b->self_mu.empty()) b->spec = SPEC_GENERIC;   // self-collision pairs are compiled into the generic instance only
+  if (const char* e = getenv("RSB_FORCE_GENERIC")) if (atoi(e)) c.spec = SPEC_GENERIC;
+  if (c.hdr.npairs > 0) c.spec = SPEC_GENERIC;   // self-collision pairs are compiled into the generic instance only
   // Warps per CTA (= resident environments per CTA).  A round of w resident warps per SM costs ~ max(13, w): latency-bound up to a
   // dozen warps, issue-bound beyond.  Choose the option with the smallest rounds x cost, ties to the larger CTA (one sub-step
   // barrier group, one copy of the model block).  On the 132 SMs of an H100, 4096 ANYmal-like environments (7.5 KB workspaces, at
@@ -317,55 +338,81 @@ static int pick_config(rsb_batch* b) {
   }
   if (const char* e = getenv("RSB_FORCE_WPC")) { int w = atoi(e); if (w == 28 || w == 16 || w == 14 || w == 8 || w == 4 || w == 1) if (blob_bytes + (size_t)w * per_warp + 1024 <= budget) best = w; }
   if (best == 0) return fail(RSB_ERR_UNSUPPORTED, "model too large for one warp's shared-memory workspace");
-  b->wpc = best;
-  b->grid = std::min((b->N + best - 1) / best, best == 14 ? 2 * sms : sms);
-  b->smem_bytes = blob_bytes + (size_t)best * per_warp;
+  c.wpc = best;
+  c.grid = std::min((b->N + best - 1) / best, best == 14 ? 2 * sms : sms);
+  c.smem_bytes = blob_bytes + (size_t)best * per_warp;
+  return RSB_OK;
+}
+
+// the launch configuration of overrides `ov`, uploaded on the batch's stream; the batch takes both only when all of it succeeded, so a
+// refused or failed call leaves the batch as it was
+static int rebuild(rsb_batch* b, Overrides ov) {
+  CK(cudaSetDevice(b->device));
+  LaunchConfig c;
+  build_blob(b->model->md, ov, c);
+  c.ws = make_ws_layout(c.dims, c.hdr.npairs);
+  int rc = pick_config(b, c); if (rc) return rc;
+  CK(b->blob.ensure(c.blob.size() * 4, b->stream));
+  CK(cudaMemcpyAsync(b->blob.get(), c.blob.data(), c.blob.size() * 4, cudaMemcpyHostToDevice, b->stream));
+  b->ovr = std::move(ov);
+  b->cfg = std::move(c);
   return RSB_OK;
 }
 
 template <int WPC>
 static cudaError_t dispatch_spec(const rsb_batch* b, const StepArgs& a) {
-  if (b->spec == SPEC_QUAD && b->slots == 1) return launch_step<WPC, 1, SPEC_QUAD>(a, b->grid, b->smem_bytes, b->stream);
-  if (b->spec == SPEC_QUAD) return launch_step<WPC, 2, SPEC_QUAD>(a, b->grid, b->smem_bytes, b->stream);
-  if (b->spec == SPEC_HUMANOID) return launch_step<WPC, 2, SPEC_HUMANOID>(a, b->grid, b->smem_bytes, b->stream);
-  if (b->slots == 1) return launch_step<WPC, 1, SPEC_GENERIC>(a, b->grid, b->smem_bytes, b->stream);
-  return launch_step<WPC, 2, SPEC_GENERIC>(a, b->grid, b->smem_bytes, b->stream);
+  const LaunchConfig& c = b->cfg;
+  if (c.spec == SPEC_QUAD && c.slots == 1) return launch_step<WPC, 1, SPEC_QUAD>(a, c.grid, c.smem_bytes, b->stream);
+  if (c.spec == SPEC_QUAD) return launch_step<WPC, 2, SPEC_QUAD>(a, c.grid, c.smem_bytes, b->stream);
+  if (c.spec == SPEC_HUMANOID) return launch_step<WPC, 2, SPEC_HUMANOID>(a, c.grid, c.smem_bytes, b->stream);
+  if (c.slots == 1) return launch_step<WPC, 1, SPEC_GENERIC>(a, c.grid, c.smem_bytes, b->stream);
+  return launch_step<WPC, 2, SPEC_GENERIC>(a, c.grid, c.smem_bytes, b->stream);
 }
 
-struct GymLaunch { const float* action; float* reward; unsigned char* done; };   // rsb_batch_gym_step: the task fused into the step launch
+// what one launch reads or writes besides the batch's own rows and bindings
+struct LaunchIO {
+  const float* pt = nullptr;     // PD-target rows read in place for this launch only (pinned host rows), stored into the batch's own rows
+  const float* vt = nullptr;     // the same for the velocity targets
+  float* obs = nullptr;          // observation rows
+  bool peers = false;            // ... gathered into the peers' buffers (rsb_batch_set_observation_peers)
+  const float* gym_action = nullptr;   // rsb_batch_gym_step: the task fused into the step launch
+  float* gym_reward = nullptr;
+  unsigned char* gym_done = nullptr;
+};
 
-static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, float* obs_dev = nullptr, bool peers = false, const GymLaunch* gym = nullptr) {
+static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, const LaunchIO& io = {}) {
   StepArgs a{};
   a.num_envs = b->N; a.substeps = substeps;
   a.gc_stride = b->gc_stride; a.gv_stride = b->gv_stride;
-  a.gc = b->gc; a.gv = b->gv; a.tau = b->tau;
+  a.gc = b->gc.get(); a.gv = b->gv.get(); a.tau = b->tau.get();
   a.use_pd = (b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && b->pd_set) ? 1 : 0;
-  a.ptarget = b->pt_bound ? b->pt_bound : b->pt; a.pt_stride = b->pt_bound ? b->pt_bound_stride : b->gc_stride;
-  a.vtarget = b->vt_bound ? b->vt_bound : b->vt; a.vt_stride = b->vt_bound ? b->vt_bound_stride : b->gv_stride;
-  a.pt_store = (b->pt_once && b->pt_bound) ? b->pt : nullptr;
-  a.vt_store = (b->vt_once && b->vt_bound) ? b->vt : nullptr;
-  a.prm = b->prm; a.ter = b->ter; a.ws = b->ws;
-  a.blob_words = (int)b->blob_host.size(); a.blob = b->blob;
-  a.tau_applied = b->tau_applied;
+  a.ptarget = b->pt_bound ? b->pt_bound : b->pt.get(); a.pt_stride = b->pt_bound ? b->pt_bound_stride : b->gc_stride;
+  a.vtarget = b->vt_bound ? b->vt_bound : b->vt.get(); a.vt_stride = b->vt_bound ? b->vt_bound_stride : b->gv_stride;
+  if (io.pt) { a.ptarget = io.pt; a.pt_stride = b->nq; a.pt_store = b->pt.get(); }
+  if (io.vt) { a.vtarget = io.vt; a.vt_stride = b->nv; a.vt_store = b->vt.get(); }
+  a.prm = b->prm; a.ter = b->ter; a.ws = b->cfg.ws;
+  a.blob_words = (int)b->cfg.blob.size(); a.blob = b->blob.get();
+  a.tau_applied = b->tau_applied.get();
   if (phase_mask == 0 && !b->contact_bodies.empty()) {   // only a launch that advances the state accumulates (and overwrites) the contact forces
-    a.cf_force = b->cf_force; a.cf_steps = b->cf_steps; a.cf_n = (int)b->contact_bodies.size();
+    a.cf_force = b->cf_force.get(); a.cf_steps = b->cf_steps.get(); a.cf_n = (int)b->contact_bodies.size();
     std::memcpy(a.cf_body, b->contact_bodies.data(), b->contact_bodies.size());
   }
-  a.ncontacts = b->ncontacts; a.contacts = b->contacts; a.contact_pt = b->contact_pt; a.iters = b->iters; a.diverged = b->diverged; a.resid = b->resid; a.solver_status = b->solver_status;
-  if (debug) { a.dbg_M = b->dbg_M; a.dbg_h = b->dbg_h; a.dbg_R = b->dbg_R; a.dbg_p = b->dbg_p; }
+  a.ncontacts = b->ncontacts.get(); a.contacts = b->contacts.get(); a.contact_pt = b->contact_pt.get(); a.iters = b->iters.get(); a.diverged = b->diverged.get();
+  a.resid = b->resid.get(); a.solver_status = b->solver_status.get();
+  if (debug) { a.dbg_M = b->dbg_M.get(); a.dbg_h = b->dbg_h.get(); a.dbg_R = b->dbg_R.get(); a.dbg_p = b->dbg_p.get(); }
   a.phase_mask = phase_mask; a.prof = b->prof; a.prof_a = b->prof_a;
-  a.ext = b->ext_active ? b->ext : nullptr;
-  a.body_inertia = b->bi_active ? b->bi_rows : nullptr;
-  a.obs = obs_dev; a.ob_dim = rsb_batch_ob_dim(b);
-  if (gym) {       // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
-    a.gym_action = gym->action; a.gym = b->gym; a.gym_reward = gym->reward; a.gym_done = gym->done;
-    a.ptarget = b->pt; a.pt_stride = b->gc_stride; a.pt_store = b->pt;
+  a.ext = b->ext_active ? b->ext.get() : nullptr;
+  a.body_inertia = b->bi_active ? b->bi_rows.get() : nullptr;
+  a.obs = io.obs; a.ob_dim = rsb_batch_ob_dim(b);
+  if (io.gym_action) {   // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
+    a.gym_action = io.gym_action; a.gym = b->gym; a.gym_reward = io.gym_reward; a.gym_done = io.gym_done;
+    a.ptarget = b->pt.get(); a.pt_stride = b->gc_stride; a.pt_store = b->pt.get();
   }
-  if (peers && b->peer_world > 0 && obs_dev && phase_mask == 0) {
+  if (io.peers && b->peer_world > 0 && io.obs && phase_mask == 0) {
     a.peer_world = b->peer_world; a.peer_rank = b->peer_rank;
     for (int p = 0; p < b->peer_world; p++) { a.peer_obs[p] = b->peer_obs[p][b->peer_epoch & 1]; a.peer_flag[p] = b->peer_flag[p]; }
     b->peer_epoch++;
-    a.peer_expected = b->peer_epoch * (unsigned)b->grid; a.peer_done = b->peer_done;
+    a.peer_expected = b->peer_epoch * (unsigned)b->cfg.grid; a.peer_done = b->peer_done.get();
   }
   if (phase_mask == 0) {   // every round of warps re-aligns at each sub-step (the kernel counts the warps of the round)
     const char* e = getenv("RSB_SUBSTEP_BARRIER");   // 0 = off, for A/B runs
@@ -374,7 +421,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
     a.pair_stage_a = p ? atoi(p) : 1;
   }
   cudaError_t e;
-  switch (b->wpc) {
+  switch (b->cfg.wpc) {
     case 28: e = dispatch_spec<28>(b, a); break;
     case 16: e = dispatch_spec<16>(b, a); break;
     case 14: e = dispatch_spec<14>(b, a); break;
@@ -390,21 +437,13 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, flo
   return RSB_OK;
 }
 
-// rows: tight [n][w] <-> padded [n][stride].  Host buffers go through one CONTIGUOUS PCIe copy into a
-// device staging area and are (un)padded on the device: pitched H2D/D2H copies of 76-byte rows are slow.
-// *slot = room for `words` in the staging area; back-to-back calls on the same stream take successive slots and stream order
-// keeps them apart
-static int staging_slot(rsb_batch* b, size_t words, float** slot) {
-  const size_t need = (size_t)b->N * 64 + 64;
-  if (b->staging_words < need) {
-    if (b->staging) { CK(cudaStreamSynchronize(b->stream)); cudaFree(b->staging); b->staging = nullptr; b->staging_words = 0; }
-    CK(cudaMalloc((void**)&b->staging, need * 4));
-    b->staging_words = need;
-  }
-  *slot = b->staging + b->staging_cursor;
-  b->staging_cursor = (b->staging_cursor + words + 31) / 32 * 32;
-  if (b->staging_cursor + (size_t)b->N * 40 > b->staging_words) b->staging_cursor = 0;
-  return RSB_OK;
+// The device buffer that host rows pass through on their way to or from the batch.  Every use is on the batch's stream, so stream
+// order keeps one use apart from the next; a pointer from here is valid until the next call, which may move the buffer.  It starts
+// with room for the rows of any state, target or force copy, so a steady loop of those never grows it.  Null (message set) on failure.
+static float* staging(rsb_batch* b, size_t words) {
+  const cudaError_t e = b->stage.ensure(std::max(words, (size_t)b->N * 64 + 64) * 4, b->stream);
+  if (e != cudaSuccess) { fail(RSB_ERR_CUDA, std::string("staging buffer: ") + cudaGetErrorString(e)); return nullptr; }
+  return b->stage.get();
 }
 // device -> the caller's buffer (where: RSB_HOST / RSB_DEVICE); a host destination has been written when this returns
 static int copy_out(rsb_batch* b, void* dst, const void* src, size_t bytes, int where) {
@@ -412,17 +451,6 @@ static int copy_out(rsb_batch* b, void* dst, const void* src, size_t bytes, int 
   if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
-// a device buffer of the batch that only grows: *buf holds at least `need` floats on return
-static int ensure_scratch(rsb_batch* b, float** buf, size_t* words, size_t need) {
-  if (*words >= need) return RSB_OK;
-  if (*buf) { CK(cudaStreamSynchronize(b->stream)); cudaFree(*buf); }
-  *buf = nullptr; *words = 0;
-  CK(cudaMalloc((void**)buf, need * 4));
-  *words = need;
-  return RSB_OK;
-}
-// device rows of observations for a host destination
-static int ensure_obs_staging(rsb_batch* b) { return ensure_scratch(b, &b->obs_staging, &b->obs_staging_words, (size_t)b->N * rsb_batch_ob_dim(b)); }
 // device-side alias of a pinned, mapped host allocation (cudaHostAlloc / cudaHostRegister / torch pin_memory); null otherwise
 static const float* mapped_alias(const void* host) {
   cudaPointerAttributes at{};
@@ -430,12 +458,13 @@ static const float* mapped_alias(const void* host) {
   if (at.type == cudaMemoryTypeHost && at.devicePointer) return static_cast<const float*>(at.devicePointer);
   return nullptr;
 }
+// rows: tight [n][w] <-> padded [n][stride].  Host buffers go through one CONTIGUOUS PCIe copy into the staging buffer and are
+// (un)padded on the device: pitched H2D/D2H copies of 76-byte rows are slow.
 static int copy_rows_in(rsb_batch* b, float* dst, int stride, const float* src, int w, int env_begin, int n, int where) {
   if (!src || n == 0) return RSB_OK;
   const float* dsrc = src;
   if (where == RSB_HOST) {
-    float* st = nullptr;
-    int rc = staging_slot(b, (size_t)n * w, &st); if (rc) return rc;
+    float* st = staging(b, (size_t)n * w); if (!st) return RSB_ERR_CUDA;
     CK(cudaMemcpyAsync(st, src, (size_t)n * w * 4, cudaMemcpyHostToDevice, b->stream));
     dsrc = st;
   }
@@ -445,8 +474,7 @@ static int copy_rows_in(rsb_batch* b, float* dst, int stride, const float* src, 
 static int copy_rows_out(rsb_batch* b, float* dst, const float* src, int stride, int w, int env_begin, int n, int where) {
   if (!dst || n == 0) return RSB_OK;
   if (where == RSB_HOST) {
-    float* st = nullptr;
-    int rc = staging_slot(b, (size_t)n * w, &st); if (rc) return rc;
+    float* st = staging(b, (size_t)n * w); if (!st) return RSB_ERR_CUDA;
     CK(cudaMemcpy2DAsync(st, (size_t)w * 4, src + (size_t)env_begin * stride, (size_t)stride * 4, (size_t)w * 4, n, cudaMemcpyDeviceToDevice, b->stream));
     CK(cudaMemcpyAsync(dst, st, (size_t)n * w * 4, cudaMemcpyDeviceToHost, b->stream));
   } else {
@@ -454,9 +482,12 @@ static int copy_rows_out(rsb_batch* b, float* dst, const float* src, int stride,
   }
   return RSB_OK;
 }
-static int check_range(const rsb_batch* b, int env_begin, int env_count) {
+static bool bad_where(int where) { return where != RSB_HOST && where != RSB_DEVICE; }
+// the checks of every entry point that copies rows of a range of environments to or from the caller's memory
+static int check_range(const rsb_batch* b, int env_begin, int env_count, int where) {
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
   if (env_begin < 0 || env_count < 0 || env_begin + env_count > b->N) return fail(RSB_ERR_INVALID, "environment range out of bounds");
+  if (bad_where(where)) return fail(RSB_ERR_INVALID, "`where` must be RSB_HOST or RSB_DEVICE");
   return RSB_OK;
 }
 
@@ -559,38 +590,31 @@ int rsb_batch_create(const rsb_model* m, int num_envs, int device, rsb_batch** o
   b->nq = md.nq; b->nv = md.nv; b->nb = md.nb;
   b->gc_stride = round_up(std::max(1, md.nq), 8); b->gv_stride = round_up(std::max(1, md.nv), 8);   // 32-byte sector-aligned rows
   rsb_params_default(&b->prm);
-  b->kp.assign(std::max(1, md.nv), 0.f); b->kd.assign(std::max(1, md.nv), 0.f);
-  build_blob(b);
-  build_ws_layout(b);
-  int rc = pick_config(b);
-  if (rc != RSB_OK) { delete b; return rc; }
-  size_t N = (size_t)num_envs;
-  auto alloc = [&](void** p, size_t bytes) { cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 16)); if (e == cudaSuccess) e = cudaMemset(*p, 0, std::max<size_t>(bytes, 16)); return e; };
-  cudaError_t e = cudaSuccess;
-  if (e == cudaSuccess) e = alloc((void**)&b->gc, N * b->gc_stride * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->gv, N * b->gv_stride * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->tau, N * b->gv_stride * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->pt, N * b->gc_stride * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->vt, N * b->gv_stride * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->tau_applied, N * b->gv_stride * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->ncontacts, N * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->contact_pt, N * KMAX * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->iters, N * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->diverged, N * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->resid, N * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->solver_status, N * 4);
-  if (e == cudaSuccess) e = alloc((void**)&b->contacts, N * KMAX * sizeof(rsb_contact));
-  if (e == cudaSuccess) e = alloc((void**)&b->blob, b->blob_host.size() * 4);
-  if (e == cudaSuccess) e = cudaMemcpy(b->blob, b->blob_host.data(), b->blob_host.size() * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) { std::string msg = cudaGetErrorString(e); rsb_batch_destroy(b); return fail(RSB_ERR_CUDA, "rsb_batch_create: " + msg); }
+  cudaError_t e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking);
+  if (e != cudaSuccess) { delete b; return fail(RSB_ERR_CUDA, std::string("rsb_batch_create: ") + cudaGetErrorString(e)); }
   b->own_stream = true;
-  // identity quaternion so that a fresh batch is a valid state
-  if (md.floating) {
-    std::vector<float> q0((size_t)N * b->gc_stride, 0.f);
+  Overrides ov;
+  ov.kp.assign(std::max(1, md.nv), 0.f); ov.kd.assign(std::max(1, md.nv), 0.f);
+  ov.pt_mu.assign(md.npts(), -1.f);
+  const int rc = rebuild(b, std::move(ov));
+  if (rc != RSB_OK) { rsb_batch_destroy(b); return rc; }
+  const size_t N = (size_t)num_envs;
+  auto zeroed = [&](auto& buf, size_t bytes) {
+    bytes = std::max<size_t>(bytes, 16);
+    if (e == cudaSuccess) e = buf.ensure(bytes, b->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(buf.get(), 0, bytes, b->stream);
+  };
+  zeroed(b->gc, N * b->gc_stride * 4); zeroed(b->gv, N * b->gv_stride * 4); zeroed(b->tau, N * b->gv_stride * 4);
+  zeroed(b->pt, N * b->gc_stride * 4); zeroed(b->vt, N * b->gv_stride * 4); zeroed(b->tau_applied, N * b->gv_stride * 4);
+  zeroed(b->ncontacts, N * 4); zeroed(b->contact_pt, N * KMAX * 4); zeroed(b->iters, N * 4); zeroed(b->diverged, N * 4);
+  zeroed(b->resid, N * 4); zeroed(b->solver_status, N * 4); zeroed(b->contacts, N * KMAX * sizeof(rsb_contact));
+  if (e == cudaSuccess && md.floating) {   // identity quaternion so that a fresh batch is a valid state
+    std::vector<float> q0(N * b->gc_stride, 0.f);
     for (size_t i = 0; i < N; i++) q0[i * b->gc_stride + 3] = 1.f;
-    cudaMemcpy(b->gc, q0.data(), q0.size() * 4, cudaMemcpyHostToDevice);
+    e = cudaMemcpyAsync(b->gc.get(), q0.data(), q0.size() * 4, cudaMemcpyHostToDevice, b->stream);
   }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
+  if (e != cudaSuccess) { std::string msg = cudaGetErrorString(e); rsb_batch_destroy(b); return fail(RSB_ERR_CUDA, "rsb_batch_create: " + msg); }
   *out = b;
   return RSB_OK;
 }
@@ -599,14 +623,8 @@ void rsb_batch_destroy(rsb_batch* b) {
   if (!b) return;
   cudaSetDevice(b->device);
   if (b->stream) cudaStreamSynchronize(b->stream);
-  for (void* p : {(void*)b->solver_status, (void*)b->resid, (void*)b->diverged, (void*)b->tau_applied, (void*)b->gc, (void*)b->gv, (void*)b->tau, (void*)b->pt, (void*)b->vt, (void*)b->ncontacts, (void*)b->contact_pt, (void*)b->iters,
-                  (void*)b->contacts, (void*)b->dbg_M, (void*)b->dbg_h, (void*)b->dbg_R, (void*)b->dbg_p, (void*)b->hmap, (void*)b->staging, (void*)b->obs_staging, (void*)b->blob, (void*)b->gym_const, (void*)b->gym_action,
-                  (void*)b->gym_obs, (void*)b->gym_reward, (void*)b->gym_done, (void*)b->ext, (void*)b->hmap_index, (void*)b->peer_done,
-                  (void*)b->frame_tab, (void*)b->frame_staging, (void*)b->cf_force, (void*)b->cf_steps, (void*)b->bi_rows, (void*)b->bi_stage,
-                  (void*)b->bi_src, (void*)b->bi_bad})
-    if (p) cudaFree(p);
   if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
-  delete b;
+  delete b;   // frees the batch's device buffers
 }
 
 int rsb_batch_set_stream(rsb_batch* b, void* s) {
@@ -637,23 +655,21 @@ int rsb_batch_clear_terrain(rsb_batch* b) {
 static int upload_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_size, float y_size, float cx, float cy, const float* h,
                              const int32_t* map_of_env) {
   CK(cudaSetDevice(b->device));
-  CK(cudaStreamSynchronize(b->stream));
-  if (b->hmap) { cudaFree(b->hmap); b->hmap = nullptr; }
-  if (b->hmap_index) { cudaFree(b->hmap_index); b->hmap_index = nullptr; }
-  b->ter = TerrainDesc{};               // nothing may point at the freed maps if an allocation below fails
+  CK(cudaStreamSynchronize(b->stream));   // no launch still reads the maps overwritten below
+  b->ter = TerrainDesc{};               // nothing may point at half-written maps if a step below fails
   const size_t words = (size_t)count * xs * ys;
-  CK(cudaMalloc((void**)&b->hmap, words * 4));
-  CK(cudaMemcpy(b->hmap, h, words * 4, cudaMemcpyHostToDevice));
+  CK(b->hmap.ensure(words * 4, b->stream));
+  CK(cudaMemcpy(b->hmap.get(), h, words * 4, cudaMemcpyHostToDevice));
   if (map_of_env) {
-    CK(cudaMalloc((void**)&b->hmap_index, (size_t)b->N * 4));
-    CK(cudaMemcpy(b->hmap_index, map_of_env, (size_t)b->N * 4, cudaMemcpyHostToDevice));
+    CK(b->hmap_index.ensure((size_t)b->N * 4, b->stream));
+    CK(cudaMemcpy(b->hmap_index.get(), map_of_env, (size_t)b->N * 4, cudaMemcpyHostToDevice));
   }
   TerrainDesc t{};
   t.type = 2; t.xs = xs; t.ys = ys;
   t.dx = x_size / (float)(xs - 1); t.dy = y_size / (float)(ys - 1); t.inv_dx = 1.0f / t.dx; t.inv_dy = 1.0f / t.dy;
   t.x0 = cx - 0.5f * x_size; t.y0 = cy - 0.5f * y_size;
   t.xmax = (float)(xs - 1); t.ymax = (float)(ys - 1);
-  t.h = b->hmap; t.env_map = b->hmap_index; t.map_words = xs * ys;
+  t.h = b->hmap.get(); t.env_map = map_of_env ? b->hmap_index.get() : nullptr; t.map_words = xs * ys;
   t.hmax = h[0];
   for (size_t i = 1; i < words; i++) t.hmax = std::max(t.hmax, h[i]);
   b->ter = t;
@@ -688,29 +704,25 @@ int rsb_batch_get_params(const rsb_batch* b, rsb_params* p) {
 }
 
 int rsb_batch_set_state(rsb_batch* b, const float* gc, const float* gv, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   b->kin_dirty = true;
-  rc = copy_rows_in(b, b->gc, b->gc_stride, gc, b->nq, env_begin, env_count, where); if (rc) return rc;
-  return copy_rows_in(b, b->gv, b->gv_stride, gv, b->nv, env_begin, env_count, where);
+  rc = copy_rows_in(b, b->gc.get(), b->gc_stride, gc, b->nq, env_begin, env_count, where); if (rc) return rc;
+  return copy_rows_in(b, b->gv.get(), b->gv_stride, gv, b->nv, env_begin, env_count, where);
 }
 int rsb_batch_get_state(rsb_batch* b, float* gc, float* gv, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
-  rc = copy_rows_out(b, gc, b->gc, b->gc_stride, b->nq, env_begin, env_count, where); if (rc) return rc;
-  rc = copy_rows_out(b, gv, b->gv, b->gv_stride, b->nv, env_begin, env_count, where); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  rc = copy_rows_out(b, gc, b->gc.get(), b->gc_stride, b->nq, env_begin, env_count, where); if (rc) return rc;
+  rc = copy_rows_out(b, gv, b->gv.get(), b->gv_stride, b->nv, env_begin, env_count, where); if (rc) return rc;
   if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
 int rsb_batch_set_pd_gains(rsb_batch* b, const float* kp, const float* kd) {
   if (!b || !kp || !kd) return fail(RSB_ERR_INVALID, "null argument");
   const Model& md = b->model->md;
-  for (int i = 0; i < md.nv; i++) { b->kp[i] = kp[i]; b->kd[i] = kd[i]; }
-  if (md.floating) for (int i = 0; i < 6; i++) { b->kp[i] = 0.f; b->kd[i] = 0.f; }   // the base is not actuated
-  for (int i = 0; i < md.nv; i++) {
-    std::memcpy(&b->blob_host[b->hdr.off_gain + i], &b->kp[i], 4);
-    std::memcpy(&b->blob_host[b->hdr.off_gain + b->hdr.nvp + i], &b->kd[i], 4);
-  }
-  CK(cudaMemcpyAsync(b->blob + b->hdr.off_gain, b->blob_host.data() + b->hdr.off_gain, (size_t)2 * b->hdr.nvp * 4, cudaMemcpyHostToDevice, b->stream));
-  CK(cudaStreamSynchronize(b->stream));
+  Overrides ov = b->ovr;
+  for (int i = 0; i < md.nv; i++) { ov.kp[i] = kp[i]; ov.kd[i] = kd[i]; }
+  if (md.floating) for (int i = 0; i < 6; i++) { ov.kp[i] = 0.f; ov.kd[i] = 0.f; }   // the base is not actuated
+  const int rc = rebuild(b, std::move(ov)); if (rc) return rc;
   b->pd_set = true;
   return RSB_OK;
 }
@@ -720,11 +732,9 @@ int rsb_batch_set_collision_friction(rsb_batch* b, int collision_body, float mu)
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
   const Model& md = b->model->md;
   if (collision_body < 0 || collision_body >= md.ncoll()) return fail(RSB_ERR_INVALID, "collision body index out of range");
-  const BlobHeader& H = b->hdr;
-  for (int k = 0; k < md.npts(); k++) if (md.pt_coll[k] == collision_body) std::memcpy(&b->blob_host[H.off_pts + 5 * H.nptp + k], &mu, 4);
-  CK(cudaMemcpyAsync(b->blob + H.off_pts + 5 * H.nptp, b->blob_host.data() + H.off_pts + 5 * H.nptp, (size_t)H.nptp * 4, cudaMemcpyHostToDevice, b->stream));
-  CK(cudaStreamSynchronize(b->stream));
-  return RSB_OK;
+  Overrides ov = b->ovr;
+  for (int k = 0; k < md.npts(); k++) if (md.pt_coll[k] == collision_body) ov.pt_mu[k] = mu;
+  return rebuild(b, std::move(ov));
 }
 // self-collision between explicit pairs of collision bodies (n = 0: none, the default).  Everything is checked before anything changes:
 // a refused call leaves the batch as it was.  The pair table goes to the end of the model blob; a batch with pairs runs the generic
@@ -749,41 +759,18 @@ int rsb_batch_set_self_collision(rsb_batch* b, const int32_t* pairs, int n, cons
                                            " is not supported (sphere-sphere, sphere-capsule, capsule-capsule and sphere-box are)");
     if (mu && !(mu[j] < 0.f || mu[j] >= 0.f)) return fail(RSB_ERR_INVALID, "self-collision pair " + std::to_string(j) + ": friction is not a number");
   }
-  CK(cudaSetDevice(b->device));
-  CK(cudaStreamSynchronize(b->stream));
-  // the friction overrides of rsb_batch_set_collision_friction live in the blob: carry them over (the candidate table does not move)
-  const std::vector<uint32_t> old_fric(b->blob_host.begin() + b->hdr.off_pts + 5 * b->hdr.nptp, b->blob_host.begin() + b->hdr.off_pts + 6 * b->hdr.nptp);
-  std::vector<int32_t> old_pairs = b->self_pairs; std::vector<float> old_mu = b->self_mu;
-  auto apply = [&]() -> int {
-    build_blob(b);
-    std::copy(old_fric.begin(), old_fric.end(), b->blob_host.begin() + b->hdr.off_pts + 5 * b->hdr.nptp);
-    build_ws_layout(b);
-    return pick_config(b);
-  };
-  b->self_pairs.assign(pairs ? pairs : nullptr, pairs ? pairs + 2 * n : nullptr);
-  b->self_mu.assign(n, -1.f);
-  for (int j = 0; j < n && mu; j++) b->self_mu[j] = mu[j];
-  int rc = apply();
-  uint32_t* blob = nullptr;
-  if (rc == RSB_OK && cudaMalloc((void**)&blob, b->blob_host.size() * 4) != cudaSuccess) rc = fail(RSB_ERR_CUDA, "rsb_batch_set_self_collision: out of device memory");
-  if (rc != RSB_OK) {   // back to the previous pair set (the message of the failure stays)
-    const std::string msg = g_err;
-    b->self_pairs = old_pairs; b->self_mu = old_mu;
-    apply();
-    g_err = msg;
-    return rc;
-  }
-  CK(cudaMemcpy(blob, b->blob_host.data(), b->blob_host.size() * 4, cudaMemcpyHostToDevice));
-  cudaFree(b->blob);
-  b->blob = blob;
-  return RSB_OK;
+  Overrides ov = b->ovr;
+  ov.self_pairs.assign(pairs ? pairs : nullptr, pairs ? pairs + 2 * n : nullptr);
+  ov.self_mu.assign(n, -1.f);
+  for (int j = 0; j < n && mu; j++) ov.self_mu[j] = mu[j];
+  return rebuild(b, std::move(ov));
 }
 
 int rsb_batch_set_pd_target(rsb_batch* b, const float* ptarget, const float* vtarget, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (ptarget) b->pt_bound = nullptr;     // copying targets in ends a zero-copy binding
-  rc = copy_rows_in(b, b->pt, b->gc_stride, ptarget, b->nq, env_begin, env_count, where); if (rc) return rc;
-  return copy_rows_in(b, b->vt, b->gv_stride, vtarget, b->nv, env_begin, env_count, where);
+  rc = copy_rows_in(b, b->pt.get(), b->gc_stride, ptarget, b->nq, env_begin, env_count, where); if (rc) return rc;
+  return copy_rows_in(b, b->vt.get(), b->gv_stride, vtarget, b->nv, env_begin, env_count, where);
 }
 int rsb_batch_bind_pd_target(rsb_batch* b, const float* ptarget_device, int row_stride) {
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
@@ -792,12 +779,12 @@ int rsb_batch_bind_pd_target(rsb_batch* b, const float* ptarget_device, int row_
   return RSB_OK;
 }
 int rsb_batch_set_generalized_force(rsb_batch* b, const float* tau, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
-  return copy_rows_in(b, b->tau, b->gv_stride, tau, b->nv, env_begin, env_count, where);
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  return copy_rows_in(b, b->tau.get(), b->gv_stride, tau, b->nv, env_begin, env_count, where);
 }
 int rsb_batch_get_generalized_force(rsb_batch* b, float* tau, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
-  rc = copy_rows_out(b, tau, b->tau_applied, b->gv_stride, b->nv, env_begin, env_count, where); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  rc = copy_rows_out(b, tau, b->tau_applied.get(), b->gv_stride, b->nv, env_begin, env_count, where); if (rc) return rc;
   if (where == RSB_HOST) CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
@@ -805,25 +792,24 @@ int rsb_batch_get_generalized_force(rsb_batch* b, float* tau, int env_begin, int
 // acting on `body` at `point_body` (body frame; null = body origin), world-frame force / torque rows (null = zero).
 // It acts during the next integrate() / control-step call (all of its fused sub-steps) and is cleared afterwards.
 int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, const float* torque, const float* point_body, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (body < 0 || body >= b->nb) return fail(RSB_ERR_INVALID, "external wrench: body index out of range");
   if (env_count == 0) return RSB_OK;
   CK(cudaSetDevice(b->device));
-  if (!b->ext) CK(cudaMalloc((void**)&b->ext, (size_t)b->N * EXT_WORDS * 4));
+  CK(b->ext.ensure((size_t)b->N * EXT_WORDS * 4, b->stream));
   if (!b->ext_active) {   // rows of an earlier call are stale: body = -1 everywhere
-    CK(cudaMemsetAsync(b->ext, 0xff, (size_t)b->N * EXT_WORDS * 4, b->stream));
+    CK(cudaMemsetAsync(b->ext.get(), 0xff, (size_t)b->N * EXT_WORDS * 4, b->stream));
     b->ext_active = true;
   }
   const float *df = force, *dtq = torque;
   if (where == RSB_HOST && (force || torque)) {
-    float* st = nullptr;
-    rc = staging_slot(b, (size_t)env_count * 6, &st); if (rc) return rc;
+    float* st = staging(b, (size_t)env_count * 6); if (!st) return RSB_ERR_CUDA;   // force rows, then torque rows
     if (force) { CK(cudaMemcpyAsync(st, force, (size_t)env_count * 12, cudaMemcpyHostToDevice, b->stream)); df = st; }
     if (torque) { CK(cudaMemcpyAsync(st + (size_t)env_count * 3, torque, (size_t)env_count * 12, cudaMemcpyHostToDevice, b->stream)); dtq = st + (size_t)env_count * 3; }
   }
   const float px = point_body ? point_body[0] : 0.f, py = point_body ? point_body[1] : 0.f, pz = point_body ? point_body[2] : 0.f;
   const int threads = 128, blocks = (env_count + threads - 1) / threads;
-  rsb_ext_pack_kernel<<<blocks, threads, 0, b->stream>>>(b->ext + (size_t)env_begin * EXT_WORDS, body, df, dtq, px, py, pz, env_count);
+  rsb_ext_pack_kernel<<<blocks, threads, 0, b->stream>>>(b->ext.get() + (size_t)env_begin * EXT_WORDS, body, df, dtq, px, py, pz, env_count);
   CK(cudaGetLastError());
   return RSB_OK;
 }
@@ -841,31 +827,30 @@ static std::vector<float> model_inertia_rows(const Model& md, int n) {
   return r;
 }
 int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
-  if (where != RSB_HOST && where != RSB_DEVICE) return fail(RSB_ERR_INVALID, "body inertia: `where` must be RSB_HOST or RSB_DEVICE");
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (env_count == 0) return RSB_OK;
   CK(cudaSetDevice(b->device));
   const Model& md = b->model->md;
   const size_t per_env = (size_t)md.nb * BI_WORDS, all = (size_t)b->N * per_env;
   const float* staged = nullptr;
   std::vector<float> model_rows;
-  if (rows) {   // check the caller's rows in bi_stage; nothing of bi_rows changes unless every value is accepted
-    if (!b->bi_stage) CK(cudaMalloc((void**)&b->bi_stage, all * 4));
-    if (!b->bi_bad) CK(cudaMalloc((void**)&b->bi_bad, 4));
-    const float* src = rows;
+  if (rows) {   // check the caller's rows in the staging buffer; nothing of bi_rows changes unless every value is accepted
+    CK(b->bi_bad.ensure(4, b->stream));
     const size_t nrows = (size_t)env_count * md.nb;
+    // the checked rows [nrows][BI_WORDS], then a host source's tight rows [nrows][10]
+    float* const st = staging(b, nrows * BI_WORDS + (where == RSB_HOST ? nrows * 10 : 0)); if (!st) return RSB_ERR_CUDA;
+    const float* src = rows;
     if (where == RSB_HOST) {
-      if (!b->bi_src) CK(cudaMalloc((void**)&b->bi_src, (size_t)b->N * md.nb * 10 * 4));
-      CK(cudaMemcpyAsync(b->bi_src, rows, nrows * 10 * 4, cudaMemcpyHostToDevice, b->stream));
-      src = b->bi_src;
+      CK(cudaMemcpyAsync(st + nrows * BI_WORDS, rows, nrows * 10 * 4, cudaMemcpyHostToDevice, b->stream));
+      src = st + nrows * BI_WORDS;
     }
     const int ok = 0x7fffffff;
-    CK(cudaMemcpyAsync(b->bi_bad, &ok, 4, cudaMemcpyHostToDevice, b->stream));
+    CK(cudaMemcpyAsync(b->bi_bad.get(), &ok, 4, cudaMemcpyHostToDevice, b->stream));
     const int threads = 128;
-    rsb_body_inertia_pack_kernel<<<(unsigned)((nrows + threads - 1) / threads), threads, 0, b->stream>>>(b->bi_stage, src, (int)nrows, 1e-6, b->bi_bad);
+    rsb_body_inertia_pack_kernel<<<(unsigned)((nrows + threads - 1) / threads), threads, 0, b->stream>>>(st, src, (int)nrows, 1e-6, b->bi_bad.get());
     CK(cudaGetLastError());
     int bad = ok;
-    CK(cudaMemcpyAsync(&bad, b->bi_bad, 4, cudaMemcpyDeviceToHost, b->stream));
+    CK(cudaMemcpyAsync(&bad, b->bi_bad.get(), 4, cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
     if (bad != ok) {
       static const char* what[] = {"", "a value that is not finite", "a negative mass", "an inertia that is not symmetric positive semidefinite"};
@@ -873,18 +858,18 @@ int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, i
       return fail(RSB_ERR_INVALID, "body inertia: environment " + std::to_string(env) + ", body " + std::to_string(body) + " (" + md.body_names[body] + ") has " + what[bad & 3] +
                                    "; no row changed");
     }
-    staged = b->bi_stage;
+    staged = st;
   } else {
     model_rows = model_inertia_rows(md, env_count);
   }
   // commit: the first call after creation or rsb_batch_clear_body_inertia starts every environment from the model's rows
-  if (!b->bi_rows) CK(cudaMalloc((void**)&b->bi_rows, all * 4));
+  CK(b->bi_rows.ensure(all * 4, b->stream));
   if (!b->bi_active) {
     const std::vector<float> init = model_inertia_rows(md, b->N);
-    CK(cudaMemcpyAsync(b->bi_rows, init.data(), all * 4, cudaMemcpyHostToDevice, b->stream));
+    CK(cudaMemcpyAsync(b->bi_rows.get(), init.data(), all * 4, cudaMemcpyHostToDevice, b->stream));
     CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
   }
-  float* const at = b->bi_rows + (size_t)env_begin * per_env;
+  float* const at = b->bi_rows.get() + (size_t)env_begin * per_env;
   if (staged) CK(cudaMemcpyAsync(at, staged, (size_t)env_count * per_env * 4, cudaMemcpyDeviceToDevice, b->stream));
   else {
     CK(cudaMemcpyAsync(at, model_rows.data(), model_rows.size() * 4, cudaMemcpyHostToDevice, b->stream));
@@ -907,12 +892,11 @@ int rsb_batch_set_control_mode(rsb_batch* b, int mode) {
 }
 
 static int ensure_debug(rsb_batch* b) {
-  if (b->dbg_M) return RSB_OK;
-  size_t N = (size_t)b->N;
-  CK(cudaMalloc((void**)&b->dbg_M, std::max<size_t>(16, N * b->nv * b->nv * 4)));
-  CK(cudaMalloc((void**)&b->dbg_h, std::max<size_t>(16, N * b->nv * 4)));
-  CK(cudaMalloc((void**)&b->dbg_R, N * b->nb * 9 * 4));
-  CK(cudaMalloc((void**)&b->dbg_p, N * b->nb * 3 * 4));
+  const size_t N = (size_t)b->N;
+  CK(b->dbg_M.ensure(std::max<size_t>(16, N * b->nv * b->nv * 4), b->stream));
+  CK(b->dbg_h.ensure(std::max<size_t>(16, N * b->nv * 4), b->stream));
+  CK(b->dbg_R.ensure(N * b->nb * 9 * 4, b->stream));
+  CK(b->dbg_p.ensure(N * b->nb * 3 * 4, b->stream));
   return RSB_OK;
 }
 
@@ -930,7 +914,7 @@ int rsb_batch_update_kinematics(rsb_batch* b) {
 }
 // lazy getters: refresh M, h and the poses when the state changed through this API since they were last computed
 static int ensure_kinematics(rsb_batch* b) {
-  if (b->dbg_M && !b->kin_dirty) return RSB_OK;
+  if (b->dbg_M.get() && !b->kin_dirty) return RSB_OK;
   return rsb_batch_update_kinematics(b);
 }
 int rsb_batch_integrate2(rsb_batch* b) {
@@ -938,7 +922,7 @@ int rsb_batch_integrate2(rsb_batch* b) {
   CK(cudaSetDevice(b->device));
   // state is unchanged since integrate1(), so the fused step recomputes stage A-B on-chip and goes on;
   // generalized forces / PD targets set between integrate1() and integrate2() are honoured
-  return do_launch(b, 1, 0, b->dbg_M != nullptr);
+  return do_launch(b, 1, 0, b->dbg_M.get() != nullptr);
 }
 int rsb_batch_integrate(rsb_batch* b, int substeps) {
   if (!b || substeps < 1) return fail(RSB_ERR_INVALID, "bad arguments to rsb_batch_integrate");
@@ -947,26 +931,26 @@ int rsb_batch_integrate(rsb_batch* b, int substeps) {
 }
 
 int rsb_batch_get_mass_matrix(rsb_batch* b, int env_begin, int env_count, float* out, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!out) return fail(RSB_ERR_INVALID, "null output buffer");
   if (env_count == 0) return RSB_OK;
   rc = ensure_kinematics(b); if (rc) return rc;
   const size_t w = (size_t)b->nv * b->nv;
-  return copy_out(b, out, b->dbg_M + env_begin * w, env_count * w * 4, where);
+  return copy_out(b, out, b->dbg_M.get() + env_begin * w, env_count * w * 4, where);
 }
 int rsb_batch_get_nonlinearities(rsb_batch* b, int env_begin, int env_count, float* out, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!out) return fail(RSB_ERR_INVALID, "null output buffer");
   if (env_count == 0) return RSB_OK;
   rc = ensure_kinematics(b); if (rc) return rc;
-  return copy_out(b, out, b->dbg_h + (size_t)env_begin * b->nv, (size_t)env_count * b->nv * 4, where);
+  return copy_out(b, out, b->dbg_h.get() + (size_t)env_begin * b->nv, (size_t)env_count * b->nv * 4, where);
 }
 int rsb_batch_get_body_poses(rsb_batch* b, int env_begin, int env_count, float* rot, float* pos, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (env_count == 0) return RSB_OK;
   rc = ensure_kinematics(b); if (rc) return rc;
-  rc = rot ? copy_out(b, rot, b->dbg_R + (size_t)env_begin * b->nb * 9, (size_t)env_count * b->nb * 9 * 4, where) : RSB_OK; if (rc) return rc;
-  return pos ? copy_out(b, pos, b->dbg_p + (size_t)env_begin * b->nb * 3, (size_t)env_count * b->nb * 3 * 4, where) : RSB_OK;
+  rc = rot ? copy_out(b, rot, b->dbg_R.get() + (size_t)env_begin * b->nb * 9, (size_t)env_count * b->nb * 9 * 4, where) : RSB_OK; if (rc) return rc;
+  return pos ? copy_out(b, pos, b->dbg_p.get() + (size_t)env_begin * b->nb * 3, (size_t)env_count * b->nb * 3 * 4, where) : RSB_OK;
 }
 
 // ---- frame kinematics: pose, velocity and Jacobian of frames rigidly attached to bodies, from the kinematics pass's poses ----------
@@ -1012,17 +996,17 @@ int rsb_batch_set_frames(rsb_batch* b, const int32_t* body, const float* pos, co
     W[o_anc + i] = (int32_t)m;
   }
   CK(cudaSetDevice(b->device));
-  if (!b->frame_tab) CK(cudaMalloc((void**)&b->frame_tab, (size_t)words * 4));   // sized for RSB_MAX_FRAMES: the layout never moves
-  CK(cudaMemcpyAsync(b->frame_tab, W.data(), (size_t)words * 4, cudaMemcpyHostToDevice, b->stream));
+  CK(b->frame_tab.ensure((size_t)words * 4, b->stream));   // sized for RSB_MAX_FRAMES: the layout never moves
+  CK(cudaMemcpyAsync(b->frame_tab.get(), W.data(), (size_t)words * 4, cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
-  const int* T = b->frame_tab;
+  const int* T = b->frame_tab.get();
   b->ftab = FrameTable{n, nb, nv, T, T + o_flags, (const float*)(T + o_pos), (const float*)(T + o_rot), T + o_dbody, T + o_dkind,
                        (const float*)(T + o_axis), (const unsigned*)(T + o_anc)};
   return RSB_OK;
 }
 // one launch of rsb_frame_kernel (after the kinematics pass when the poses are stale); out = {pos, rot, lin_vel, ang_vel, jac}
 static int frame_outputs(rsb_batch* b, int env_begin, int env_count, float* const out[5], int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (b->ftab.nf == 0) return fail(RSB_ERR_INVALID, "no frames: call rsb_batch_set_frames() first");
   if (env_count == 0 || !(out[0] || out[1] || out[2] || out[3] || out[4])) return RSB_OK;
   CK(cudaSetDevice(b->device));
@@ -1034,13 +1018,12 @@ static int frame_outputs(rsb_batch* b, int env_begin, int env_count, float* cons
   if (where == RSB_HOST) {
     size_t need = 0;
     for (int k = 0; k < 5; k++) if (out[k]) need += rows * per[k];
-    rc = ensure_scratch(b, &b->frame_staging, &b->frame_staging_words, need); if (rc) return rc;
-    float* s = b->frame_staging;
+    float* s = staging(b, need); if (!s) return RSB_ERR_CUDA;
     for (int k = 0; k < 5; k++) if (out[k]) { dst[k] = s; s += rows * per[k]; }
   }
   const int threads = 128;
   const unsigned blocks = (unsigned)((rows * 32 + threads - 1) / threads);
-  rsb_frame_kernel<<<blocks, threads, 0, b->stream>>>(b->ftab, b->dbg_R, b->dbg_p, b->gv, b->gv_stride, env_begin, env_count, dst[0], dst[1], dst[2], dst[3], dst[4]);
+  rsb_frame_kernel<<<blocks, threads, 0, b->stream>>>(b->ftab, b->dbg_R.get(), b->dbg_p.get(), b->gv.get(), b->gv_stride, env_begin, env_count, dst[0], dst[1], dst[2], dst[3], dst[4]);
   CK(cudaGetLastError());
   b->launches++;
   if (where != RSB_HOST) return RSB_OK;
@@ -1052,7 +1035,7 @@ int rsb_batch_get_frame_states(rsb_batch* b, int env_begin, int env_count, float
   return frame_outputs(b, env_begin, env_count, out, where);
 }
 int rsb_batch_get_frame_jacobians(rsb_batch* b, int env_begin, int env_count, float* jac, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!jac) return fail(RSB_ERR_INVALID, "null output buffer");
   float* const out[5] = {nullptr, nullptr, nullptr, nullptr, jac};
   return frame_outputs(b, env_begin, env_count, out, where);
@@ -1067,58 +1050,58 @@ int rsb_batch_set_contact_bodies(rsb_batch* b, const int32_t* body, int n) {
   if (n == 0) { b->contact_bodies.clear(); return RSB_OK; }
   CK(cudaSetDevice(b->device));
   const size_t rows = (size_t)b->N * RSB_MAX_CONTACT_BODIES;
-  if (!b->cf_force) CK(cudaMalloc((void**)&b->cf_force, rows * 3 * 4));
-  if (!b->cf_steps) CK(cudaMalloc((void**)&b->cf_steps, rows * 4));
+  CK(b->cf_force.ensure(rows * 3 * 4, b->stream));
+  CK(b->cf_steps.ensure(rows * 4, b->stream));
   // the rows of a new list read zero until a launch advances the state (in stream order: a step enqueued before this call still wrote the old layout)
-  CK(cudaMemsetAsync(b->cf_force, 0, rows * 3 * 4, b->stream));
-  CK(cudaMemsetAsync(b->cf_steps, 0, rows * 4, b->stream));
+  CK(cudaMemsetAsync(b->cf_force.get(), 0, rows * 3 * 4, b->stream));
+  CK(cudaMemsetAsync(b->cf_steps.get(), 0, rows * 4, b->stream));
   b->contact_bodies.assign(body, body + n);
   return RSB_OK;
 }
 int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count, float* force, int32_t* steps_in_contact, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (b->contact_bodies.empty()) return fail(RSB_ERR_INVALID, "no contact bodies: call rsb_batch_set_contact_bodies() first");
   if (env_count == 0) return RSB_OK;
   CK(cudaSetDevice(b->device));
   const size_t S = b->contact_bodies.size();
-  rc = force ? copy_out(b, force, b->cf_force + (size_t)env_begin * S * 3, (size_t)env_count * S * 3 * 4, where) : RSB_OK; if (rc) return rc;
-  return steps_in_contact ? copy_out(b, steps_in_contact, b->cf_steps + (size_t)env_begin * S, (size_t)env_count * S * 4, where) : RSB_OK;
+  rc = force ? copy_out(b, force, b->cf_force.get() + (size_t)env_begin * S * 3, (size_t)env_count * S * 3 * 4, where) : RSB_OK; if (rc) return rc;
+  return steps_in_contact ? copy_out(b, steps_in_contact, b->cf_steps.get() + (size_t)env_begin * S, (size_t)env_count * S * 4, where) : RSB_OK;
 }
 int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
-  rc = out ? copy_out(b, out, b->contacts + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * sizeof(rsb_contact), where) : RSB_OK; if (rc) return rc;
-  return counts ? copy_out(b, counts, b->ncontacts + env_begin, (size_t)env_count * 4, where) : RSB_OK;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  rc = out ? copy_out(b, out, b->contacts.get() + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * sizeof(rsb_contact), where) : RSB_OK; if (rc) return rc;
+  return counts ? copy_out(b, counts, b->ncontacts.get() + env_begin, (size_t)env_count * 4, where) : RSB_OK;
 }
 int rsb_batch_get_contact_points(rsb_batch* b, int32_t* pt, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!pt) return fail(RSB_ERR_INVALID, "null output buffer");
-  return copy_out(b, pt, b->contact_pt + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * 4, where);
+  return copy_out(b, pt, b->contact_pt.get() + (size_t)env_begin * KMAX, (size_t)env_count * KMAX * 4, where);
 }
 int rsb_batch_get_solver_iterations(rsb_batch* b, int32_t* it, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!it) return fail(RSB_ERR_INVALID, "null output buffer");
-  return copy_out(b, it, b->iters + env_begin, (size_t)env_count * 4, where);
+  return copy_out(b, it, b->iters.get() + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_get_solver_status(rsb_batch* b, int32_t* status, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!status) return fail(RSB_ERR_INVALID, "null output buffer");
-  return copy_out(b, status, b->solver_status + env_begin, (size_t)env_count * 4, where);
+  return copy_out(b, status, b->solver_status.get() + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_get_solver_residual(rsb_batch* b, float* resid, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!resid) return fail(RSB_ERR_INVALID, "null output buffer");
-  return copy_out(b, resid, b->resid + env_begin, (size_t)env_count * 4, where);
+  return copy_out(b, resid, b->resid.get() + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_get_diverged(rsb_batch* b, int32_t* flags, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!flags) return fail(RSB_ERR_INVALID, "null output buffer");
-  return copy_out(b, flags, b->diverged + env_begin, (size_t)env_count * 4, where);
+  return copy_out(b, flags, b->diverged.get() + env_begin, (size_t)env_count * 4, where);
 }
 int rsb_batch_device_ptrs(rsb_batch* b, rsb_device_view* v) {
   if (!b || !v) return fail(RSB_ERR_INVALID, "null argument");
   v->num_envs = b->N; v->nq = b->nq; v->nv = b->nv; v->gc_stride = b->gc_stride; v->gv_stride = b->gv_stride;
-  v->gc = b->gc; v->gv = b->gv; v->tau_ff = b->tau; v->ptarget = b->pt; v->vtarget = b->vt;
-  v->ncontacts = b->ncontacts; v->contacts = b->contacts;
+  v->gc = b->gc.get(); v->gv = b->gv.get(); v->tau_ff = b->tau.get(); v->ptarget = b->pt.get(); v->vtarget = b->vt.get();
+  v->ncontacts = b->ncontacts.get(); v->contacts = b->contacts.get();
   return RSB_OK;
 }
 int64_t rsb_batch_launch_count(const rsb_batch* b) { return b ? b->launches : 0; }
@@ -1130,19 +1113,16 @@ int rsb_batch_ob_dim(const rsb_batch* b) {
 static int observe_impl(rsb_batch* b, float* obs, int env_begin, int env_count, int where) {
   const int od = rsb_batch_ob_dim(b);
   float* dst = obs;
-  if (where == RSB_HOST) {
-    int rc = ensure_obs_staging(b); if (rc) return rc;
-    dst = b->obs_staging;
-  }
+  if (where == RSB_HOST && !(dst = staging(b, (size_t)env_count * od))) return RSB_ERR_CUDA;
   int threads = 128, blocks = (env_count * 32 + threads - 1) / threads;
-  rsb_observe_kernel<<<blocks, threads, 0, b->stream>>>(b->gc + (size_t)env_begin * b->gc_stride, b->gv + (size_t)env_begin * b->gv_stride,
+  rsb_observe_kernel<<<blocks, threads, 0, b->stream>>>(b->gc.get() + (size_t)env_begin * b->gc_stride, b->gv.get() + (size_t)env_begin * b->gv_stride,
                                                          b->gc_stride, b->gv_stride, b->nq, b->nv, b->model->md.floating, env_count, dst, od);
   CK(cudaGetLastError());
   b->launches++;
   return where == RSB_HOST ? copy_out(b, obs, dst, (size_t)env_count * od * 4, RSB_HOST) : RSB_OK;
 }
 int rsb_batch_observe(rsb_batch* b, float* obs, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count); if (rc) return rc;
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
   if (!obs) return fail(RSB_ERR_INVALID, "null obs");
   if (env_count == 0) return RSB_OK;
   CK(cudaSetDevice(b->device));
@@ -1154,48 +1134,47 @@ int rsb_batch_observe(rsb_batch* b, float* obs, int env_begin, int env_count, in
 // torch pin_memory) so that the copies overlap; the call returns after the observations have landed.
 int rsb_batch_control_step(rsb_batch* b, const float* ptarget, const float* vtarget, int where_in, int substeps, float* obs, int where_out) {
   if (!b || substeps < 1) return fail(RSB_ERR_INVALID, "bad arguments to rsb_batch_control_step");
+  if (bad_where(where_in) || bad_where(where_out)) return fail(RSB_ERR_INVALID, "`where_in` and `where_out` must be RSB_HOST or RSB_DEVICE");
   CK(cudaSetDevice(b->device));
   // Host buffers in pinned (page-locked, mapped) memory are read and written IN PLACE by the step kernel over PCIe:
   // no staging copy, no separate H2D / D2H operations on the stream.  Pageable buffers take the staged path.
-  int rc = RSB_OK;
-  const float* pt_alias = (ptarget && where_in == RSB_HOST) ? mapped_alias(ptarget) : nullptr;
-  const float* vt_alias = (vtarget && where_in == RSB_HOST) ? mapped_alias(vtarget) : nullptr;
+  // Targets given here end a persistent rsb_batch_bind_pd_target() binding; pinned ones are read in place by this launch only.
   const bool pd_mode = b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && b->pd_set;
-  // one-shot bindings end with this call; a persistent rsb_batch_bind_pd_target() binding the call did not replace survives it
-  struct Unbind { rsb_batch* b; ~Unbind() { if (b->pt_once) { b->pt_bound = nullptr; b->pt_once = false; } if (b->vt_once) { b->vt_bound = nullptr; b->vt_once = false; } } } unbind{b};
+  LaunchIO io;
+  int rc = RSB_OK;
   if (ptarget) {
     b->pt_bound = nullptr;
-    if (pt_alias && pd_mode) { b->pt_bound = pt_alias; b->pt_bound_stride = b->nq; b->pt_once = true; }
-    else { rc = copy_rows_in(b, b->pt, b->gc_stride, ptarget, b->nq, 0, b->N, where_in); if (rc) return rc; }
+    io.pt = (where_in == RSB_HOST && pd_mode) ? mapped_alias(ptarget) : nullptr;
+    if (!io.pt) { rc = copy_rows_in(b, b->pt.get(), b->gc_stride, ptarget, b->nq, 0, b->N, where_in); if (rc) return rc; }
   }
   if (vtarget) {
     b->vt_bound = nullptr;
-    if (vt_alias && pd_mode) { b->vt_bound = vt_alias; b->vt_bound_stride = b->nv; b->vt_once = true; }
-    else { rc = copy_rows_in(b, b->vt, b->gv_stride, vtarget, b->nv, 0, b->N, where_in); if (rc) return rc; }
+    io.vt = (where_in == RSB_HOST && pd_mode) ? mapped_alias(vtarget) : nullptr;
+    if (!io.vt) { rc = copy_rows_in(b, b->vt.get(), b->gv_stride, vtarget, b->nv, 0, b->N, where_in); if (rc) return rc; }
   }
-  const bool bound_once = b->pt_once || b->vt_once;
+  const bool in_place = io.pt || io.vt;   // the caller may reuse its pinned target buffer when the call returns
   if (!obs || !b->model->md.floating) {
-    rc = do_launch(b, substeps, 0, false); if (rc) return rc;
+    rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;
     if (obs) rc = observe_impl(b, obs, 0, b->N, where_out);
-    if (bound_once) CK(cudaStreamSynchronize(b->stream));   // the caller may reuse its pinned target buffer on return
+    if (in_place) CK(cudaStreamSynchronize(b->stream));
     return rc;
   }
   // observation rows are written by the step kernel itself (no separate observe launch)
-  float* dst = obs;
   const int od = rsb_batch_ob_dim(b);
-  float* obs_alias = where_out == RSB_HOST ? const_cast<float*>(mapped_alias(obs)) : nullptr;
-  if (obs_alias) {   // observation rows go straight to the caller's pinned buffer as each environment finishes
-    rc = do_launch(b, substeps, 0, false, obs_alias); if (rc) return rc;
+  io.obs = where_out == RSB_HOST ? const_cast<float*>(mapped_alias(obs)) : nullptr;
+  if (io.obs) {   // observation rows go straight to the caller's pinned buffer as each environment finishes
+    rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;
     CK(cudaStreamSynchronize(b->stream));
     return RSB_OK;
   }
   if (where_out == RSB_HOST) {
-    rc = ensure_obs_staging(b); if (rc) return rc;
-    dst = b->obs_staging;
+    if (!(io.obs = staging(b, (size_t)b->N * od))) return RSB_ERR_CUDA;
+    rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;
+    return copy_out(b, obs, io.obs, (size_t)b->N * od * 4, RSB_HOST);
   }
-  rc = do_launch(b, substeps, 0, false, dst, where_out == RSB_DEVICE); if (rc) return rc;
-  if (where_out == RSB_HOST) return copy_out(b, obs, dst, (size_t)b->N * od * 4, RSB_HOST);
-  if (bound_once) CK(cudaStreamSynchronize(b->stream));
+  io.obs = obs; io.peers = true;
+  rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;
+  if (in_place) CK(cudaStreamSynchronize(b->stream));
   return RSB_OK;
 }
 
@@ -1209,15 +1188,15 @@ int rsb_batch_gym_configure(rsb_batch* b, const float* gc_init, const float* gv_
   std::vector<float> h((size_t)nq + nv + 2 * nj);
   std::memcpy(h.data(), gc_init, nq * 4); std::memcpy(h.data() + nq, gv_init, nv * 4);
   std::memcpy(h.data() + nq + nv, action_mean, nj * 4); std::memcpy(h.data() + nq + nv + nj, action_std, nj * 4);
-  // every buffer under its own check: a retry after a failed allocation finishes the set instead of skipping it
-  if (!b->gym_const) CK(cudaMalloc((void**)&b->gym_const, h.size() * 4));
-  if (!b->gym_action) CK(cudaMalloc((void**)&b->gym_action, (size_t)b->N * nj * 4));
-  if (!b->gym_obs) CK(cudaMalloc((void**)&b->gym_obs, (size_t)b->N * rsb_batch_ob_dim(b) * 4));
-  if (!b->gym_reward) CK(cudaMalloc((void**)&b->gym_reward, (size_t)b->N * 4));
-  if (!b->gym_done) CK(cudaMalloc((void**)&b->gym_done, (size_t)b->N));
-  CK(cudaMemcpyAsync(b->gym_const, h.data(), h.size() * 4, cudaMemcpyHostToDevice, b->stream));
+  CK(b->gym_const.ensure(h.size() * 4, b->stream));
+  CK(b->gym_action.ensure((size_t)b->N * nj * 4, b->stream));
+  CK(b->gym_obs.ensure((size_t)b->N * rsb_batch_ob_dim(b) * 4, b->stream));
+  CK(b->gym_reward.ensure((size_t)b->N * 4, b->stream));
+  CK(b->gym_done.ensure((size_t)b->N, b->stream));
+  CK(cudaMemcpyAsync(b->gym_const.get(), h.data(), h.size() * 4, cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
-  b->gym.gc_init = b->gym_const; b->gym.gv_init = b->gym_const + nq; b->gym.action_mean = b->gym_const + nq + nv; b->gym.action_std = b->gym_const + nq + nv + nj;
+  const float* c = b->gym_const.get();
+  b->gym.gc_init = c; b->gym.gv_init = c + nq; b->gym.action_mean = c + nq + nv; b->gym.action_std = c + nq + nv + nj;
   b->gym.foot_mask = 0;
   for (int i = 0; i < n_foot; i++) {
     if (foot_bodies[i] < 0 || foot_bodies[i] >= b->nb) return fail(RSB_ERR_INVALID, "foot body index out of range");
@@ -1233,7 +1212,7 @@ int rsb_batch_gym_reset(rsb_batch* b) {
   if (!b || !b->gym_ready) return fail(RSB_ERR_INVALID, "call rsb_batch_gym_configure() first");
   CK(cudaSetDevice(b->device));
   int threads = 128, blocks = (b->N * 32 + threads - 1) / threads;
-  rsb_gym_reset_kernel<<<blocks, threads, 0, b->stream>>>(b->gc, b->gv, b->pt, b->vt, b->gym, b->gc_stride, b->gv_stride, b->nq, b->nv, b->N);
+  rsb_gym_reset_kernel<<<blocks, threads, 0, b->stream>>>(b->gc.get(), b->gv.get(), b->pt.get(), b->vt.get(), b->gym, b->gc_stride, b->gv_stride, b->nq, b->nv, b->N);
   CK(cudaGetLastError());
   b->kin_dirty = true;
   b->launches++;
@@ -1245,6 +1224,7 @@ int rsb_batch_gym_reset(rsb_batch* b) {
 int rsb_batch_gym_step(rsb_batch* b, const float* action, int where_in, int substeps, float* obs, float* reward, unsigned char* done, int where_out) {
   if (!b || !b->gym_ready) return fail(RSB_ERR_INVALID, "call rsb_batch_gym_configure() first");
   if (!action || substeps < 1) return fail(RSB_ERR_INVALID, "bad arguments to rsb_batch_gym_step");
+  if (bad_where(where_in) || bad_where(where_out)) return fail(RSB_ERR_INVALID, "`where_in` and `where_out` must be RSB_HOST or RSB_DEVICE");
   CK(cudaSetDevice(b->device));
   const int nj = b->nq - 7, od = rsb_batch_ob_dim(b);
   b->pt_bound = nullptr;              // the task writes its own PD-target rows
@@ -1253,28 +1233,29 @@ int rsb_batch_gym_step(rsb_batch* b, const float* action, int where_in, int subs
   if (where_in == RSB_HOST) {
     act = mapped_alias(action);
     if (!act) {
-      CK(cudaMemcpyAsync(b->gym_action, action, (size_t)b->N * nj * 4, cudaMemcpyHostToDevice, b->stream));
-      act = b->gym_action;
+      CK(cudaMemcpyAsync(b->gym_action.get(), action, (size_t)b->N * nj * 4, cudaMemcpyHostToDevice, b->stream));
+      act = b->gym_action.get();
     }
   }
   const bool host_out = where_out == RSB_HOST;
   float* a_obs = (host_out && obs) ? const_cast<float*>(mapped_alias(obs)) : nullptr;
   float* a_rew = (host_out && reward) ? const_cast<float*>(mapped_alias(reward)) : nullptr;
   unsigned char* a_done = (host_out && done) ? reinterpret_cast<unsigned char*>(const_cast<float*>(mapped_alias(done))) : nullptr;
-  float* d_obs = a_obs ? a_obs : (host_out || !obs) ? b->gym_obs : obs;
-  float* d_rew = a_rew ? a_rew : (host_out || !reward) ? b->gym_reward : reward;
-  unsigned char* d_done = a_done ? a_done : (host_out || !done) ? b->gym_done : done;
+  float* d_obs = a_obs ? a_obs : (host_out || !obs) ? b->gym_obs.get() : obs;
+  float* d_rew = a_rew ? a_rew : (host_out || !reward) ? b->gym_reward.get() : reward;
+  unsigned char* d_done = a_done ? a_done : (host_out || !done) ? b->gym_done.get() : done;
   // ONE launch: action rows -> PD targets, `substeps` x World::integrate(), reward, isTerminalState(), reset() of the terminated
   // environments and the observation rows of the resulting state (the task used to be an action kernel and a post kernel around the step)
   if (!(b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && b->pd_set)) return fail(RSB_ERR_INVALID, "the gym task drives the robot through PD targets: call rsb_batch_set_pd_gains() first");
-  const GymLaunch gl{act, d_rew, d_done};
-  int rc = do_launch(b, substeps, 0, false, d_obs, false, &gl); if (rc) return rc;
+  LaunchIO io;
+  io.obs = d_obs; io.gym_action = act; io.gym_reward = d_rew; io.gym_done = d_done;
+  int rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;
   if (where_out == RSB_HOST) {
     if (obs && !a_obs) CK(cudaMemcpyAsync(obs, d_obs, (size_t)b->N * od * 4, cudaMemcpyDeviceToHost, b->stream));
     if (reward && !a_rew) CK(cudaMemcpyAsync(reward, d_rew, (size_t)b->N * 4, cudaMemcpyDeviceToHost, b->stream));
     if (done && !a_done) CK(cudaMemcpyAsync(done, d_done, (size_t)b->N, cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
-  } else if (where_in == RSB_HOST && act != b->gym_action) {
+  } else if (where_in == RSB_HOST && act != b->gym_action.get()) {
     CK(cudaStreamSynchronize(b->stream));   // the action rows were read in place from pinned host memory: the caller may reuse them on return
   }
   return RSB_OK;
@@ -1323,8 +1304,8 @@ int rsb_batch_set_observation_peers(rsb_batch* b, int world, int rank, void* con
   CK(cudaSetDevice(b->device));
   CK(cudaStreamSynchronize(b->stream));
   b->peer_world = 0;              // a failure below leaves the batch without peers
-  if (!b->peer_done) CK(cudaMalloc(&b->peer_done, sizeof(unsigned)));
-  CK(cudaMemsetAsync(b->peer_done, 0, sizeof(unsigned), b->stream));
+  CK(b->peer_done.ensure(sizeof(unsigned), b->stream));
+  CK(cudaMemsetAsync(b->peer_done.get(), 0, sizeof(unsigned), b->stream));
   for (int p = 0; p < world; p++) { b->peer_obs[p][0] = (float*)obs_all[2 * p]; b->peer_obs[p][1] = (float*)obs_all[2 * p + 1]; b->peer_flag[p] = (unsigned*)flags[p]; }
   b->peer_world = world; b->peer_rank = rank; b->peer_epoch = 0;
   return RSB_OK;
@@ -1355,14 +1336,14 @@ int rsb_internal_set_profile_stage_a(rsb_batch* b, unsigned* dev) { if (!b) retu
 // memory, so a caller that forces a configuration reads back what it got here.
 int rsb_internal_launch_config(const rsb_batch* b, int* wpc, int* grid) {
   if (!b || !wpc || !grid) return fail(RSB_ERR_INVALID, "null argument");
-  *wpc = b->wpc; *grid = b->grid;
+  *wpc = b->cfg.wpc; *grid = b->cfg.grid;
   return RSB_OK;
 }
 // compiled instance of the step kernel that the batch launches (dispatch_spec): spec 0 generic, 1 quadruped, 2 humanoid; slots =
 // candidate points per lane (tests).  A hook of its own, so that callers of rsb_internal_launch_config keep their signature
 int rsb_internal_launch_instance(const rsb_batch* b, int* spec, int* slots) {
   if (!b || !spec || !slots) return fail(RSB_ERR_INVALID, "null argument");
-  *spec = b->spec; *slots = b->slots;
+  *spec = b->cfg.spec; *slots = b->cfg.slots;
   return RSB_OK;
 }
 void rsb_internal_set_error(const char* msg) { g_err = msg ? msg : ""; }

@@ -108,23 +108,35 @@ def _setup(capi, monkeypatch, name, terrain, n, seed, params=None):
 # ---- 1 / 2: nothing changes where nothing may ---------------------------------------------------------------------------------
 
 def test_clearing_pairs_restores_default_instance(capi, monkeypatch):
-    """enabling pairs and clearing them again (n = 0) gives back the default instance and bit-identical results"""
+    """enabling pairs and clearing them again (n = 0) gives back the default instance and bit-identical results, whatever the order in
+    which the terrain friction, the pairs and the PD gains were set around them"""
     _env(monkeypatch)
+    kp, kd = np.r_[np.zeros(6), 80.0 * np.ones(12)], np.r_[np.zeros(6), 2.0 * np.ones(12)]
+    orders = [("friction", "gains"), ("friction", "pairs", "gains", "clear"), ("pairs", "gains", "friction", "clear")]
     runs = []
-    for clear in (False, True):
+    for order in orders:
         t, bt, _, _, gc, gv, tau = setup_batch(capi, "anymal_c_like.urdf", 512, 7, terrain="hm", tau_scale=20.0)
-        bt.set_collision_friction(4, 0.5)
+        bt.set_control_mode(capi.PD_PLUS_FEEDFORWARD_TORQUE)
+        bt.set_pd_target(np.tile(ANYMAL_GC0, (512, 1)).astype(np.float32), np.zeros((512, 18), np.float32))
         before = launch_config(capi, bt)
-        if clear:
-            bt.set_self_collision(anymal_leg_pairs())
-            assert launch_config(capi, bt)["spec"] == SPEC_GENERIC
-            bt.set_self_collision([])
+        for step in order:
+            if step == "friction":
+                bt.set_collision_friction(4, 0.5)
+            elif step == "gains":
+                bt.set_pd_gains(kp, kd)
+            elif step == "pairs":
+                bt.set_self_collision(anymal_leg_pairs())
+            else:
+                assert launch_config(capi, bt)["spec"] == SPEC_GENERIC
+                bt.set_self_collision([])
         cfg = launch_config(capi, bt)
-        assert cfg == before and cfg["spec"] == 1
+        assert cfg == before and cfg["spec"] == 1, order
         bt.integrate(4)
         bt.integrate(4)
         runs.append(_outputs(bt))
-    _same(runs[0], runs[1])
+    for order, run in zip(orders[1:], runs[1:]):
+        print("compared:", order)
+        _same(runs[0], run)
 
 
 def test_unreachable_pairs_bit_identical_to_generic(capi, monkeypatch):
