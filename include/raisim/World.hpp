@@ -106,6 +106,9 @@ struct LockStep {
   bool cfValid = false;
   std::vector<float> bodyInertia;           // [n][nb][10] inertial rows (ArticulatedSystem::updateMassInfo); empty until the first one
   bool bodyInertiaDirty = false;
+  int ncoll = 0;
+  std::vector<float> friction;              // [n][ncoll] terrain friction rows (World material calls; -1: the batch's value); empty until the first one
+  bool frictionDirty = false;
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
   bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
@@ -155,7 +158,8 @@ struct LockStep {
     if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
-    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = false;
+    if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
+    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = false;
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
@@ -167,7 +171,16 @@ struct LockStep {
     if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
-    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = false;
+    if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
+    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = false;
+  }
+  // environment env's terrain friction of one collision body, uploaded with the next flush() or pushWrites() (no launch of its own)
+  void setFriction(int env, size_t collisionBody, double mu) {
+    if (collisionBody >= size_t(ncoll)) throw std::runtime_error("setCollisionBodyFriction: collision body index out of range");
+    sync(env);
+    if (friction.empty()) friction.assign(size_t(n) * ncoll, -1.f);
+    friction[size_t(env) * ncoll + collisionBody] = float(mu);
+    frictionDirty = true;
   }
 };
 
@@ -199,7 +212,11 @@ class BatchedWorld {
   void advanceTime(double t) { worldTime_ += t; }
   // lock-step mode (VectorizedEnvironment<ENVIRONMENT>): per-environment views work on host mirrors, integrate() is deferred
   LockStep* lockStep() { return ls_.get(); }
-  void enableLockStep() { if (!ls_) { ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); ls_->cfBodies = int(contactBodies_.size()); } }
+  void enableLockStep() {
+    if (ls_) return;
+    ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); ls_->cfBodies = int(contactBodies_.size());
+    rsbCheck(rsb_model_dims(model_, nullptr, nullptr, nullptr, &ls_->ncoll, nullptr), "dims");
+  }
   // bodies whose contact force every integrate() gathers (ArticulatedSystem::setContactBodies): one list for all environments
   void setContactBodies(const std::vector<size_t>& bodies) {
     if (bodies == contactBodies_) return;      // every environment of a VectorizedEnvironment sets the same list in its constructor
@@ -484,8 +501,11 @@ class ArticulatedSystem {
   const std::map<size_t, std::string>& collisionMaterials() const { return collisionMaterial_; }
   bool materialsDirty() const { return materialsDirty_; }
   void materialsApplied() { materialsDirty_ = false; }
-  // friction of one collision body against the terrain (upstream: getCollisionBody(name).setMaterial + setMaterialPairProp)
+  // friction of one collision body against the terrain (upstream: getCollisionBody(name).setMaterial + setMaterialPairProp); mu < 0:
+  // the default material.  A stand-alone World sets it for its batch; in a VectorizedEnvironment it is this environment's own, kept in
+  // the host mirror's friction row and uploaded with the next launch (include/rsb.h rsb_batch_set_contact_friction)
   void setCollisionBodyFriction(size_t collisionBodyIdx, double mu) {
+    if (LockStep* ls = w_->lockStep()) { ls->setFriction(env_, collisionBodyIdx, mu); return; }
     rsbCheck(rsb_batch_set_collision_friction(w_->batch(), int(collisionBodyIdx), float(mu)), "setCollisionBodyFriction");
   }
   // Self-collision.  Upstream checks the bodies of an articulated system against each other and user code switches single pairs off
@@ -997,8 +1017,12 @@ class World {
     p.alpha_init = float(alpha_init); p.alpha_min = float(alpha_min); p.alpha_decay = float(alpha_decay); p.max_iter = maxIter; p.threshold = float(threshold);
     w_->setParams(p);
   }
+  // In a VectorizedEnvironment the friction is this environment's own: every collision body without a material pair of its own takes it
+  // (through the environment's friction row); restitution, and the default friction of self-collision pairs, stay batch-wide
   void setDefaultMaterial(double friction, double restitution, double resThreshold) {
-    need(); rsb_params p = w_->params(); p.mu = float(friction); p.restitution = float(restitution); p.rest_threshold = float(resThreshold); w_->setParams(p);
+    need(); rsb_params p = w_->params(); p.restitution = float(restitution); p.rest_threshold = float(resThreshold);
+    if (w_->lockStep()) { w_->setParams(p); defaultFriction_ = friction; if (robot_) applyMaterials(true); return; }
+    p.mu = float(friction); w_->setParams(p);
   }
   // named material pairs: friction of (collision-body material, terrain material); restitution is global (setDefaultMaterial)
   void setMaterialPairProp(const std::string& m1, const std::string& m2, double friction, double /*restitution*/ = 0, double /*resThreshold*/ = 0) {
@@ -1019,6 +1043,7 @@ class World {
   void integrate() {
     need();
     if (LockStep* ls = w_->lockStep()) {   // deferred: counted now, executed for every environment at once when the result is first needed
+      applyMaterials(false);
       ls->pending[env_]++;
       if (env_ == 0) w_->advanceTime(w_->params().dt);
       return;
@@ -1034,6 +1059,21 @@ class World {
   void need() const { if (!w_) throw std::runtime_error("World: call addArticulatedSystem() first (the batch is created with the robot)"); }
   void applyMaterials(bool force) {
     if (!robot_ || (!force && !robot_->materialsDirty())) return;
+    if (LockStep* ls = w_->lockStep()) {   // this environment's whole row: its pair friction, else its default friction (< 0: the batch's)
+      if (ls->friction.empty() && robot_->collisionMaterials().empty() && defaultFriction_ < 0) return;   // every entry -1: no rows needed
+      for (int c = 0; c < ls->ncoll; c++) {
+        auto m = robot_->collisionMaterials().find(size_t(c));
+        double mu = defaultFriction_;
+        if (m != robot_->collisionMaterials().end()) {
+          const std::string& a = m->second; const std::string& b = terrainMaterial_;
+          auto it = pairFriction_.find(a < b ? std::make_pair(a, b) : std::make_pair(b, a));
+          if (it != pairFriction_.end()) mu = it->second;
+        }
+        robot_->setCollisionBodyFriction(size_t(c), mu);
+      }
+      robot_->materialsApplied();
+      return;
+    }
     for (const auto& kv : robot_->collisionMaterials()) {
       const std::string& a = kv.second; const std::string& b = terrainMaterial_;
       auto it = pairFriction_.find(a < b ? std::make_pair(a, b) : std::make_pair(b, a));
@@ -1043,6 +1083,7 @@ class World {
   }
   std::map<std::pair<std::string, std::string>, double> pairFriction_;
   std::string terrainMaterial_ = "default";
+  double defaultFriction_ = -1;        // VectorizedEnvironment: this environment's setDefaultMaterial friction (< 0: not set, the batch's)
   std::unique_ptr<BatchedWorld> owned_;
   BatchedWorld* w_ = nullptr;
   BatchContext* ctx_ = nullptr;

@@ -156,8 +156,23 @@ int rsb_batch_set_params(rsb_batch* b, const rsb_params* p);
 int rsb_batch_get_params(const rsb_batch* b, rsb_params* p);
 int rsb_params_default(rsb_params* p);
 /* friction of one collision body (index in rsb_model_tables order) against the terrain; mu < 0 = default material.
- * The per-body half of World::setMaterialPairProp / getCollisionBody(name).setMaterial */
+ * The per-body half of World::setMaterialPairProp / getCollisionBody(name).setMaterial, shared by all environments; per-environment
+ * rows (rsb_batch_set_contact_friction) take precedence where they hold a value >= 0 */
 int rsb_batch_set_collision_friction(rsb_batch* b, int collision_body, float mu);
+/* Per-environment terrain friction of every collision body (World::setMaterialPairProp / setDefaultMaterial /
+ * getCollisionBody(name).setMaterial, per World upstream).  rows [env_count][ncoll] float32 in the collision-body order of
+ * rsb_model_tables; host or device source (`where`).  An entry mu >= 0 is the friction of that collision body's terrain contacts in that
+ * environment; mu < 0 is the batch-level value, resolved at every launch: rsb_batch_set_collision_friction for that body if set, else
+ * rsb_params.mu.  rows == NULL resets the range to -1.  The first call (and the first after rsb_batch_clear_contact_friction) starts
+ * every environment at -1, then writes the range: no rows, rows of -1 and rows set then cleared compute the same bits.
+ * Self contacts (candidates npts + j) keep their pair's friction; restitution stays per batch.  The rows live outside the model blob, so
+ * rsb_batch_set_collision_friction, set_self_collision, set_params, the terrain calls and gym resets keep them.  The friction does not
+ * enter M, h or the poses: nothing goes stale and no launch is added.
+ * Refused with RSB_ERR_INVALID, changing nothing: a null batch, a bad range or `where`, or a value that is NaN or +-inf.  The rows are
+ * checked on the device in the batch's staging buffer before any of them is committed; the call waits for that check. */
+int rsb_batch_set_contact_friction(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
+/* drop all per-environment friction rows: every later launch runs as if none had been set */
+int rsb_batch_clear_contact_friction(rsb_batch* b);
 /* Self-collision between the bodies of the robot (ArticulatedSystem collisions between its own bodies): OFF unless pairs are enabled
  * here.  pairs[n][2] are collision-body indices (rsb_model_tables / rsb_model_collision_index order), at most RSB_MAX_SELF_PAIRS; there
  * is no "all pairs" mode.  Supported: sphere-sphere, sphere-capsule, capsule-capsule, sphere-box (RSB_ERR_UNSUPPORTED, naming the pair,
@@ -200,7 +215,8 @@ int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, co
  * Refused with RSB_ERR_INVALID, changing nothing: a bad range or `where`, a value that is not finite, a negative mass, or an inertia
  * that is not positive semidefinite.  The inertia test, in double precision with t = xx + yy + zz: every diagonal entry >= -1e-6 t,
  * every 2 x 2 principal minor >= -1e-6 t^2 and the determinant >= -1e-6 t^3.  The rows are checked on the device in the batch's
- * staging buffer before any of them is committed; the call waits for that check.  Gains, effort limits, friction and collision shapes stay per batch. */
+ * staging buffer before any of them is committed; the call waits for that check.  Gains, effort limits and collision shapes stay per
+ * batch; terrain friction has rows of its own (rsb_batch_set_contact_friction). */
 int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
 /* drop all per-environment rows: every later launch runs exactly as if none had ever been set */
 int rsb_batch_clear_body_inertia(rsb_batch* b);

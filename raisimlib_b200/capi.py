@@ -96,7 +96,7 @@ EXPORTED = [
     "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
     "rsb_batch_set_collision_friction", "rsb_batch_set_self_collision",
     "rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_gains", "rsb_batch_set_pd_target",
-    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
+    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
     "rsb_batch_integrate1", "rsb_batch_integrate2", "rsb_batch_integrate",
     "rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities", "rsb_batch_get_body_poses", "rsb_batch_get_contacts",
     "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
@@ -182,6 +182,9 @@ def lib():
         if hasattr(L, "rsb_batch_set_body_inertia"):       # absent from an older build loaded through RSB_LIB_PATH (tools/body_inertia_probe.py)
             L.rsb_batch_set_body_inertia.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
             L.rsb_batch_clear_body_inertia.argtypes = [C.c_void_p]
+        if hasattr(L, "rsb_batch_set_contact_friction"):   # absent from an older build loaded through RSB_LIB_PATH (tools/contact_friction_probe.py)
+            L.rsb_batch_set_contact_friction.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+            L.rsb_batch_clear_contact_friction.argtypes = [C.c_void_p]
         L.rsb_batch_device_ptrs.argtypes = [C.c_void_p, C.POINTER(DeviceView)]
         L.rsb_batch_launch_count.argtypes = [C.c_void_p]
         L.rsb_batch_ob_dim.argtypes = [C.c_void_p]
@@ -603,6 +606,29 @@ class Batch:
     def clear_body_inertia(self):
         """drop every per-environment row: later steps run as if none had been set"""
         _ck(lib().rsb_batch_clear_body_inertia(self.h))
+
+    # per-environment terrain friction
+    def set_contact_friction(self, rows, env_begin=0, env_count=None):
+        """rows [n, ncoll] (numpy; collision-body order of the model tables) for environments [env_begin, env_begin + n): an entry
+        >= 0 is the friction of that collision body's terrain contacts in that environment, < 0 the batch-level value
+        (set_collision_friction, else params mu).  rows None resets env_count environments (default: to the end of the batch) to -1.
+        A refused call (NaN or +-inf anywhere) changes nothing."""
+        if rows is None:
+            _ck(lib().rsb_batch_set_contact_friction(self.h, None, env_begin, self._count(env_begin, env_count), HOST))
+            return
+        r = np.ascontiguousarray(rows, np.float32)
+        if r.ndim != 2 or r.shape[1] != self.model.ncoll:
+            raise ValueError(f"rows: need shape [n, {self.model.ncoll}], got {r.shape}")
+        _ck(lib().rsb_batch_set_contact_friction(self.h, r.ctypes.data_as(C.c_void_p), env_begin, r.shape[0], HOST))
+
+    def set_contact_friction_from(self, rows, env_begin=0):
+        """set_contact_friction() from a contiguous float32 torch tensor [n, ncoll] on the batch's device, checked there"""
+        n = rows.shape[0] if hasattr(rows, "shape") and len(rows.shape) > 0 else -1
+        _ck(lib().rsb_batch_set_contact_friction(self.h, self._device_out(rows, (n, self.model.ncoll), "rows"), env_begin, n, DEVICE))
+
+    def clear_contact_friction(self):
+        """drop every per-environment friction row: later steps run as if none had been set"""
+        _ck(lib().rsb_batch_clear_contact_friction(self.h))
 
     def control_step(self, ptarget, substeps, obs_out, vtarget=None):
         """one RaisimGym control step for the whole batch: targets in, fused sub-steps, observations out"""

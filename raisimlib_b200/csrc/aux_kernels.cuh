@@ -59,6 +59,16 @@ __global__ void rsb_body_inertia_pack_kernel(float* __restrict__ out, const floa
   if (fault) atomicMin(bad, r * 4 + fault);
 }
 
+// per-environment terrain friction rows (rsb_batch_set_contact_friction, StepArgs::contact_friction): `n` values of the caller copied as
+// they are.  A value that is NaN or +-inf lowers *bad to its index; *bad is left alone when every value is accepted
+__global__ void rsb_contact_friction_check_kernel(float* __restrict__ out, const float* __restrict__ src, int n, int* bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float v = src[i];
+  out[i] = v;
+  if (!isfinite(v)) atomicMin(bad, i);
+}
+
 // ---- frame kinematics (rsb_batch_set_frames / get_frame_states / get_frame_jacobians) ----------------------------------------------
 // Frames rigidly attached to bodies and, per dof, what its Jacobian column needs; device arrays uploaded by rsb_batch_set_frames.
 // A dof turns or slides along the axis a of its body k (a = R_k axis: the joint frame's rotation about its own axis leaves the axis

@@ -70,6 +70,12 @@ struct Overrides {
   std::vector<float> self_mu;        // [n] their friction (< 0: default material)
 };
 
+// per-environment rows that a step launch reads in place of a batch-level value while `active` (commit_env_rows)
+struct EnvRows {
+  DevBuf<float> rows;
+  bool active = false;
+};
+
 struct rsb_batch {
   const rsb_model* model = nullptr;
   int N = 0, device = 0;
@@ -123,11 +129,10 @@ struct rsb_batch {
   std::vector<uint8_t> contact_bodies;
   DevBuf<float> cf_force;
   DevBuf<int> cf_steps;
-  // per-environment inertial rows of rsb_batch_set_body_inertia: bi_rows [N][nb][BI_WORDS], read by every step launch while bi_active;
-  // bi_bad: the verdict of the check a call's rows pass before they replace any of bi_rows
-  DevBuf<float> bi_rows;
-  DevBuf<int> bi_bad;
-  bool bi_active = false;
+  // per-environment rows: inertial ones of rsb_batch_set_body_inertia [N][nb][BI_WORDS], terrain friction of
+  // rsb_batch_set_contact_friction [N][ncoll]; row_bad: the verdict of the check a call's rows pass before they replace any of them
+  EnvRows body_inertia, contact_friction;
+  DevBuf<int> row_bad;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
@@ -402,7 +407,8 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
   if (debug) { a.dbg_M = b->dbg_M.get(); a.dbg_h = b->dbg_h.get(); a.dbg_R = b->dbg_R.get(); a.dbg_p = b->dbg_p.get(); }
   a.phase_mask = phase_mask; a.prof = b->prof; a.prof_a = b->prof_a;
   a.ext = b->ext_active ? b->ext.get() : nullptr;
-  a.body_inertia = b->bi_active ? b->bi_rows.get() : nullptr;
+  a.body_inertia = b->body_inertia.active ? b->body_inertia.rows.get() : nullptr;
+  a.contact_friction = b->contact_friction.active ? b->contact_friction.rows.get() : nullptr;
   a.obs = io.obs; a.ob_dim = rsb_batch_ob_dim(b);
   if (io.gym_action) {   // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
     a.gym_action = io.gym_action; a.gym = b->gym; a.gym_reward = io.gym_reward; a.gym_done = io.gym_done;
@@ -488,6 +494,63 @@ static int check_range(const rsb_batch* b, int env_begin, int env_count, int whe
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
   if (env_begin < 0 || env_count < 0 || env_begin + env_count > b->N) return fail(RSB_ERR_INVALID, "environment range out of bounds");
   if (bad_where(where)) return fail(RSB_ERR_INVALID, "`where` must be RSB_HOST or RSB_DEVICE");
+  return RSB_OK;
+}
+
+// The one path by which a call's per-environment rows reach an EnvRows table (rsb_batch_set_body_inertia, set_contact_friction).
+// `dflt` is one environment's row of the table (w words) when nothing overrides it: every environment starts from it at the first commit
+// after creation or a clear, and rows == null writes it to the range.  Otherwise the caller's rows (src_w words per environment) are
+// checked and packed to w words by check(out, src, env_count, bad) in the staging buffer (a host source passes through it too), and the
+// call waits for the verdict: *bad stays ROWS_OK when every value is accepted; else nothing of the table changes and the call is
+// refused with what(verdict).
+static constexpr int ROWS_OK = 0x7fffffff;
+static std::vector<float> repeat_row(const std::vector<float>& row, size_t n) {
+  std::vector<float> r(n * row.size());
+  for (size_t e = 0; e < n; e++) std::copy(row.begin(), row.end(), r.begin() + e * row.size());
+  return r;
+}
+template <class Check, class What>
+static int commit_env_rows(rsb_batch* b, EnvRows& t, const std::vector<float>& dflt, const float* rows, int env_begin, int env_count, int where,
+                           size_t src_w, Check check, What what) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (env_count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const size_t w = dflt.size(), n = (size_t)env_count;
+  const float* staged = nullptr;
+  std::vector<float> reset;
+  if (rows) {
+    CK(b->row_bad.ensure(4, b->stream));
+    // the checked rows [n][w], then a host source's rows [n][src_w]
+    float* const st = staging(b, n * w + (where == RSB_HOST ? n * src_w : 0)); if (!st) return RSB_ERR_CUDA;
+    const float* src = rows;
+    if (where == RSB_HOST) {
+      CK(cudaMemcpyAsync(st + n * w, rows, n * src_w * 4, cudaMemcpyHostToDevice, b->stream));
+      src = st + n * w;
+    }
+    const int ok = ROWS_OK;
+    CK(cudaMemcpyAsync(b->row_bad.get(), &ok, 4, cudaMemcpyHostToDevice, b->stream));
+    if (n * src_w > 0) { check(st, src, env_count, b->row_bad.get()); CK(cudaGetLastError()); }
+    int bad = ok;
+    CK(cudaMemcpyAsync(&bad, b->row_bad.get(), 4, cudaMemcpyDeviceToHost, b->stream));
+    CK(cudaStreamSynchronize(b->stream));
+    if (bad != ok) return fail(RSB_ERR_INVALID, what(bad) + "; no row changed");
+    staged = st;
+  } else {
+    reset = repeat_row(dflt, n);
+  }
+  CK(t.rows.ensure((size_t)b->N * w * 4, b->stream));
+  if (!t.active) {
+    const std::vector<float> init = repeat_row(dflt, (size_t)b->N);
+    CK(cudaMemcpyAsync(t.rows.get(), init.data(), init.size() * 4, cudaMemcpyHostToDevice, b->stream));
+    CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
+  }
+  float* const at = t.rows.get() + (size_t)env_begin * w;
+  if (staged) CK(cudaMemcpyAsync(at, staged, n * w * 4, cudaMemcpyDeviceToDevice, b->stream));
+  else {
+    CK(cudaMemcpyAsync(at, reset.data(), reset.size() * 4, cudaMemcpyHostToDevice, b->stream));
+    CK(cudaStreamSynchronize(b->stream));
+  }
+  t.active = true;
   return RSB_OK;
 }
 
@@ -814,75 +877,58 @@ int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, co
   return RSB_OK;
 }
 // ---- per-environment inertial parameters (ArticulatedSystem::getMass / getBodyCOM_B / getInertia + updateMassInfo per World upstream) ----
-// the model's row of every body, in float32 exactly as build_blob writes BF_MASS / BF_COM / BF_INERTIA, repeated for n environments
-static std::vector<float> model_inertia_rows(const Model& md, int n) {
-  std::vector<float> r((size_t)n * md.nb * BI_WORDS, 0.f);
-  for (int e = 0; e < n; e++)
-    for (int i = 0; i < md.nb; i++) {
-      float* o = &r[((size_t)e * md.nb + i) * BI_WORDS];
-      o[0] = (float)md.mass[i];
-      for (int k = 0; k < 3; k++) o[1 + k] = (float)md.com[3 * i + k];
-      for (int k = 0; k < 6; k++) o[4 + k] = (float)md.inertia[6 * i + k];
-    }
+// the model's row of every body, in float32 exactly as build_blob writes BF_MASS / BF_COM / BF_INERTIA
+static std::vector<float> model_inertia_row(const Model& md) {
+  std::vector<float> r((size_t)md.nb * BI_WORDS, 0.f);
+  for (int i = 0; i < md.nb; i++) {
+    float* o = &r[(size_t)i * BI_WORDS];
+    o[0] = (float)md.mass[i];
+    for (int k = 0; k < 3; k++) o[1 + k] = (float)md.com[3 * i + k];
+    for (int k = 0; k < 6; k++) o[4 + k] = (float)md.inertia[6 * i + k];
+  }
   return r;
 }
 int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {
-  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
-  if (env_count == 0) return RSB_OK;
-  CK(cudaSetDevice(b->device));
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
   const Model& md = b->model->md;
-  const size_t per_env = (size_t)md.nb * BI_WORDS, all = (size_t)b->N * per_env;
-  const float* staged = nullptr;
-  std::vector<float> model_rows;
-  if (rows) {   // check the caller's rows in the staging buffer; nothing of bi_rows changes unless every value is accepted
-    CK(b->bi_bad.ensure(4, b->stream));
-    const size_t nrows = (size_t)env_count * md.nb;
-    // the checked rows [nrows][BI_WORDS], then a host source's tight rows [nrows][10]
-    float* const st = staging(b, nrows * BI_WORDS + (where == RSB_HOST ? nrows * 10 : 0)); if (!st) return RSB_ERR_CUDA;
-    const float* src = rows;
-    if (where == RSB_HOST) {
-      CK(cudaMemcpyAsync(st + nrows * BI_WORDS, rows, nrows * 10 * 4, cudaMemcpyHostToDevice, b->stream));
-      src = st + nrows * BI_WORDS;
-    }
-    const int ok = 0x7fffffff;
-    CK(cudaMemcpyAsync(b->bi_bad.get(), &ok, 4, cudaMemcpyHostToDevice, b->stream));
-    const int threads = 128;
-    rsb_body_inertia_pack_kernel<<<(unsigned)((nrows + threads - 1) / threads), threads, 0, b->stream>>>(st, src, (int)nrows, 1e-6, b->bi_bad.get());
-    CK(cudaGetLastError());
-    int bad = ok;
-    CK(cudaMemcpyAsync(&bad, b->bi_bad.get(), 4, cudaMemcpyDeviceToHost, b->stream));
-    CK(cudaStreamSynchronize(b->stream));
-    if (bad != ok) {
-      static const char* what[] = {"", "a value that is not finite", "a negative mass", "an inertia that is not symmetric positive semidefinite"};
-      const int r = bad / 4, env = env_begin + r / md.nb, body = r % md.nb;
-      return fail(RSB_ERR_INVALID, "body inertia: environment " + std::to_string(env) + ", body " + std::to_string(body) + " (" + md.body_names[body] + ") has " + what[bad & 3] +
-                                   "; no row changed");
-    }
-    staged = st;
-  } else {
-    model_rows = model_inertia_rows(md, env_count);
-  }
-  // commit: the first call after creation or rsb_batch_clear_body_inertia starts every environment from the model's rows
-  CK(b->bi_rows.ensure(all * 4, b->stream));
-  if (!b->bi_active) {
-    const std::vector<float> init = model_inertia_rows(md, b->N);
-    CK(cudaMemcpyAsync(b->bi_rows.get(), init.data(), all * 4, cudaMemcpyHostToDevice, b->stream));
-    CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
-  }
-  float* const at = b->bi_rows.get() + (size_t)env_begin * per_env;
-  if (staged) CK(cudaMemcpyAsync(at, staged, (size_t)env_count * per_env * 4, cudaMemcpyDeviceToDevice, b->stream));
-  else {
-    CK(cudaMemcpyAsync(at, model_rows.data(), model_rows.size() * 4, cudaMemcpyHostToDevice, b->stream));
-    CK(cudaStreamSynchronize(b->stream));
-  }
-  b->bi_active = true;
-  b->kin_dirty = true;   // M, h and the poses of the getters describe the new parameters from the next getter on
-  return RSB_OK;
+  auto check = [&](float* out, const float* src, int n, int* bad) {
+    const int nrows = n * md.nb, threads = 128;
+    rsb_body_inertia_pack_kernel<<<(unsigned)((nrows + threads - 1) / threads), threads, 0, b->stream>>>(out, src, nrows, 1e-6, bad);
+  };
+  auto what = [&](int bad) {
+    static const char* fault[] = {"", "a value that is not finite", "a negative mass", "an inertia that is not symmetric positive semidefinite"};
+    const int r = bad / 4, env = env_begin + r / md.nb, body = r % md.nb;
+    return "body inertia: environment " + std::to_string(env) + ", body " + std::to_string(body) + " (" + md.body_names[body] + ") has " + fault[bad & 3];
+  };
+  const int rc = commit_env_rows(b, b->body_inertia, model_inertia_row(md), rows, env_begin, env_count, where, (size_t)md.nb * 10, check, what);
+  if (rc == RSB_OK && env_count > 0) b->kin_dirty = true;   // M, h and the poses of the getters describe the new parameters from the next getter on
+  return rc;
 }
 int rsb_batch_clear_body_inertia(rsb_batch* b) {
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
-  if (b->bi_active) b->kin_dirty = true;
-  b->bi_active = false;
+  if (b->body_inertia.active) b->kin_dirty = true;
+  b->body_inertia.active = false;
+  return RSB_OK;
+}
+// ---- per-environment terrain friction (World::setMaterialPairProp / setDefaultMaterial / CollisionBody::setMaterial per World
+// upstream): -1 is the batch-level value, resolved by the step kernel at every launch; the friction enters no getter, so nothing goes stale
+int rsb_batch_set_contact_friction(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  const Model& md = b->model->md;
+  const int ncoll = md.ncoll();
+  auto check = [&](float* out, const float* src, int n, int* bad) {
+    const int words = n * ncoll, threads = 128;
+    rsb_contact_friction_check_kernel<<<(unsigned)((words + threads - 1) / threads), threads, 0, b->stream>>>(out, src, words, bad);
+  };
+  auto what = [&](int bad) {
+    const int env = env_begin + bad / ncoll, c = bad % ncoll;
+    return "contact friction: environment " + std::to_string(env) + ", collision body " + std::to_string(c) + " (" + md.coll_names[c] + ") is not finite";
+  };
+  return commit_env_rows(b, b->contact_friction, std::vector<float>((size_t)ncoll, -1.f), rows, env_begin, env_count, where, (size_t)ncoll, check, what);
+}
+int rsb_batch_clear_contact_friction(rsb_batch* b) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  b->contact_friction.active = false;
   return RSB_OK;
 }
 int rsb_batch_set_control_mode(rsb_batch* b, int mode) {

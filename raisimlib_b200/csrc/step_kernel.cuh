@@ -232,6 +232,8 @@ struct StepArgs {
   const float* ext;    // optional [num_envs][EXT_WORDS] external wrench rows (body, F world, T world, point in body frame); null = none
   const float* body_inertia;   // optional [num_envs][nb][BI_WORDS] inertial rows (rsb_batch_set_body_inertia) read by stage A in place
                                // of the blob's BF_MASS / BF_COM / BF_INERTIA; null = the model's values for every environment
+  const float* contact_friction;   // optional [num_envs][ncoll] terrain friction rows (rsb_batch_set_contact_friction) read by stage C;
+                                   // an entry >= 0 replaces the batch-level value of the collision body's terrain contacts; null = none
   unsigned* prof;      // optional [num_envs][4 sub-steps][8] SM-clock stamps at the stage boundaries (tools/balance_probe.py)
   unsigned* prof_a;    // optional [num_envs][4 sub-steps][4] SM-clock stamps inside stage A: after the FK walk, the per-body terms, the
                        // subtree sums, the M columns (tools/stage_probe.py)
@@ -1553,11 +1555,15 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           float id = 1.0f / (a * c00 + bq * c01 + cc * c02);
           float* o = s_u + CB_WORDS * lane;
           float pm;
+          const int cand = __float_as_int(s_ct[lane * CT_WORDS + CF_PT]);
           if constexpr (SELF) {   // a self contact (candidate npts + j) takes the friction of its pair
-            const int cand = __float_as_int(s_ct[lane * CT_WORDS + CF_PT]);
             pm = cand < H.npts ? ptsf[5 * H.nptp + cand] : reinterpret_cast<const float*>(blob_s + H.off_pair)[PAIR_WORDS * (cand - H.npts) + PR_MU];
           } else {
-            pm = ptsf[5 * H.nptp + __float_as_int(s_ct[lane * CT_WORDS + CF_PT])];
+            pm = ptsf[5 * H.nptp + cand];
+          }
+          if (args.contact_friction && (!SELF || cand < H.npts)) {   // this environment's row for the candidate's collision body, if >= 0
+            const float pe = args.contact_friction[(size_t)env * H.ncoll + reinterpret_cast<const int*>(ptsf)[10 * H.nptp + cand]];
+            if (pe >= 0.f) pm = pe;
           }
           o[0] = a; o[1] = bq; o[2] = cc; o[3] = d; o[4] = e; o[5] = f;
           o[6] = pm >= 0.f ? pm : args.prm.mu;     // per-collision-body friction (World::setMaterialPairProp analogue)
