@@ -109,6 +109,8 @@ struct LockStep {
   int ncoll = 0;
   std::vector<float> friction;              // [n][ncoll] terrain friction rows (World material calls; -1: the batch's value); empty until the first one
   bool frictionDirty = false;
+  std::vector<float> actuator;              // [n][nv][3] kp, kd, effort limit (setPdGains / setActuationLimits; -1: the batch's); empty until the first one
+  bool actuatorDirty = false;
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
   bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
@@ -159,7 +161,8 @@ struct LockStep {
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
     if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
-    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = false;
+    if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
+    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
@@ -172,7 +175,8 @@ struct LockStep {
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
     if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
-    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = false;
+    if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
+    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
   }
   // environment env's terrain friction of one collision body, uploaded with the next flush() or pushWrites() (no launch of its own)
   void setFriction(int env, size_t collisionBody, double mu) {
@@ -181,6 +185,13 @@ struct LockStep {
     if (friction.empty()) friction.assign(size_t(n) * ncoll, -1.f);
     friction[size_t(env) * ncoll + collisionBody] = float(mu);
     frictionDirty = true;
+  }
+  // environment env's actuator row [nv][3] (batch gv order), written by the caller and uploaded with the next flush() or pushWrites()
+  float* actuatorRow(int env) {
+    sync(env);
+    if (actuator.empty()) actuator.assign(size_t(n) * nv * 3, -1.f);
+    actuatorDirty = true;
+    return &actuator[size_t(env) * nv * 3];
   }
 };
 
@@ -393,8 +404,14 @@ class ArticulatedSystem {
     for (size_t i = 0; i < t.size(); i++) t[vi(i)] = float(tau[i]);
     rsbCheck(rsb_batch_set_generalized_force(w_->batch(), t.data(), env_, 1, RSB_HOST), "setGeneralizedForce");
   }
-  // gains are shared by every environment of the batch (they are per-robot-model constants in RaisimGym)
+  // A stand-alone World sets the gains of its batch.  In a VectorizedEnvironment they are this environment's own: they go to its
+  // actuator row of the host mirror and up before the next launch (no launch of their own), as upstream's per-World gains do.
   template <class VV> void setPdGains(const VV& p, const VV& d) {
+    if (LockStep* ls = w_->lockStep()) {
+      float* r = ls->actuatorRow(env_);
+      for (int i = 0; i < ls->nv; i++) { r[3 * vi(i)] = float(p[i]); r[3 * vi(i) + 1] = float(d[i]); }
+      return;
+    }
     std::vector<float> kp(w_->nv()), kd(w_->nv());
     for (size_t i = 0; i < kp.size(); i++) { kp[vi(i)] = float(p[i]); kd[vi(i)] = float(d[i]); }
     rsbCheck(rsb_batch_set_pd_gains(w_->batch(), kp.data(), kd.data()), "setPdGains");
@@ -609,13 +626,14 @@ class ArticulatedSystem {
       for (int b = 1; b < t.nb; b++) if (t.vidx[b] == int(vi(size_t(i)))) { r[size_t(i)][0] = t.jlimit[2 * b]; r[size_t(i)][1] = t.jlimit[2 * b + 1]; }
     return r;
   }
-  // actuator effort limits per generalized velocity index (URDF <limit effort>; none: 1e30); the step kernel saturates the commanded torque there
+  // actuator effort limits per generalized velocity index (URDF <limit effort>, or this environment's setActuationLimits; none: 1e30
+  // or +inf); the step kernel saturates the commanded torque there
   VecDyn getActuationUpperLimits() const {
     const rsb_model_tables t = tables();
     VecDyn r(size_t(t.nv));
     for (int i = 0; i < t.nv; i++) {
       r[size_t(i)] = 1e30;
-      for (int b = 1; b < t.nb; b++) if (t.vidx[b] == int(vi(size_t(i)))) r[size_t(i)] = t.jeffort[b];
+      for (int b = 1; b < t.nb; b++) if (t.vidx[b] == int(vi(size_t(i)))) r[size_t(i)] = effort_.empty() ? t.jeffort[b] : effort_[size_t(i)];
     }
     return r;
   }
@@ -758,6 +776,24 @@ class ArticulatedSystem {
     kdLast_.resize(size_t(w_->nv())); for (size_t i = 0; i < kdLast_.size(); i++) kdLast_[i] = d[i];
     if (kpLast_.size() != kdLast_.size()) kpLast_.resize(kdLast_.size());
     setPdGains(kpLast_, kdLast_);
+  }
+  // This environment's actuator effort limits, per generalized velocity index: the commanded torque (feed-forward + PD) saturates at
+  // +-upper.  The step saturates symmetrically, so lower must be -upper with upper >= 0 (+inf: no limit); anything else fails loudly.
+  // The base dofs of a floating robot are not actuated and their entries are ignored.  A stand-alone World uploads the limits at once;
+  // in a VectorizedEnvironment they go to this environment's actuator row of the host mirror and up before the next launch.
+  template <class VV> void setActuationLimits(const VV& upper, const VV& lower) {
+    const int nv = w_->nv();
+    for (int i = 0; i < nv; i++)
+      if (!(upper[i] >= 0.0) || !(lower[i] == -upper[i]))
+        throw std::runtime_error("setActuationLimits: dof " + std::to_string(i) + ": only symmetric limits (lower = -upper, upper >= 0) are implemented by the batched step");
+    float* r = nullptr;
+    std::vector<float> own;
+    if (LockStep* ls = w_->lockStep()) r = ls->actuatorRow(env_);
+    else { own.assign(size_t(nv) * 3, -1.f); r = own.data(); }       // gains -1: the batch's (setPdGains)
+    for (int i = 0; i < nv; i++) r[3 * vi(i) + 2] = float(upper[i]);
+    if (!w_->lockStep()) rsbCheck(rsb_batch_set_actuator_params(w_->batch(), own.data(), env_, 1, RSB_HOST), "setActuationLimits");
+    effort_.assign(size_t(nv), 0.0);
+    for (int i = 0; i < nv; i++) effort_[size_t(i)] = upper[i];
   }
   // The batch integrates semi-implicitly (DESIGN.md section 2: v+ from the implicit PD / contact solve, then q+ = q (+) dt v+);
   // asking for another scheme fails loudly instead of silently integrating differently from what the caller expects.
@@ -909,6 +945,7 @@ class ArticulatedSystem {
   std::vector<Vec<3>> com_, appliedCom_;
   std::vector<Mat<3, 3>> inertia_;
   VecDyn lastP_, lastD_, kpLast_, kdLast_;
+  std::vector<double> effort_;                        // the last setActuationLimits() upper limits in the caller's order (empty: the URDF's)
   std::vector<int> qmap_, vmap_;
   BatchedWorld* w_;
   int env_;

@@ -191,7 +191,8 @@ int rsb_batch_set_self_collision(rsb_batch* b, const int32_t* pairs, int n, cons
  *      setGeneralizedForce/setControlMode); buffers are tight [env_count][nq|nv] float32 ---------- */
 int rsb_batch_set_state(rsb_batch* b, const float* gc, const float* gv, int env_begin, int env_count, int where);
 int rsb_batch_get_state(rsb_batch* b, float* gc, float* gv, int env_begin, int env_count, int where);
-int rsb_batch_set_pd_gains(rsb_batch* b, const float* kp, const float* kd);        /* [nv], host, all envs */
+/* [nv], host, all envs; per-environment actuator rows (rsb_batch_set_actuator_params) take precedence where they hold a value >= 0 */
+int rsb_batch_set_pd_gains(rsb_batch* b, const float* kp, const float* kd);
 int rsb_batch_set_pd_target(rsb_batch* b, const float* ptarget, const float* vtarget, int env_begin, int env_count, int where);
 /* zero-copy PD targets for trainers on the same GPU: the step kernel reads rows [env][0..nq) straight from the
  * caller's device buffer (row_stride floats apart) until targets are copied in again or NULL is bound */
@@ -215,11 +216,31 @@ int rsb_batch_set_external_wrench(rsb_batch* b, int body, const float* force, co
  * Refused with RSB_ERR_INVALID, changing nothing: a bad range or `where`, a value that is not finite, a negative mass, or an inertia
  * that is not positive semidefinite.  The inertia test, in double precision with t = xx + yy + zz: every diagonal entry >= -1e-6 t,
  * every 2 x 2 principal minor >= -1e-6 t^2 and the determinant >= -1e-6 t^3.  The rows are checked on the device in the batch's
- * staging buffer before any of them is committed; the call waits for that check.  Gains, effort limits and collision shapes stay per
- * batch; terrain friction has rows of its own (rsb_batch_set_contact_friction). */
+ * staging buffer before any of them is committed; the call waits for that check.  Collision shapes stay per batch; terrain friction
+ * (rsb_batch_set_contact_friction) and gains and effort limits (rsb_batch_set_actuator_params) have rows of their own. */
 int rsb_batch_set_body_inertia(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
 /* drop all per-environment rows: every later launch runs exactly as if none had ever been set */
 int rsb_batch_clear_body_inertia(rsb_batch* b);
+/* Per-environment PD gains and actuator effort limits (ArticulatedSystem::setPdGains / setPGains / setDGains / setActuationLimits, per
+ * World upstream).  rows [env_count][nv][3] float32 in the batch's gv order: kp, kd and the effort limit of every dof; host or device
+ * source (`where`).  An entry < 0 is the batch-level value, resolved at every launch: kp and kd of rsb_batch_set_pd_gains (0 if it was
+ * never called), the URDF <limit effort> of the joint; so a later rsb_batch_set_pd_gains still reaches the entries of -1.  An entry
+ * >= 0 replaces it for that dof in that environment: kp = kd = 0 gives the dof no PD law, effort 0 lets the actuator give no torque,
+ * effort +inf is no limit (stored as the batch's "none" value, so an unlimited joint computes the same bits either way).  The six
+ * base dofs of a floating robot are not actuated: their entries are ignored and stored as -1.  rows == NULL resets the range to -1.
+ * The first call (and the first after rsb_batch_clear_actuator_params) starts every environment at -1, then writes the range: no
+ * rows, rows of -1 and rows set then cleared compute the same bits, and so do rows equal to the batch-level values.
+ * The step kernel applies PD laws in RSB_PD_PLUS_FEEDFORWARD_TORQUE mode once rsb_batch_set_pd_gains was called or rows are active,
+ * and rsb_batch_gym_step accepts either.  The effort limit holds in both control modes, as the URDF one does (in RSB_FORCE_AND_TORQUE
+ * it saturates the feed-forward torque).  The rows live outside the model blob, so rsb_batch_set_pd_gains, set_collision_friction,
+ * set_self_collision, set_params, the terrain calls and gym resets keep them.  The gains enter neither M, h nor the poses: nothing
+ * goes stale and no launch is added.
+ * Refused with RSB_ERR_INVALID, changing nothing: a null batch, a bad range or `where`, NaN anywhere, +-inf in kp or kd, or -inf in
+ * the effort limit.  The rows are checked on the device in the batch's staging buffer before any of them is committed; the call waits
+ * for that check. */
+int rsb_batch_set_actuator_params(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
+/* drop all per-environment actuator rows: every later launch runs as if none had been set */
+int rsb_batch_clear_actuator_params(rsb_batch* b);
 /* ArticulatedSystem::getGeneralizedForce(): feed-forward + PD force applied over the last integrate() */
 int rsb_batch_get_generalized_force(rsb_batch* b, float* tau, int env_begin, int env_count, int where);
 
@@ -358,7 +379,8 @@ int rsb_batch_gym_configure(rsb_batch* b, const float* gc_init, const float* gv_
                             const int32_t* foot_bodies, int n_foot, float torque_coeff, float forward_vel_coeff, float terminal_reward);
 int rsb_batch_gym_reset(rsb_batch* b);                                             /* VectorizedEnvironment::reset() */
 /* ::step() + ::observe() in ONE launch of the step kernel: action rows -> PD targets, `substeps` x World::integrate(), reward,
- * isTerminalState(), reset() of the terminated environments, observation rows of the resulting state.  Needs rsb_batch_set_pd_gains(). */
+ * isTerminalState(), reset() of the terminated environments, observation rows of the resulting state.  Needs rsb_batch_set_pd_gains()
+ * or active per-environment actuator rows (rsb_batch_set_actuator_params). */
 int rsb_batch_gym_step(rsb_batch* b, const float* action, int where_in, int substeps, float* obs, float* reward, unsigned char* done,
                        int where_out);
 

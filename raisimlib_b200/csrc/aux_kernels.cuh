@@ -69,6 +69,25 @@ __global__ void rsb_contact_friction_check_kernel(float* __restrict__ out, const
   if (!isfinite(v)) atomicMin(bad, i);
 }
 
+// per-environment actuator rows (rsb_batch_set_actuator_params, StepArgs::actuator): the caller's [envs][nv][3] (kp, kd, effort limit)
+// repacked planar to [envs][3][nv], so that the lanes of a warp read one field of consecutive dofs.  The first `nbase` dofs (a floating
+// base: not actuated) are stored as -1; an effort limit >= 0 is clamped to the blob's "none" value 3e38 (+inf: no limit).  NaN
+// anywhere, +-inf in kp or kd and -inf in the effort limit lower *bad to (env * nv + dof) * 3 + field; *bad is left alone when every
+// value is accepted
+__global__ void rsb_actuator_params_check_kernel(float* __restrict__ out, const float* __restrict__ src, int envs, int nv, int nbase, int* bad) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= envs * nv) return;
+  const int e = r / nv, i = r - e * nv;
+  float* o = out + (size_t)e * 3 * nv + i;
+  for (int f = 0; f < 3; f++) {
+    float v = src[(size_t)r * 3 + f];
+    const bool ok = f < 2 ? isfinite(v) : !isnan(v) && v != -INFINITY;
+    if (!ok) atomicMin(bad, r * 3 + f);
+    if (f == 2 && v >= 0.f) v = fminf(v, 3.0e38f);
+    o[(size_t)f * nv] = i < nbase ? -1.f : v;
+  }
+}
+
 // ---- frame kinematics (rsb_batch_set_frames / get_frame_states / get_frame_jacobians) ----------------------------------------------
 // Frames rigidly attached to bodies and, per dof, what its Jacobian column needs; device arrays uploaded by rsb_batch_set_frames.
 // A dof turns or slides along the axis a of its body k (a = R_k axis: the joint frame's rotation about its own axis leaves the axis

@@ -130,12 +130,15 @@ struct rsb_batch {
   DevBuf<float> cf_force;
   DevBuf<int> cf_steps;
   // per-environment rows: inertial ones of rsb_batch_set_body_inertia [N][nb][BI_WORDS], terrain friction of
-  // rsb_batch_set_contact_friction [N][ncoll]; row_bad: the verdict of the check a call's rows pass before they replace any of them
-  EnvRows body_inertia, contact_friction;
+  // rsb_batch_set_contact_friction [N][ncoll], kp | kd | effort limit of rsb_batch_set_actuator_params [N][3][nv]; row_bad: the verdict
+  // of the check a call's rows pass before they replace any of them
+  EnvRows body_inertia, contact_friction, actuator;
   DevBuf<int> row_bad;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
+// the step kernel applies PD laws: PD mode, and gains from rsb_batch_set_pd_gains or per-environment actuator rows
+static bool pd_active(const rsb_batch* b) { return b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && (b->pd_set || b->actuator.active); }
 
 // ------------------------------------------------------------------ blob ------------------------
 static void build_blob(const Model& md, const Overrides& ov, LaunchConfig& cfg) {
@@ -390,7 +393,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
   a.num_envs = b->N; a.substeps = substeps;
   a.gc_stride = b->gc_stride; a.gv_stride = b->gv_stride;
   a.gc = b->gc.get(); a.gv = b->gv.get(); a.tau = b->tau.get();
-  a.use_pd = (b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && b->pd_set) ? 1 : 0;
+  a.use_pd = pd_active(b) ? 1 : 0;
   a.ptarget = b->pt_bound ? b->pt_bound : b->pt.get(); a.pt_stride = b->pt_bound ? b->pt_bound_stride : b->gc_stride;
   a.vtarget = b->vt_bound ? b->vt_bound : b->vt.get(); a.vt_stride = b->vt_bound ? b->vt_bound_stride : b->gv_stride;
   if (io.pt) { a.ptarget = io.pt; a.pt_stride = b->nq; a.pt_store = b->pt.get(); }
@@ -409,6 +412,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
   a.ext = b->ext_active ? b->ext.get() : nullptr;
   a.body_inertia = b->body_inertia.active ? b->body_inertia.rows.get() : nullptr;
   a.contact_friction = b->contact_friction.active ? b->contact_friction.rows.get() : nullptr;
+  a.actuator = b->actuator.active ? b->actuator.rows.get() : nullptr;
   a.obs = io.obs; a.ob_dim = rsb_batch_ob_dim(b);
   if (io.gym_action) {   // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
     a.gym_action = io.gym_action; a.gym = b->gym; a.gym_reward = io.gym_reward; a.gym_done = io.gym_done;
@@ -497,7 +501,8 @@ static int check_range(const rsb_batch* b, int env_begin, int env_count, int whe
   return RSB_OK;
 }
 
-// The one path by which a call's per-environment rows reach an EnvRows table (rsb_batch_set_body_inertia, set_contact_friction).
+// The one path by which a call's per-environment rows reach an EnvRows table (rsb_batch_set_body_inertia, set_contact_friction,
+// set_actuator_params).
 // `dflt` is one environment's row of the table (w words) when nothing overrides it: every environment starts from it at the first commit
 // after creation or a clear, and rows == null writes it to the range.  Otherwise the caller's rows (src_w words per environment) are
 // checked and packed to w words by check(out, src, env_count, bad) in the staging buffer (a host source passes through it too), and the
@@ -931,6 +936,30 @@ int rsb_batch_clear_contact_friction(rsb_batch* b) {
   b->contact_friction.active = false;
   return RSB_OK;
 }
+// ---- per-environment PD gains and actuator effort limits (ArticulatedSystem::setPdGains / setActuationLimits per World upstream):
+// -1 is the batch-level value (rsb_batch_set_pd_gains, the URDF effort limit), resolved by the step kernel at every launch; the gains
+// enter no getter, so nothing goes stale
+int rsb_batch_set_actuator_params(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  const Model& md = b->model->md;
+  const int nv = md.nv;
+  auto check = [&](float* out, const float* src, int n, int* bad) {
+    const int threads = 128;
+    rsb_actuator_params_check_kernel<<<(unsigned)((n * nv + threads - 1) / threads), threads, 0, b->stream>>>(out, src, n, nv, md.floating ? 6 : 0, bad);
+  };
+  auto what = [&](int bad) {
+    static const char* field[] = {"kp", "kd", "effort limit"};
+    static const char* fault[] = {"is NaN or infinite", "is NaN or infinite", "is NaN or -inf"};
+    const int r = bad / 3, env = env_begin + r / nv, dof = r % nv;
+    return "actuator params: environment " + std::to_string(env) + ", dof " + std::to_string(dof) + ": " + field[bad % 3] + " " + fault[bad % 3];
+  };
+  return commit_env_rows(b, b->actuator, std::vector<float>((size_t)3 * nv, -1.f), rows, env_begin, env_count, where, (size_t)3 * nv, check, what);
+}
+int rsb_batch_clear_actuator_params(rsb_batch* b) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  b->actuator.active = false;
+  return RSB_OK;
+}
 int rsb_batch_set_control_mode(rsb_batch* b, int mode) {
   if (!b || (mode != RSB_FORCE_AND_TORQUE && mode != RSB_PD_PLUS_FEEDFORWARD_TORQUE)) return fail(RSB_ERR_INVALID, "bad control mode");
   b->control_mode = mode;
@@ -1185,7 +1214,7 @@ int rsb_batch_control_step(rsb_batch* b, const float* ptarget, const float* vtar
   // Host buffers in pinned (page-locked, mapped) memory are read and written IN PLACE by the step kernel over PCIe:
   // no staging copy, no separate H2D / D2H operations on the stream.  Pageable buffers take the staged path.
   // Targets given here end a persistent rsb_batch_bind_pd_target() binding; pinned ones are read in place by this launch only.
-  const bool pd_mode = b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && b->pd_set;
+  const bool pd_mode = pd_active(b);
   LaunchIO io;
   int rc = RSB_OK;
   if (ptarget) {
@@ -1292,7 +1321,7 @@ int rsb_batch_gym_step(rsb_batch* b, const float* action, int where_in, int subs
   unsigned char* d_done = a_done ? a_done : (host_out || !done) ? b->gym_done.get() : done;
   // ONE launch: action rows -> PD targets, `substeps` x World::integrate(), reward, isTerminalState(), reset() of the terminated
   // environments and the observation rows of the resulting state (the task used to be an action kernel and a post kernel around the step)
-  if (!(b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && b->pd_set)) return fail(RSB_ERR_INVALID, "the gym task drives the robot through PD targets: call rsb_batch_set_pd_gains() first");
+  if (!pd_active(b)) return fail(RSB_ERR_INVALID, "the gym task drives the robot through PD targets: call rsb_batch_set_pd_gains() or rsb_batch_set_actuator_params() first");
   LaunchIO io;
   io.obs = d_obs; io.gym_action = act; io.gym_reward = d_rew; io.gym_done = d_done;
   int rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;

@@ -234,6 +234,8 @@ struct StepArgs {
                                // of the blob's BF_MASS / BF_COM / BF_INERTIA; null = the model's values for every environment
   const float* contact_friction;   // optional [num_envs][ncoll] terrain friction rows (rsb_batch_set_contact_friction) read by stage C;
                                    // an entry >= 0 replaces the batch-level value of the collision body's terrain contacts; null = none
+  const float* actuator;   // optional [num_envs][3][nv] kp | kd | effort limit rows (rsb_batch_set_actuator_params) read by stages C and E;
+                           // an entry >= 0 replaces the blob's value of that dof; null = none
   unsigned* prof;      // optional [num_envs][4 sub-steps][8] SM-clock stamps at the stage boundaries (tools/balance_probe.py)
   unsigned* prof_a;    // optional [num_envs][4 sub-steps][4] SM-clock stamps inside stage A: after the FK walk, the per-body terms, the
                        // subtree sums, the M columns (tools/stage_probe.py)
@@ -767,6 +769,23 @@ __device__ __forceinline__ void apply_row_bias(float& u_c, const rsb_params& prm
   }
 }
 
+// Stages C and E: kp, kd and effort limit of dof i in environment env.  The blob's value (gain: kp | kd | effort, nvp each) unless the
+// environment has a row (StepArgs::actuator) whose entry is >= 0; the gains are 0 outside PD mode (use_pd), the effort limit holds in
+// both control modes
+__device__ __forceinline__ void dof_actuator(const StepArgs& args, const float* gain, int nvp, int env, int nv, int i, float& kpi, float& kdi, float& emi) {
+  kpi = args.use_pd ? gain[i] : 0.f; kdi = args.use_pd ? gain[nvp + i] : 0.f; emi = gain[2 * nvp + i];
+  if (args.actuator) {
+    const float* r = args.actuator + (size_t)env * 3 * nv + i;
+    if (args.use_pd) {
+      const float rp = r[0], rd = r[nv];
+      if (rp >= 0.f) kpi = rp;
+      if (rd >= 0.f) kdi = rd;
+    }
+    const float re = r[2 * nv];
+    if (re >= 0.f) emi = re;
+  }
+}
+
 // Stage E, static humanoid and generic instances: adds Y[di] . lam of the contacts whose column block Y (rows 3k..3k+2) lies on a chain
 // through dof i (depth di) to sacc; SECOND: the self contacts' second halves (the chain of the pair's second body), subtracted
 template <int UNR, bool SECOND>
@@ -848,9 +867,8 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
   const int* bodyi = reinterpret_cast<const int*>(blob_s + HO(off_body));
   const int* anc = reinterpret_cast<const int*>(blob_s + HO(off_anc));
   const float* ptsf = reinterpret_cast<const float*>(blob_s + HO(off_pts));
-  const float* kp = reinterpret_cast<const float*>(blob_s + HO(off_gain));
-  const float* kd = kp + nvp;
-  const float* emax = kp + 2 * nvp;     // actuator effort limit per dof (URDF <limit effort>, 3e38 = none)
+  // kp | kd | actuator effort limit per dof (URDF <limit effort>, 3e38 = none), each nvp long (dof_actuator)
+  const float* gain = reinterpret_cast<const float*>(blob_s + HO(off_gain));
   const int* dofq = reinterpret_cast<const int*>(blob_s + HO(off_dofq));
   const float* sec_c = reinterpret_cast<const float*>(blob_s + HO(off_sec));
   const int nbase = HO(nbase), maxdd = HO(maxdd), DLP = HO(dlp);
@@ -1234,15 +1252,16 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         // actuator effort limit (oracle step()): when feed-forward + PD law at the current state exceed it, the joint is driven by the
         // constant limit torque over this step and gets no implicit PD terms
         float te = s_tau[i];
-        const float kpi = args.use_pd ? kp[i] : 0.f, kdi = args.use_pd ? kd[i] : 0.f;
+        float kpi, kdi, emi;
+        dof_actuator(args, gain, nvp, env, nv, i, kpi, kdi, emi);
         const bool pd = kpi != 0.f || kdi != 0.f;
         const int qi = pd ? dofq[i] : 0;
         if (pd) te += kpi * (s_pt[qi] - s_gc[qi]) + kdi * (s_vt[i] - s_gv[i]);
         // ... judged on the torque the implicit law would really apply (the explicit value over 1 + (dt kd + dt^2 kp) / M_dd)
         const float soft = args.prm.dt * kdi + args.prm.dt * args.prm.dt * kpi;
-        const bool sat = fabsf(te) > emax[i] * (1.f + soft / s_L[i * DLP + ddepth[i]]);
+        const bool sat = fabsf(te) > emi * (1.f + soft / s_L[i * DLP + ddepth[i]]);
         s_sat[i] = sat ? 1.f : 0.f;          // remembered for stage E (generalized force applied)
-        if (sat) bi += copysignf(emax[i], te) - s_tau[i];
+        if (sat) bi += copysignf(emi, te) - s_tau[i];
         else if (pd) {
           bi += kpi * (s_pt[qi] - s_gc[qi] - args.prm.dt * s_gv[i]) + kdi * (s_vt[i] - s_gv[i]);
           s_L[i * DLP + ddepth[i]] += args.prm.dt * kdi + args.prm.dt * args.prm.dt * kpi;
@@ -1667,12 +1686,13 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         s_gv[i] = vp;
         // generalized force applied over this step (implicit PD evaluated at q + dt v+, v+; the effort limit where it was hit): getGeneralizedForce()
         float ta = s_tau[i];
-        const float kpi = args.use_pd ? kp[i] : 0.f, kdi = args.use_pd ? kd[i] : 0.f;
+        float kpi, kdi, emi;
+        dof_actuator(args, gain, nvp, env, nv, i, kpi, kdi, emi);
         const bool pd = kpi != 0.f || kdi != 0.f;
         const int qi = pd ? dofq[i] : 0;
         float te = ta;
         if (pd) te += kpi * (s_pt[qi] - s_gc[qi]) + kdi * (s_vt[i] - v0);
-        if (s_sat[i] != 0.f) ta = copysignf(emax[i], te);
+        if (s_sat[i] != 0.f) ta = copysignf(emi, te);
         else if (pd) ta += kpi * (s_pt[qi] - s_gc[qi] - args.prm.dt * vp) + kdi * (s_vt[i] - vp);
         s_b[i] = ta;
       }

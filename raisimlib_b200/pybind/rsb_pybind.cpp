@@ -119,6 +119,10 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void set_contact_friction(uintptr_t rows_dev, int env_begin, int env_count) {
     check(rsb_batch_set_contact_friction(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_contact_friction");
   }
+  // per-environment actuator rows [env_count, nv, 3] float32 (kp, kd, effort limit; >= 0: this dof's own, < 0: the batch's) from a device address
+  void set_actuator_params(uintptr_t rows_dev, int env_begin, int env_count) {
+    check(rsb_batch_set_actuator_params(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_actuator_params");
+  }
   int num_envs() const { return view_.num_envs; }
   int nq() const { return view_.nq; }
   int nv() const { return view_.nv; }
@@ -157,6 +161,7 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("body_contact_forces", &Batch::body_contact_forces, py::arg("force_dev"), py::arg("steps_dev"))
       .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_contact_friction", &Batch::set_contact_friction, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
+      .def("set_actuator_params", &Batch::set_actuator_params, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("sync", &Batch::sync)
       .def_property_readonly("num_envs", &Batch::num_envs)
       .def_property_readonly("nq", &Batch::nq)
