@@ -111,6 +111,9 @@ struct LockStep {
   bool frictionDirty = false;
   std::vector<float> actuator;              // [n][nv][3] kp, kd, effort limit (setPdGains / setActuationLimits; -1: the batch's); empty until the first one
   bool actuatorDirty = false;
+  std::vector<float> scan, scanXy;          // [n][P], [n][P][2] heights and sample locations of the height scan (ArticulatedSystem::setHeightScan)
+  int scanPoints = 0;
+  bool scanValid = false;
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
   bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
@@ -149,6 +152,15 @@ struct LockStep {
     rsbCheck(rsb_batch_get_body_contact_forces(batch, 0, n, cfForce.data(), cfSteps.data(), RSB_HOST), "getBodyContactForce");
     cfValid = true;
   }
+  // the height scan of every environment in one call, after the rows written since the last launch went up (a reset() that moved a
+  // robot is seen); valid until the next flush() or state write
+  void needHeightScan() {
+    pushWrites();
+    if (scanValid) return;
+    scan.resize(size_t(n) * scanPoints); scanXy.resize(size_t(n) * scanPoints * 2);
+    rsbCheck(rsb_batch_get_height_scan(batch, 0, n, scan.data(), scanXy.data(), RSB_HOST), "getHeightScan");
+    scanValid = true;
+  }
   // every environment is parked (or finished) with the same number of integrate() calls pending: upload, one launch, invalidate
   void flush() {
     int k = 0;
@@ -166,11 +178,11 @@ struct LockStep {
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
-    stateValid = tauAppliedValid = contactsValid = cfValid = false;
+    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = false;
   }
   // rows written outside a step (reset(), init()): push them before anything else reads the device
   void pushWrites() {
-    if (stateDirty) rsbCheck(rsb_batch_set_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "setState");
+    if (stateDirty) { rsbCheck(rsb_batch_set_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "setState"); scanValid = false; }
     if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
     if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
@@ -225,7 +237,7 @@ class BatchedWorld {
   LockStep* lockStep() { return ls_.get(); }
   void enableLockStep() {
     if (ls_) return;
-    ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); ls_->cfBodies = int(contactBodies_.size());
+    ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); ls_->cfBodies = int(contactBodies_.size()); ls_->scanPoints = int(scanBodies_.size());
     rsbCheck(rsb_model_dims(model_, nullptr, nullptr, nullptr, &ls_->ncoll, nullptr), "dims");
   }
   // bodies whose contact force every integrate() gathers (ArticulatedSystem::setContactBodies): one list for all environments
@@ -241,11 +253,23 @@ class BatchedWorld {
     throw std::runtime_error("getBodyContactForce: body " + std::to_string(bodyIdx) + " is not among the bodies given to setContactBodies()");
   }
   size_t numContactBodies() const { return contactBodies_.size(); }
+  // terrain height-scan points (ArticulatedSystem::setHeightScan): one list for all environments
+  void setHeightScan(const std::vector<int32_t>& bodies, const std::vector<float>& xy, bool yawAligned) {
+    if (bodies == scanBodies_ && xy == scanXy_ && yawAligned == scanYaw_) return;   // every environment sets the same list in its constructor
+    if (xy.size() != 2 * bodies.size()) throw std::runtime_error("setHeightScan: one offset per body");
+    rsbCheck(rsb_batch_set_height_scan(batch_, bodies.data(), xy.data(), int(bodies.size()), yawAligned ? RSB_SCAN_YAW : RSB_SCAN_WORLD), "setHeightScan");
+    scanBodies_ = bodies; scanXy_ = xy; scanYaw_ = yawAligned;
+    if (ls_) { ls_->scanPoints = int(bodies.size()); ls_->scanValid = false; }
+  }
+  size_t numHeightScanPoints() const { return scanBodies_.size(); }
   const std::string& urdf() const { return urdf_; }
   void rememberUrdf(const std::string& u) { urdf_ = u; }
  private:
   std::unique_ptr<LockStep> ls_;
   std::vector<size_t> contactBodies_;
+  std::vector<int32_t> scanBodies_;
+  std::vector<float> scanXy_;
+  bool scanYaw_ = true;
   std::string urdf_;
   rsb_model* model_ = nullptr;
   rsb_batch* batch_ = nullptr;
@@ -843,6 +867,40 @@ class ArticulatedSystem {
     std::vector<int32_t> n(S);
     rsbCheck(rsb_batch_get_body_contact_forces(w_->batch(), env_, 1, nullptr, n.data(), RSB_HOST), "getBodyContactSteps");
     return n[s];
+  }
+  // setHeightScan: terrain height samples at horizontal offsets (x, y) from bodies (getBodyIdx order, at most RSB_MAX_SCAN_POINTS),
+  // turned with each body's heading (yawAligned) or along the world axes: what an upstream observe() builds with one
+  // HeightMap::getHeight call per point.  The list belongs to the batch: every environment shares it, and each environment of a
+  // VectorizedEnvironment may set the same list in its constructor.
+  void setHeightScan(const std::vector<size_t>& bodies, const std::vector<Vec<2>>& offsets, bool yawAligned = true) {
+    if (offsets.size() != bodies.size()) throw std::runtime_error("setHeightScan: one offset per body");
+    std::vector<int32_t> b(bodies.begin(), bodies.end());
+    std::vector<float> xy(2 * offsets.size());
+    for (size_t i = 0; i < offsets.size(); i++) { xy[2 * i] = float(offsets[i][0]); xy[2 * i + 1] = float(offsets[i][1]); }
+    w_->setHeightScan(b, xy, yawAligned);
+  }
+  // the world z of the collision surface under every point at the current state, in setHeightScan order, and (samples, optional) the
+  // world (x, y) each was taken at.  In a VectorizedEnvironment one call scans every environment for the control step; a stand-alone
+  // World scans this environment
+  void getHeightScan(VecDyn& heights, std::vector<Vec<2>>* samples = nullptr) {
+    const size_t P = w_->numHeightScanPoints();
+    if (P == 0) throw std::runtime_error("getHeightScan: call setHeightScan() first");
+    const float *h, *xy;
+    std::vector<float> own;
+    if (LockStep* ls = w_->lockStep()) {
+      ls->sync(env_); ls->needHeightScan();
+      h = &ls->scan[size_t(env_) * P]; xy = &ls->scanXy[size_t(env_) * P * 2];
+    } else {
+      own.resize(3 * P);
+      rsbCheck(rsb_batch_get_height_scan(w_->batch(), env_, 1, own.data(), samples ? own.data() + P : nullptr, RSB_HOST), "getHeightScan");
+      h = own.data(); xy = own.data() + P;
+    }
+    heights.resize(P);
+    for (size_t i = 0; i < P; i++) heights[i] = h[i];
+    if (samples) {
+      samples->resize(P);
+      for (size_t i = 0; i < P; i++) { (*samples)[i][0] = xy[2 * i]; (*samples)[i][1] = xy[2 * i + 1]; }
+    }
   }
   int env() const { return env_; }
  private:

@@ -313,6 +313,31 @@ int rsb_batch_set_contact_bodies(rsb_batch* b, const int32_t* body, int n);
 /* force [n][S][3] float32, steps_in_contact [n][S] int32, S = the number of bodies set; a NULL output is skipped; RSB_ERR_INVALID when
  * no bodies are set.  A plain copy of a contiguous slice of the batch's rows in stream order: no launch, host or device destination. */
 int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count, float* force, int32_t* steps_in_contact, int where);
+/* ---- terrain height scans (what an upstream ENVIRONMENT builds in observe() with HeightMap::getHeight(x, y) once per point, for
+ *      every environment at once).  One list of points, shared by all environments; point i hangs on body[i] at the horizontal
+ *      offset xy[i][2].  Its sample is, with (p, R) the body's world pose:
+ *        RSB_SCAN_YAW    p_xy + Rz(psi) offset, (cos psi, sin psi) = (R00, R10) normalised (psi = 0 when that norm is < 1e-6):
+ *                        the offsets turn with the body's heading and ignore its roll and pitch;
+ *        RSB_SCAN_WORLD  p_xy + offset.
+ *      The height is the world z of the collision surface there: the ground's z, or the environment's own height map (terrain atlas),
+ *      two triangles per cell split along P00-P11 with the narrow phase's float arithmetic, so the scan shows the surface the robot
+ *      collides with.  Outside the map the sample is clamped to the nearest border point, as HeightMap::getHeight does.  A sample with
+ *      a coordinate that is not finite (a diverged environment) reads NaN.  The terrain is read at call time.
+ *      Poses: a point on the root of a floating-base robot takes its pose from gc (position gc[0:3], heading from the normalised
+ *      quaternion), so a list of base points is one launch and never runs the kinematics pass; a point on any other body uses the
+ *      kinematics pass's poses, which the call runs first when they are stale, as the frame getters do.  The scan leaves the state,
+ *      contact records, contact forces, solver outputs, diverged flags and applied torques as they were and has no effect on any
+ *      later step.  Host outputs are staged through the batch's staging buffer (env_count * P * 3 floats). */
+#define RSB_MAX_SCAN_POINTS 1024
+#define RSB_SCAN_YAW 0   /* offsets turn with the anchor body's heading */
+#define RSB_SCAN_WORLD 1 /* offsets are along the world x / y axes      */
+/* body[n] in rsb_model_body_index order, xy[n][2], align RSB_SCAN_YAW / RSB_SCAN_WORLD for all points.  n = 0 clears.  Refused with
+ * RSB_ERR_INVALID, changing nothing: n < 0 or > RSB_MAX_SCAN_POINTS, body or xy NULL with n > 0, a body out of range, an offset that is
+ * not finite, another align. */
+int rsb_batch_set_height_scan(rsb_batch* b, const int32_t* body, const float* xy, int n, int align);
+/* height [n][P] (world z of the surface at each sample) and xy_out [n][P][2] (the world sample location), P = the number of points
+ * set; a NULL output is skipped (both NULL: nothing is launched).  RSB_ERR_INVALID when no points are set or there is no terrain. */
+int rsb_batch_get_height_scan(rsb_batch* b, int env_begin, int env_count, float* height, float* xy_out, int where);
 /* FK, M and h of the CURRENT state for the getters above, without touching the contact records of the last integrate()
  * (upstream's getters are lazy the same way).  The getters call it themselves when the state changed through this API;
  * call it explicitly after writing the state through rsb_batch_device_ptrs() views. */

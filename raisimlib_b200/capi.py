@@ -12,6 +12,8 @@ LIB_PATH = os.environ.get("RSB_LIB_PATH") or os.path.join(_HERE, "librsb.so")   
 KMAX = 8
 HOST, DEVICE = 0, 1
 FORCE_AND_TORQUE, PD_PLUS_FEEDFORWARD_TORQUE = 0, 1
+SCAN_YAW, SCAN_WORLD = 0, 1
+MAX_SCAN_POINTS = 1024
 
 
 class RsbError(RuntimeError):
@@ -102,6 +104,7 @@ EXPORTED = [
     "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
     "rsb_batch_set_frames", "rsb_batch_get_frame_states", "rsb_batch_get_frame_jacobians",
     "rsb_batch_set_contact_bodies", "rsb_batch_get_body_contact_forces",
+    "rsb_batch_set_height_scan", "rsb_batch_get_height_scan",
     "rsb_batch_ob_dim", "rsb_batch_observe", "rsb_batch_control_step",
     "rsb_batch_gym_configure", "rsb_batch_gym_reset", "rsb_batch_gym_step",
     "rsb_peer_buffer_create", "rsb_peer_buffer_open", "rsb_peer_buffer_close", "rsb_peer_buffer_destroy", "rsb_batch_set_observation_peers", "rsb_batch_wait_observation_peers",
@@ -188,6 +191,9 @@ def lib():
         if hasattr(L, "rsb_batch_set_actuator_params"):    # absent from an older build loaded through RSB_LIB_PATH (tools/actuator_params_probe.py)
             L.rsb_batch_set_actuator_params.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
             L.rsb_batch_clear_actuator_params.argtypes = [C.c_void_p]
+        if hasattr(L, "rsb_batch_set_height_scan"):        # absent from an older build loaded through RSB_LIB_PATH (tools/height_scan_probe.py)
+            L.rsb_batch_set_height_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+            L.rsb_batch_get_height_scan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
         L.rsb_batch_device_ptrs.argtypes = [C.c_void_p, C.POINTER(DeviceView)]
         L.rsb_batch_launch_count.argtypes = [C.c_void_p]
         L.rsb_batch_ob_dim.argtypes = [C.c_void_p]
@@ -293,7 +299,7 @@ class Batch:
         h = C.c_void_p()
         _ck(lib().rsb_batch_create(model.h, num_envs, device, C.byref(h)))
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
-        self.device, self.nframes, self.ncontact_bodies = device, 0, 0
+        self.device, self.nframes, self.ncontact_bodies, self.nscan = device, 0, 0, 0
 
     def __del__(self):
         if getattr(self, "h", None) and lib is not None and _lib is not None:
@@ -542,6 +548,38 @@ class Batch:
         n, S = self._count(env_begin, env_count), self.ncontact_bodies
         _ck(lib().rsb_batch_get_body_contact_forces(self.h, env_begin, n, self._device_out(force, (n, S, 3), "force"),
                                                     self._device_out(steps, (n, S), "steps", "int32"), DEVICE))
+
+    # terrain height scans
+    def set_height_scan(self, body, xy, align="yaw"):
+        """sample points shared by all environments: point i hangs on body[i] at the horizontal offset xy[i] = (dx, dy); align "yaw"
+        turns the offsets with the body's heading, "world" keeps them along the world axes.  An empty list clears them; a refused
+        call keeps the points set before."""
+        modes = {"yaw": SCAN_YAW, "world": SCAN_WORLD}
+        if align not in modes:
+            raise ValueError(f"set_height_scan: align must be 'yaw' or 'world', got {align!r}")
+        bd = np.ascontiguousarray(body, np.int32).reshape(-1)
+        p = np.ascontiguousarray(xy, np.float32).reshape(-1, 2)
+        if len(p) != len(bd):
+            raise ValueError(f"set_height_scan: {len(bd)} bodies, {len(p)} offsets")
+        _ck(lib().rsb_batch_set_height_scan(self.h, bd.ctypes.data_as(C.c_void_p), p.ctypes.data_as(C.c_void_p), len(bd), modes[align]))
+        self.nscan = len(bd)
+
+    def set_height_scan_by_name(self, names, xy, align="yaw"):
+        """set_height_scan() with the bodies given by link name (rsb_model_body_index: a merged link names its body)"""
+        self.set_height_scan([self.model.body_index(n) for n in names], xy, align)
+
+    def height_scan(self, env_begin=0, env_count=None):
+        """(height [n, P]: world z of the collision surface under every sample, xy [n, P, 2]: the world sample locations) at the
+        current state"""
+        n = self._count(env_begin, env_count)
+        h, xy = np.empty((n, self.nscan), np.float32), np.empty((n, self.nscan, 2), np.float32)
+        _ck(lib().rsb_batch_get_height_scan(self.h, env_begin, n, h.ctypes.data_as(C.c_void_p), xy.ctypes.data_as(C.c_void_p), HOST))
+        return h, xy
+
+    def height_scan_into(self, height=None, xy=None, env_begin=0, env_count=None):
+        """height_scan() written into torch CUDA tensors [n, P] / [n, P, 2] (None skips one), in the batch's stream order"""
+        n, P = self._count(env_begin, env_count), self.nscan
+        _ck(lib().rsb_batch_get_height_scan(self.h, env_begin, n, self._device_out(height, (n, P), "height"), self._device_out(xy, (n, P, 2), "xy"), DEVICE))
 
     def diverged(self, env_begin=0, env_count=None):
         return self._read(lib().rsb_batch_get_diverged, (), np.int32, env_begin, env_count)

@@ -174,6 +174,74 @@ __global__ void __launch_bounds__(128) rsb_frame_kernel(FrameTable ft, const flo
   }
 }
 
+// ---- terrain height scans (rsb_batch_set_height_scan / get_height_scan) ----------------------------------------------------------
+// World z of the collision surface under (x, y), clamped to the nearest border point outside a height map as HeightMap::getHeight
+// does.  Inside the map the float arithmetic is terrain_query's (step_kernel.cuh): the division by the pitch, fx >= fy picking the
+// triangle, zt = h00 + sx fx + sy fy; so the scan reports the heights the narrow phase collides with.  A coordinate that is not finite
+// gives NaN (clamping it would report a corner of the map for a diverged environment).
+__device__ __forceinline__ float scan_surface_height(const TerrainDesc& t, int hm_offset, float x, float y) {
+  if (!isfinite(x) || !isfinite(y)) return __int_as_float(0x7fffffff);
+  if (t.type == 1) return t.ground_z;
+  const float gx = fminf(fmaxf((x - t.x0) / t.dx, 0.f), t.xmax), gy = fminf(fmaxf((y - t.y0) / t.dy, 0.f), t.ymax);
+  const int ix = min((int)gx, t.xs - 2), iy = min((int)gy, t.ys - 2);
+  const float fx = gx - (float)ix, fy = gy - (float)iy;
+  const float* H = t.h + hm_offset + iy * t.xs + ix;
+  const float h00 = __ldg(H), h10 = __ldg(H + 1), h01 = __ldg(H + t.xs), h11 = __ldg(H + t.xs + 1);
+  float sx, sy;
+  if (fx >= fy) { sx = h10 - h00; sy = h11 - h10; }
+  else { sx = h11 - h01; sy = h01 - h00; }
+  return h00 + sx * fx + sy * fy;
+}
+
+// The points of rsb_batch_set_height_scan: body [RSB_MAX_SCAN_POINTS] | offsets xy [RSB_MAX_SCAN_POINTS][2], one device allocation.
+struct ScanTable {
+  int n, align;             // points, RSB_SCAN_YAW / RSB_SCAN_WORLD
+  int root_from_gc;         // a floating base: points on body 0 take its pose from gc
+  const int* body;
+  const float* xy;
+};
+
+// One thread per (environment, point), in flat output order: height is written coalesced.  R [N][nb][9], P [N][nb][3]: the kinematics
+// pass's poses (read only for points off a floating root); outputs are tight rows of the environments [env_begin, env_begin + count);
+// a null output is skipped.
+__global__ void __launch_bounds__(256) rsb_height_scan_kernel(ScanTable st, TerrainDesc ter, const float* __restrict__ gc, int gc_stride,
+                                                              const float* __restrict__ R, const float* __restrict__ P, int nb, int env_begin,
+                                                              int count, float* __restrict__ height_out, float* __restrict__ xy_out) {
+  const long w = (long)blockIdx.x * blockDim.x + threadIdx.x;   // output row: (environment - env_begin) * n + point
+  if (w >= (long)count * st.n) return;
+  const int i = (int)(w % st.n);
+  const long e = env_begin + w / st.n;
+  const int b = __ldg(st.body + i);
+  const float ox = __ldg(st.xy + 2 * i), oy = __ldg(st.xy + 2 * i + 1);
+  float px, py, c0, c1;                           // anchor position and (R00, R10) of its rotation
+  if (b == 0 && st.root_from_gc) {
+    const float* q = gc + e * gc_stride;
+    px = q[0]; py = q[1];
+    float qw = q[3], qx = q[4], qy = q[5], qz = q[6];
+    const float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);   // as write_obs_row normalises it
+    qw *= inv; qx *= inv; qy *= inv; qz *= inv;
+    float c2;
+    obs_rot_column(qw, qx, qy, qz, 0, c0, c1, c2);
+  } else {
+    const float* Rb = R + (e * nb + b) * 9;
+    const float* pb = P + (e * nb + b) * 3;
+    px = pb[0]; py = pb[1]; c0 = Rb[0]; c1 = Rb[3];
+  }
+  float sx = px + ox, sy = py + oy;
+  if (st.align == RSB_SCAN_YAW) {
+    const float nrm = sqrtf(c0 * c0 + c1 * c1);
+    float c = 1.f, s = 0.f;
+    if (!(nrm < 1e-6f)) { c = c0 / nrm; s = c1 / nrm; }   // a NaN heading stays NaN
+    sx = px + (c * ox - s * oy);
+    sy = py + (s * ox + c * oy);
+  }
+  if (xy_out) { xy_out[2 * w] = sx; xy_out[2 * w + 1] = sy; }
+  if (height_out) {
+    const int hm_offset = ter.env_map ? __ldg(ter.env_map + e) * ter.map_words : 0;   // terrain atlas
+    height_out[w] = scan_surface_height(ter, hm_offset, sx, sy);
+  }
+}
+
 }  // namespace rsb
 
 // ---- RaisimGym ANYmal locomotion task on the device (SURVEY.md 8f N1; [RECALL] raisimGymTorch

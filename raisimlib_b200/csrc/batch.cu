@@ -129,6 +129,11 @@ struct rsb_batch {
   std::vector<uint8_t> contact_bodies;
   DevBuf<float> cf_force;
   DevBuf<int> cf_steps;
+  // points of rsb_batch_set_height_scan (scan.n = 0: none) in one device allocation sized for RSB_MAX_SCAN_POINTS; scan_off_root: a
+  // point hangs on a body whose pose comes from the kinematics pass
+  ScanTable scan{};
+  DevBuf<int> scan_tab;
+  bool scan_off_root = false;
   // per-environment rows: inertial ones of rsb_batch_set_body_inertia [N][nb][BI_WORDS], terrain friction of
   // rsb_batch_set_contact_friction [N][ncoll], kp | kd | effort limit of rsb_batch_set_actuator_params [N][3][nv]; row_bad: the verdict
   // of the check a call's rows pass before they replace any of them
@@ -1141,6 +1146,57 @@ int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count
   const size_t S = b->contact_bodies.size();
   rc = force ? copy_out(b, force, b->cf_force.get() + (size_t)env_begin * S * 3, (size_t)env_count * S * 3 * 4, where) : RSB_OK; if (rc) return rc;
   return steps_in_contact ? copy_out(b, steps_in_contact, b->cf_steps.get() + (size_t)env_begin * S, (size_t)env_count * S * 4, where) : RSB_OK;
+}
+// ---- terrain height scans: the surface height under body-attached sample points, one launch of rsb_height_scan_kernel -------------
+int rsb_batch_set_height_scan(rsb_batch* b, const int32_t* body, const float* xy, int n, int align) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (n < 0 || n > RSB_MAX_SCAN_POINTS) return fail(RSB_ERR_INVALID, "at most " + std::to_string(RSB_MAX_SCAN_POINTS) + " height-scan points per batch (got " + std::to_string(n) + ")");
+  if (n > 0 && (!body || !xy)) return fail(RSB_ERR_INVALID, "null height-scan body or offset list");
+  if (align != RSB_SCAN_YAW && align != RSB_SCAN_WORLD) return fail(RSB_ERR_INVALID, "height-scan align must be RSB_SCAN_YAW or RSB_SCAN_WORLD");
+  for (int i = 0; i < n; i++) {
+    if (body[i] < 0 || body[i] >= b->nb) return fail(RSB_ERR_INVALID, "height-scan point " + std::to_string(i) + ": body index out of range (the model has " + std::to_string(b->nb) + ")");
+    if (!std::isfinite(xy[2 * i]) || !std::isfinite(xy[2 * i + 1])) return fail(RSB_ERR_INVALID, "height-scan point " + std::to_string(i) + ": offset is not finite");
+  }
+  if (n == 0) { b->scan.n = 0; return RSB_OK; }
+  const int M = RSB_MAX_SCAN_POINTS;
+  std::vector<int32_t> W((size_t)3 * M, 0);   // body[M] | xy[M][2]
+  std::memcpy(W.data(), body, (size_t)n * 4);
+  std::memcpy(W.data() + M, xy, (size_t)n * 8);
+  const bool from_gc = b->model->md.floating;
+  bool off_root = false;
+  for (int i = 0; i < n; i++) off_root = off_root || !(body[i] == 0 && from_gc);
+  CK(cudaSetDevice(b->device));
+  CK(b->scan_tab.ensure(W.size() * 4, b->stream));   // sized for RSB_MAX_SCAN_POINTS: the layout never moves
+  CK(cudaMemcpyAsync(b->scan_tab.get(), W.data(), W.size() * 4, cudaMemcpyHostToDevice, b->stream));
+  CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
+  const int* T = b->scan_tab.get();
+  b->scan = ScanTable{n, align, from_gc ? 1 : 0, T, (const float*)(T + M)};
+  b->scan_off_root = off_root;
+  return RSB_OK;
+}
+int rsb_batch_get_height_scan(rsb_batch* b, int env_begin, int env_count, float* height, float* xy_out, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (b->scan.n == 0) return fail(RSB_ERR_INVALID, "no height-scan points: call rsb_batch_set_height_scan() first");
+  if (b->ter.type != 1 && b->ter.type != 2) return fail(RSB_ERR_INVALID, "height scan: no terrain (set a ground or a height map first)");
+  if (env_count == 0 || !(height || xy_out)) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  // poses off a floating root come from the kinematics pass; after integrate2() its buffers hold the state before the step
+  if (b->scan_off_root) { rc = b->kin_prestep ? rsb_batch_update_kinematics(b) : ensure_kinematics(b); if (rc) return rc; }
+  const size_t rows = (size_t)env_count * b->scan.n;
+  float *dh = height, *dxy = xy_out;
+  if (where == RSB_HOST) {
+    float* s = staging(b, (height ? rows : 0) + (xy_out ? 2 * rows : 0)); if (!s) return RSB_ERR_CUDA;
+    if (height) { dh = s; s += rows; }
+    if (xy_out) dxy = s;
+  }
+  const int threads = 256;
+  const unsigned blocks = (unsigned)((rows + threads - 1) / threads);
+  rsb_height_scan_kernel<<<blocks, threads, 0, b->stream>>>(b->scan, b->ter, b->gc.get(), b->gc_stride, b->dbg_R.get(), b->dbg_p.get(), b->nb, env_begin, env_count, dh, dxy);
+  CK(cudaGetLastError());
+  b->launches++;
+  if (where != RSB_HOST) return RSB_OK;
+  if (height) { rc = copy_out(b, height, dh, rows * 4, RSB_HOST); if (rc) return rc; }
+  return xy_out ? copy_out(b, xy_out, dxy, rows * 2 * 4, RSB_HOST) : RSB_OK;
 }
 int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;

@@ -111,6 +111,16 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void body_contact_forces(uintptr_t force_dev, uintptr_t steps_dev) {
     check(rsb_batch_get_body_contact_forces(b_, 0, view_.num_envs, reinterpret_cast<float*>(force_dev), reinterpret_cast<int32_t*>(steps_dev), RSB_DEVICE), "body_contact_forces");
   }
+  // terrain height-scan points shared by all environments: body [P], xy [P*2] horizontal offsets, align "yaw" or "world" (empty clears)
+  void set_height_scan(const std::vector<int32_t>& body, const std::vector<float>& xy, const std::string& align) {
+    if (xy.size() != 2 * body.size()) throw std::runtime_error("set_height_scan: need 2 offset entries per point");
+    if (align != "yaw" && align != "world") throw std::runtime_error("set_height_scan: align must be 'yaw' or 'world'");
+    check(rsb_batch_set_height_scan(b_, body.data(), xy.data(), (int)body.size(), align == "yaw" ? RSB_SCAN_YAW : RSB_SCAN_WORLD), "set_height_scan");
+  }
+  // the scan of every environment into tensor addresses ([num_envs, P] and [num_envs, P, 2] float32, contiguous); 0 skips an output
+  void height_scan(uintptr_t height_dev, uintptr_t xy_dev) {
+    check(rsb_batch_get_height_scan(b_, 0, view_.num_envs, reinterpret_cast<float*>(height_dev), reinterpret_cast<float*>(xy_dev), RSB_DEVICE), "height_scan");
+  }
   // per-environment inertial rows [env_count, nb, 10] float32 (mass, com, inertia xx xy xz yy yz zz) from a device address
   void set_body_inertia(uintptr_t rows_dev, int env_begin, int env_count) {
     check(rsb_batch_set_body_inertia(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_body_inertia");
@@ -159,6 +169,8 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("frame_jacobians", &Batch::frame_jacobians, py::arg("jac_dev"))
       .def("set_contact_bodies", &Batch::set_contact_bodies, py::arg("body"))
       .def("body_contact_forces", &Batch::body_contact_forces, py::arg("force_dev"), py::arg("steps_dev"))
+      .def("set_height_scan", &Batch::set_height_scan, py::arg("body"), py::arg("xy"), py::arg("align") = std::string("yaw"))
+      .def("height_scan", &Batch::height_scan, py::arg("height_dev"), py::arg("xy_dev"))
       .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_contact_friction", &Batch::set_contact_friction, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_actuator_params", &Batch::set_actuator_params, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
