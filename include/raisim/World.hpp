@@ -18,6 +18,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <functional>
 #include <map>
 #include <memory>
@@ -114,6 +115,21 @@ struct LockStep {
   std::vector<float> scan, scanXy;          // [n][P], [n][P][2] heights and sample locations of the height scan (ArticulatedSystem::setHeightScan)
   int scanPoints = 0;
   bool scanValid = false;
+  // terrain of every environment (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding the same heights
+  // share one MapEntry; `atlas` is what the device holds, in atlas order (atlasSingle: one map set without an index)
+  struct MapEntry {
+    int xs = 0, ys = 0;
+    double xSize = 0, ySize = 0, cx = 0, cy = 0;
+    std::vector<float> h;
+    uint64_t hash = 0;
+    bool sameGeometry(const MapEntry& o) const { return xs == o.xs && ys == o.ys && xSize == o.xSize && ySize == o.ySize && cx == o.cx && cy == o.cy; }
+    bool sameMap(const MapEntry& o) const { return hash == o.hash && sameGeometry(o) && h == o.h; }
+  };
+  std::vector<std::shared_ptr<const MapEntry>> envMap, atlas;   // [n] map of every environment (null: none), maps on the device
+  std::vector<char> envGround;              // [n] the environment added a ground
+  std::vector<int32_t> atlasIndex;          // [n] map of every environment on the device (empty with atlasSingle)
+  bool atlasSingle = false, terrainDirty = false;
+  long mapUploads = 0, indexUploads = 0;    // terrain calls issued: maps uploaded (rsb_batch_set_heightmap / _heightmaps), index moves
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
   bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
@@ -124,6 +140,7 @@ struct LockStep {
     gc.assign(size_t(n) * nq, 0.f); gv.assign(size_t(n) * nv, 0.f); pt.assign(size_t(n) * nq, 0.f); vt.assign(size_t(n) * nv, 0.f);
     tau.assign(size_t(n) * nv, 0.f); tauApplied.assign(size_t(n) * nv, 0.f); contacts.resize(size_t(n) * RSB_KMAX); ncontacts.assign(n, 0);
     pending.assign(n, 0);
+    envMap.assign(n, nullptr); envGround.assign(n, 0);
   }
   // an environment is about to read or write the world: whatever it integrated before must have happened
   void sync(int env) {
@@ -174,6 +191,7 @@ struct LockStep {
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
     if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
     if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
+    pushTerrain();
     stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
@@ -188,7 +206,97 @@ struct LockStep {
     if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
     if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
     if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
+    pushTerrain();
     stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
+  }
+  // environment env's height map (World::addHeightMap), uploaded with the next flush() or pushWrites(): environments holding the same
+  // heights share one entry, found by a hash and confirmed by comparison
+  void setHeightMap(int env, int xs, int ys, double xSize, double ySize, double cx, double cy, std::vector<float> h) {
+    sync(env);
+    auto e = std::make_shared<MapEntry>();
+    e->xs = xs; e->ys = ys; e->xSize = xSize; e->ySize = ySize; e->cx = cx; e->cy = cy; e->h = std::move(h);
+    uint64_t x = 1469598103934665603ull;   // FNV-1a over the float32 words
+    for (float v : e->h) { uint32_t u; std::memcpy(&u, &v, 4); x = (x ^ u) * 1099511628211ull; }
+    e->hash = x;
+    std::shared_ptr<const MapEntry> found;
+    for (const auto& m : atlas) if (!found && m->sameMap(*e)) found = m;
+    for (const auto& m : envMap) if (!found && m && m->sameMap(*e)) found = m;
+    envMap[size_t(env)] = found ? found : e;
+    envGround[size_t(env)] = 0;
+    terrainDirty = true;
+  }
+  // environment env added a ground, which World::addGround sets on the batch at once (dropping any map there)
+  void setGround(int env) {
+    envMap[size_t(env)] = nullptr; envGround[size_t(env)] = 1;
+    atlas.clear(); atlasIndex.clear(); atlasSingle = false;
+    terrainDirty = true;
+  }
+  // the environments' maps onto the device, with the cheapest call that does it: nothing when the device already has them; one index
+  // move when every map in use is in the atlas (a curriculum moving environments among its levels); else one upload of the maps in use,
+  // a single map when every environment holds the same heights.  An environment that added no terrain of its own shares the map of the
+  // lowest-numbered environment that did (with one common map, the map every environment collided with before maps were per environment).
+  // A rebuilt atlas keeps maps of the previous one that no environment holds right now (a curriculum level nobody is on), up to twice
+  // as many maps as are in use, so that moving back to them needs no upload
+  void pushTerrain() {
+    if (!terrainDirty) return;
+    int firstMap = -1, firstGround = -1, firstNone = -1;
+    for (int e = 0; e < n; e++) {
+      int& first = envMap[size_t(e)] ? firstMap : envGround[size_t(e)] ? firstGround : firstNone;
+      if (first < 0) first = e;
+    }
+    if (firstMap < 0) { terrainDirty = false; return; }
+    if (firstGround >= 0)
+      throw std::runtime_error("VectorizedEnvironment: environment " + std::to_string(firstGround) + " added a ground and environment " + std::to_string(firstMap) +
+                               " a height map; every environment must use the same kind of terrain");
+    std::vector<std::shared_ptr<const MapEntry>> use(envMap);
+    for (auto& m : use) if (!m) m = envMap[size_t(firstMap)];
+    const MapEntry& g = *use[size_t(firstMap)];
+    for (int e = 0; e < n; e++)
+      if (!use[size_t(e)]->sameGeometry(g))
+        throw std::runtime_error("VectorizedEnvironment: the height maps of environments " + std::to_string(firstMap) + " and " + std::to_string(e) +
+                                 " differ in samples, size or centre; the maps of one batch must share them");
+    std::vector<int32_t> idx(size_t(n), -1);
+    bool inAtlas = true;
+    for (int e = 0; e < n && inAtlas; e++) {
+      for (size_t m = 0; m < atlas.size(); m++) if (atlas[m] == use[size_t(e)]) { idx[size_t(e)] = int32_t(m); break; }
+      inAtlas = idx[size_t(e)] >= 0;
+    }
+    if (inAtlas && !atlasSingle) {
+      int lo = 0, hi = n;
+      while (lo < n && idx[size_t(lo)] == atlasIndex[size_t(lo)]) lo++;
+      while (hi > lo && idx[size_t(hi - 1)] == atlasIndex[size_t(hi - 1)]) hi--;
+      if (hi > lo) {
+        rsbCheck(rsb_batch_set_heightmap_index(batch, idx.data() + lo, lo, hi - lo, RSB_HOST), "addHeightMap");
+        atlasIndex = idx;
+        indexUploads++;
+      }
+    } else if (!inAtlas) {
+      std::vector<std::shared_ptr<const MapEntry>> maps;   // the maps in use, in order of first appearance
+      for (int e = 0; e < n; e++) {
+        size_t m = 0;
+        while (m < maps.size() && maps[m] != use[size_t(e)]) m++;
+        if (m == maps.size()) maps.push_back(use[size_t(e)]);
+        idx[size_t(e)] = int32_t(m);
+      }
+      const size_t inUse = maps.size();
+      for (const auto& old : atlas)
+        if (maps.size() < 2 * inUse && old->sameGeometry(g) && std::find(maps.begin(), maps.end(), old) == maps.end()) maps.push_back(old);
+      atlas.clear(); atlasIndex.clear();
+      if (maps.size() == 1) {
+        rsbCheck(rsb_batch_set_heightmap(batch, g.xs, g.ys, float(g.xSize), float(g.ySize), float(g.cx), float(g.cy), g.h.data()), "addHeightMap");
+        atlasSingle = true;
+      } else {
+        std::vector<float> all;
+        all.reserve(maps.size() * g.h.size());
+        for (const auto& m : maps) all.insert(all.end(), m->h.begin(), m->h.end());
+        rsbCheck(rsb_batch_set_heightmaps(batch, int(maps.size()), g.xs, g.ys, float(g.xSize), float(g.ySize), float(g.cx), float(g.cy), all.data(), idx.data()), "addHeightMap");
+        atlasSingle = false; atlasIndex = idx;
+      }
+      atlas = std::move(maps);
+      mapUploads++;
+    }
+    terrainDirty = false;
+    scanValid = false;
   }
   // environment env's terrain friction of one collision body, uploaded with the next flush() or pushWrites() (no launch of its own)
   void setFriction(int env, size_t collisionBody, double mu) {
@@ -1040,7 +1148,7 @@ class World {
       rsb_params p = w_->params();
       p.dt = float(dt_); p.gravity[0] = float(g_[0]); p.gravity[1] = float(g_[1]); p.gravity[2] = float(g_[2]);
       w_->setParams(p);
-      if (haveGround_) rsbCheck(rsb_batch_set_ground(w_->batch(), float(groundZ_)), "addGround");
+      if (haveGround_) setGround();
       robot_.reset(new ArticulatedSystem(w_, env_));
       robot_->setJointOrder(jointOrder);
       return robot_.get();
@@ -1058,16 +1166,13 @@ class World {
   Ground* addGround(double zHeight = 0.0, const std::string& material = "default", CollisionGroup = CollisionGroup(-1)) {
     haveGround_ = true; groundZ_ = zHeight; terrainMaterial_ = material; ground_.setHeight(zHeight);
     if (robot_) applyMaterials(true);
-    if (w_) rsbCheck(rsb_batch_set_ground(w_->batch(), float(zHeight)), "addGround");
+    if (w_) setGround();
     return &ground_;
   }
   HeightMap* addHeightMap(size_t xSamples, size_t ySamples, double xSize, double ySize, double centerX, double centerY,
                           const std::vector<double>& height, const std::string& = "default", CollisionGroup = 1, CollisionGroup = CollisionGroup(-1)) {
     need();
-    std::vector<float> h(height.begin(), height.end());
-    rsbCheck(rsb_batch_set_heightmap(w_->batch(), int(xSamples), int(ySamples), float(xSize), float(ySize), float(centerX), float(centerY), h.data()), "addHeightMap");
-    hm_.set(xSamples, ySamples, xSize, ySize, centerX, centerY, std::vector<double>(h.begin(), h.end()));   // what the batch collides with (float32 heights)
-    return &hm_;
+    return useHeightMap(int(xSamples), int(ySamples), xSize, ySize, centerX, centerY, std::vector<float>(height.begin(), height.end()));
   }
   HeightMap* addHeightMap(double centerX, double centerY, const TerrainProperties& tp, const std::string& = "default", CollisionGroup = 1,
                           CollisionGroup = CollisionGroup(-1)) {
@@ -1076,9 +1181,7 @@ class World {
                              tp.fractalGain, tp.stepSize, tp.heightOffset, tp.seed};
     std::vector<float> h(tp.xSamples * tp.ySamples);
     rsbCheck(rsb_terrain_generate(&p, h.data()), "TerrainGenerator");
-    rsbCheck(rsb_batch_set_heightmap(w_->batch(), int(tp.xSamples), int(tp.ySamples), float(tp.xSize), float(tp.ySize), float(centerX), float(centerY), h.data()), "addHeightMap");
-    hm_.set(tp.xSamples, tp.ySamples, tp.xSize, tp.ySize, centerX, centerY, std::vector<double>(h.begin(), h.end()));
-    return &hm_;
+    return useHeightMap(int(tp.xSamples), int(tp.ySamples), tp.xSize, tp.ySize, centerX, centerY, std::move(h));
   }
   // height-map files (upstream overloads of the same name; [RECALL] formats, see include/rsb.h)
   HeightMap* addHeightMap(const std::string& raisimHeightMapFileName, double centerX, double centerY, const std::string& = "default",
@@ -1088,9 +1191,7 @@ class World {
     rsbCheck(rsb_heightmap_read_text(raisimHeightMapFileName.c_str(), &xs, &ys, &sx, &sy, nullptr, 0), "addHeightMap");
     std::vector<float> h(size_t(xs) * ys);
     rsbCheck(rsb_heightmap_read_text(raisimHeightMapFileName.c_str(), &xs, &ys, &sx, &sy, h.data(), int(h.size())), "addHeightMap");
-    rsbCheck(rsb_batch_set_heightmap(w_->batch(), xs, ys, float(sx), float(sy), float(centerX), float(centerY), h.data()), "addHeightMap");
-    hm_.set(size_t(xs), size_t(ys), sx, sy, centerX, centerY, std::vector<double>(h.begin(), h.end()));
-    return &hm_;
+    return useHeightMap(xs, ys, sx, sy, centerX, centerY, std::move(h));
   }
   HeightMap* addHeightMap(const std::string& pngFileName, double centerX, double centerY, double xSize, double ySize, double heightScale,
                           double heightOffset, const std::string& = "default", CollisionGroup = 1, CollisionGroup = CollisionGroup(-1)) {
@@ -1099,9 +1200,7 @@ class World {
     rsbCheck(rsb_heightmap_read_png(pngFileName.c_str(), heightScale, heightOffset, &xs, &ys, nullptr, 0), "addHeightMap");
     std::vector<float> h(size_t(xs) * ys);
     rsbCheck(rsb_heightmap_read_png(pngFileName.c_str(), heightScale, heightOffset, &xs, &ys, h.data(), int(h.size())), "addHeightMap");
-    rsbCheck(rsb_batch_set_heightmap(w_->batch(), xs, ys, float(xSize), float(ySize), float(centerX), float(centerY), h.data()), "addHeightMap");
-    hm_.set(size_t(xs), size_t(ys), xSize, ySize, centerX, centerY, std::vector<double>(h.begin(), h.end()));
-    return &hm_;
+    return useHeightMap(xs, ys, xSize, ySize, centerX, centerY, std::move(h));
   }
   void setTimeStep(double dt) { dt_ = dt; if (w_) { rsb_params p = w_->params(); p.dt = float(dt); w_->setParams(p); } }
   double getTimeStep() const { return dt_; }
@@ -1152,6 +1251,19 @@ class World {
   BatchedWorld* batched() { return w_; }
  private:
   void need() const { if (!w_) throw std::runtime_error("World: call addArticulatedSystem() first (the batch is created with the robot)"); }
+  // the terrain of this environment: in a VectorizedEnvironment its own map goes to the LockStep mirror, which uploads the maps of all
+  // environments before the next launch, getter or scan; a stand-alone World sets it at once.  hm_ holds the float32 heights the batch
+  // collides with, so HeightMap::getHeight answers for them
+  HeightMap* useHeightMap(int xs, int ys, double xSize, double ySize, double cx, double cy, std::vector<float> h) {
+    if (LockStep* ls = w_->lockStep()) ls->setHeightMap(env_, xs, ys, xSize, ySize, cx, cy, h);
+    else rsbCheck(rsb_batch_set_heightmap(w_->batch(), xs, ys, float(xSize), float(ySize), float(cx), float(cy), h.data()), "addHeightMap");
+    hm_.set(size_t(xs), size_t(ys), xSize, ySize, cx, cy, std::vector<double>(h.begin(), h.end()));
+    return &hm_;
+  }
+  void setGround() {
+    if (LockStep* ls = w_->lockStep()) ls->setGround(env_);
+    rsbCheck(rsb_batch_set_ground(w_->batch(), float(groundZ_)), "addGround");
+  }
   void applyMaterials(bool force) {
     if (!robot_ || (!force && !robot_->materialsDirty())) return;
     if (LockStep* ls = w_->lockStep()) {   // this environment's whole row: its pair friction, else its default friction (< 0: the batch's)

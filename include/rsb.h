@@ -152,6 +152,27 @@ int rsb_batch_clear_terrain(rsb_batch* b);
  * maps ([count][y_samples][x_samples], host) share one batch and map_of_env[num_envs] (host) picks one per environment */
 int rsb_batch_set_heightmaps(rsb_batch* b, int count, int x_samples, int y_samples, float x_size, float y_size,
                              float center_x, float center_y, const float* heights_host, const int32_t* map_of_env);
+/* Terrain curriculum (legged_gym-style: an environment moves to a harder or easier map when it resets): environments
+ * [env_begin, env_begin + env_count) collide with the maps map_of_env[env_count] (int32, host or device source, `where`) of the atlas
+ * set by rsb_batch_set_heightmaps, from the next launch on.  No map is uploaded.  The indices are copied into the batch's staging
+ * buffer (env_count words) and checked there on the device; the call waits for that check, then copies them into the atlas index in
+ * stream order: launches enqueued before the call see the old assignment, later ones the new.  env_count == 0 does nothing.
+ * The terrain enters neither M, h nor the poses: nothing goes stale and no step launch is added; the contact records and contact forces
+ * of the last step stay as they were, and height scans read the new assignment from the call on.  Gym resets keep the assignment;
+ * rsb_batch_set_heightmaps replaces it, rsb_batch_set_ground and rsb_batch_clear_terrain drop it.
+ * Refused with RSB_ERR_INVALID, changing nothing: a null batch or map_of_env, a bad range or `where`, an index outside [0, count), or
+ * no atlas (ground, no terrain, or the single map of rsb_batch_set_heightmap). */
+int rsb_batch_set_heightmap_index(rsb_batch* b, const int32_t* map_of_env, int env_begin, int env_count, int where);
+/* Maps first .. first + count - 1 of the terrain overwritten in place with heights [count][y_samples][x_samples] float32 (host or device
+ * source, `where`), the samples, size and centre staying those of the terrain; any height-map terrain, the single map of
+ * rsb_batch_set_heightmap being map 0.  Environments keep their map index.  The heights are copied into the batch's staging buffer,
+ * which grows to count * x_samples * y_samples words, and checked there on the device, which also finds the largest height of every new
+ * map; the call waits for that, then copies them over the maps in stream order (launches enqueued before the call see the old
+ * heights, later ones the new).  The stage-B cull height stays the exact maximum over all maps.  count == 0 does nothing.  Like
+ * rsb_batch_set_heightmap_index it adds no launch and makes nothing stale; height scans read the new heights from the call on.
+ * Refused with RSB_ERR_INVALID, changing nothing: a null batch or heights, a bad `where`, first or count out of range, a height that is
+ * not finite, or no height map. */
+int rsb_batch_update_heightmaps(rsb_batch* b, int first, int count, const float* heights, int where);
 int rsb_batch_set_params(rsb_batch* b, const rsb_params* p);
 int rsb_batch_get_params(const rsb_batch* b, rsb_params* p);
 int rsb_params_default(rsb_params* p);

@@ -95,7 +95,7 @@ EXPORTED = [
     "rsb_model_create_from_urdf", "rsb_model_destroy", "rsb_model_save", "rsb_model_load", "rsb_model_dims", "rsb_model_get_tables", "rsb_model_body_index",
     "rsb_model_body_name", "rsb_model_collision_index", "rsb_model_joint_name", "rsb_model_frame_index", "rsb_model_frame",
     "rsb_batch_create", "rsb_batch_destroy", "rsb_batch_set_stream", "rsb_batch_sync", "rsb_batch_num_envs",
-    "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
+    "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_set_heightmap_index", "rsb_batch_update_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
     "rsb_batch_set_collision_friction", "rsb_batch_set_self_collision",
     "rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_gains", "rsb_batch_set_pd_target",
     "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_actuator_params", "rsb_batch_clear_actuator_params", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
@@ -150,6 +150,9 @@ def lib():
         L.rsb_batch_set_heightmap.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p]
         L.rsb_batch_set_heightmaps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
         L.rsb_batch_clear_terrain.argtypes = [C.c_void_p]
+        if hasattr(L, "rsb_batch_set_heightmap_index"):    # absent from an older build loaded through RSB_LIB_PATH (tools/terrain_curriculum_probe.py)
+            L.rsb_batch_set_heightmap_index.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+            L.rsb_batch_update_heightmaps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
         L.rsb_batch_set_collision_friction.argtypes = [C.c_void_p, C.c_int, C.c_float]
         L.rsb_batch_set_self_collision.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.rsb_batch_set_params.argtypes = [C.c_void_p, C.POINTER(Params)]
@@ -300,6 +303,7 @@ class Batch:
         _ck(lib().rsb_batch_create(model.h, num_envs, device, C.byref(h)))
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
         self.device, self.nframes, self.ncontact_bodies, self.nscan = device, 0, 0, 0
+        self.hm_shape = None                 # (ys, xs) of the height map(s) set through this object
 
     def __del__(self):
         if getattr(self, "h", None) and lib is not None and _lib is not None:
@@ -333,6 +337,7 @@ class Batch:
         hh = np.ascontiguousarray(heights, dtype=np.float32).reshape(-1)
         assert hh.size == xs * ys
         _ck(lib().rsb_batch_set_heightmap(self.h, xs, ys, x_size, y_size, cx, cy, hh.ctypes.data_as(C.c_void_p)))
+        self.hm_shape = (ys, xs)
 
     def set_heightmaps(self, x_size, y_size, cx, cy, heights, map_of_env):
         """terrain atlas: heights [count, ys, xs] float32, map_of_env [n] int32 -> one height map per environment"""
@@ -341,6 +346,42 @@ class Batch:
         m = np.ascontiguousarray(map_of_env, np.int32)
         assert m.shape == (self.n,)
         _ck(lib().rsb_batch_set_heightmaps(self.h, count, xs, ys, x_size, y_size, cx, cy, h.ctypes.data_as(C.c_void_p), m.ctypes.data_as(C.c_void_p)))
+        self.hm_shape = (ys, xs)
+
+    def set_heightmap_index(self, map_of_env, env_begin=0, env_count=None):
+        """terrain curriculum: environments [env_begin, env_begin + n) collide with the atlas maps map_of_env [n] (numpy int32) from the
+        next launch on; no map is uploaded.  env_count defaults to len(map_of_env).  A refused call changes nothing."""
+        m = np.ascontiguousarray(map_of_env, np.int32).reshape(-1)
+        n = len(m) if env_count is None else env_count
+        if n > len(m):
+            raise ValueError(f"set_heightmap_index: {n} environments, {len(m)} indices")
+        _ck(lib().rsb_batch_set_heightmap_index(self.h, m.ctypes.data_as(C.c_void_p), env_begin, n, HOST))
+
+    def set_heightmap_index_from(self, map_of_env, env_begin=0):
+        """set_heightmap_index() from a contiguous int32 torch tensor [n] on the batch's device, checked there"""
+        n = map_of_env.shape[0] if hasattr(map_of_env, "shape") and len(map_of_env.shape) > 0 else -1
+        _ck(lib().rsb_batch_set_heightmap_index(self.h, self._device_out(map_of_env, (n,), "map_of_env", "int32"), env_begin, n, DEVICE))
+
+    def update_heightmaps(self, first, heights):
+        """overwrite maps first .. first + count - 1 of the terrain in place with heights [count, ys, xs] (numpy float32; [ys, xs]: one
+        map), the map shape being that of the terrain set by set_heightmap / set_heightmaps.  Every height must be finite; a refused
+        call changes nothing."""
+        if self.hm_shape is None:
+            raise ValueError("update_heightmaps: no height map set through this object")
+        h = np.ascontiguousarray(heights, np.float32)
+        if h.ndim == 2:
+            h = h[None]
+        if h.ndim != 3 or h.shape[1:] != self.hm_shape:
+            raise ValueError(f"update_heightmaps: need heights [count, {self.hm_shape[0]}, {self.hm_shape[1]}], got shape {h.shape}")
+        _ck(lib().rsb_batch_update_heightmaps(self.h, first, h.shape[0], h.ctypes.data_as(C.c_void_p), HOST))
+
+    def update_heightmaps_from(self, first, heights):
+        """update_heightmaps() from a contiguous float32 torch tensor [count, ys, xs] on the batch's device, checked there; the map
+        shape is that of the terrain set by set_heightmap / set_heightmaps"""
+        if self.hm_shape is None:
+            raise ValueError("update_heightmaps_from: no height map set through this object")
+        n = heights.shape[0] if hasattr(heights, "shape") and len(heights.shape) > 0 else -1
+        _ck(lib().rsb_batch_update_heightmaps(self.h, first, n, self._device_out(heights, (n,) + self.hm_shape, "heights"), DEVICE))
 
     def clear_terrain(self):
         _ck(lib().rsb_batch_clear_terrain(self.h))

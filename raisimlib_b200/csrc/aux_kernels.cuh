@@ -4,6 +4,7 @@
 // One warp per environment, coalesced row reads and writes; fixed-base models get [q | qdot].
 #pragma once
 #include <cuda_runtime.h>
+#include <climits>
 #include <stdint.h>
 #include "../../include/rsb.h"
 
@@ -85,6 +86,43 @@ __global__ void rsb_actuator_params_check_kernel(float* __restrict__ out, const 
     if (!ok) atomicMin(bad, r * 3 + f);
     if (f == 2 && v >= 0.f) v = fminf(v, 3.0e38f);
     o[(size_t)f * nv] = i < nbase ? -1.f : v;
+  }
+}
+
+// atlas map index of a range of environments (rsb_batch_set_heightmap_index, TerrainDesc::env_map): `n` indices of the caller copied as
+// they are (out may be src: the check runs in place on a host source's staged copy).  An index outside [0, count) lowers *bad to its
+// position; *bad is left alone when every index is accepted
+__global__ void rsb_heightmap_index_check_kernel(int* out, const int* src, int n, int count, int* bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int v = src[i];
+  out[i] = v;
+  if (v < 0 || v >= count) atomicMin(bad, i);
+}
+
+// ordered-integer image of a float: signed integer order is the float order (-0 just below +0), so atomicMax on it takes the largest
+// value whatever the order in which the threads arrive
+__device__ __forceinline__ int float_order_key(float v) {
+  const int i = __float_as_int(v);
+  return i >= 0 ? i : i ^ 0x7fffffff;
+}
+
+// height maps replacing maps of the atlas (rsb_batch_update_heightmaps): `count` maps of `words` heights each, copied as they are (out
+// may be src, as above); blockIdx.y strides over the maps, so any count runs on a grid of at most 65535 rows.  A value that is not finite
+// lowers *bad to its position in the caller's array; the largest value of map m goes to map_max[m] as float_order_key (the caller starts
+// it at INT_MIN).  One atomic per warp and map
+__global__ void __launch_bounds__(256) rsb_heightmap_check_kernel(float* out, const float* src, int words, int count, int* bad, int* map_max) {
+  for (int m = blockIdx.y; m < count; m += gridDim.y) {
+    const size_t base = (size_t)m * words;
+    int key = INT_MIN;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < words; i += gridDim.x * blockDim.x) {
+      const float v = src[base + i];
+      out[base + i] = v;
+      if (isfinite(v)) key = max(key, float_order_key(v));
+      else atomicMin(bad, (int)(base + i));
+    }
+    key = __reduce_max_sync(0xffffffffu, key);
+    if ((threadIdx.x & 31) == 0 && key != INT_MIN) atomicMax(map_max + m, key);
   }
 }
 

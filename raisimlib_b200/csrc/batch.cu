@@ -2,6 +2,8 @@
 // No CPU fallback: every compute entry point launches the sm_90a kernel or fails loudly.
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -103,6 +105,7 @@ struct rsb_batch {
   TerrainDesc ter{};
   DevBuf<float> hmap;
   DevBuf<int> hmap_index;            // terrain atlas: map index per environment
+  std::vector<float> hmap_max;       // [maps] largest height of every map while ter.type == 2; ter.hmax is the largest of them
   DevBuf<float> ext;                 // [N][EXT_WORDS] external wrench rows; ext_active: rows hold a wrench for the next launch
   bool ext_active = false;
   // state and solver outputs, allocated and zeroed by rsb_batch_create
@@ -506,14 +509,46 @@ static int check_range(const rsb_batch* b, int env_begin, int env_count, int whe
   return RSB_OK;
 }
 
+// The staging and verdict part of every call that checks the caller's values on the device before any of them is committed
+// (commit_env_rows, rsb_batch_set_heightmap_index, rsb_batch_update_heightmaps).  The caller's src_words (host or device memory, 4-byte
+// elements) are checked and packed to out_words in the staging buffer by check(out, src, verdict), and the call waits for the verdict.
+// A host source is copied into the staging buffer first: behind the checked words, or, with in_place (the check copies element i to
+// element i), onto them, so that the buffer grows to out_words only.  verdict[0] stays ROWS_OK when every value is accepted;
+// verdict[1 .. extra] start at INT_MIN for what the check gathers with atomicMax.  On success *staged holds the checked words, valid
+// until the next use of the staging buffer; a refused value fails the call with RSB_ERR_INVALID and what(verdict[0]).
+static constexpr int ROWS_OK = 0x7fffffff;
+template <class T, class Check, class What>
+static int stage_checked(rsb_batch* b, const T* src, size_t out_words, size_t src_words, int where, bool in_place, int extra, Check check,
+                         What what, T** staged, std::vector<int>* verdict = nullptr) {
+  static_assert(sizeof(T) == 4, "the staging buffer holds 4-byte words");
+  CK(b->row_bad.ensure((size_t)(1 + extra) * 4, b->stream));
+  const bool host = where == RSB_HOST;
+  float* const stf = staging(b, out_words + (host && !in_place ? src_words : 0)); if (!stf) return RSB_ERR_CUDA;
+  T* const st = reinterpret_cast<T*>(stf);
+  const T* dsrc = src;
+  if (host) {
+    T* const to = in_place ? st : st + out_words;
+    CK(cudaMemcpyAsync(to, src, src_words * 4, cudaMemcpyHostToDevice, b->stream));
+    dsrc = to;
+  }
+  std::vector<int> v(1 + extra, INT_MIN);
+  v[0] = ROWS_OK;
+  CK(cudaMemcpyAsync(b->row_bad.get(), v.data(), v.size() * 4, cudaMemcpyHostToDevice, b->stream));
+  if (src_words > 0) { check(st, dsrc, b->row_bad.get()); CK(cudaGetLastError()); }
+  CK(cudaMemcpyAsync(v.data(), b->row_bad.get(), v.size() * 4, cudaMemcpyDeviceToHost, b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  if (v[0] != ROWS_OK) return fail(RSB_ERR_INVALID, what(v[0]));
+  *staged = st;
+  if (verdict) *verdict = std::move(v);
+  return RSB_OK;
+}
+
 // The one path by which a call's per-environment rows reach an EnvRows table (rsb_batch_set_body_inertia, set_contact_friction,
 // set_actuator_params).
 // `dflt` is one environment's row of the table (w words) when nothing overrides it: every environment starts from it at the first commit
 // after creation or a clear, and rows == null writes it to the range.  Otherwise the caller's rows (src_w words per environment) are
-// checked and packed to w words by check(out, src, env_count, bad) in the staging buffer (a host source passes through it too), and the
-// call waits for the verdict: *bad stays ROWS_OK when every value is accepted; else nothing of the table changes and the call is
-// refused with what(verdict).
-static constexpr int ROWS_OK = 0x7fffffff;
+// checked and packed to w words by check(out, src, env_count, bad) through stage_checked; a refused row changes nothing of the table and
+// the call fails with what(verdict).
 static std::vector<float> repeat_row(const std::vector<float>& row, size_t n) {
   std::vector<float> r(n * row.size());
   for (size_t e = 0; e < n; e++) std::copy(row.begin(), row.end(), r.begin() + e * row.size());
@@ -526,25 +561,12 @@ static int commit_env_rows(rsb_batch* b, EnvRows& t, const std::vector<float>& d
   if (env_count == 0) return RSB_OK;
   CK(cudaSetDevice(b->device));
   const size_t w = dflt.size(), n = (size_t)env_count;
-  const float* staged = nullptr;
+  float* staged = nullptr;
   std::vector<float> reset;
   if (rows) {
-    CK(b->row_bad.ensure(4, b->stream));
-    // the checked rows [n][w], then a host source's rows [n][src_w]
-    float* const st = staging(b, n * w + (where == RSB_HOST ? n * src_w : 0)); if (!st) return RSB_ERR_CUDA;
-    const float* src = rows;
-    if (where == RSB_HOST) {
-      CK(cudaMemcpyAsync(st + n * w, rows, n * src_w * 4, cudaMemcpyHostToDevice, b->stream));
-      src = st + n * w;
-    }
-    const int ok = ROWS_OK;
-    CK(cudaMemcpyAsync(b->row_bad.get(), &ok, 4, cudaMemcpyHostToDevice, b->stream));
-    if (n * src_w > 0) { check(st, src, env_count, b->row_bad.get()); CK(cudaGetLastError()); }
-    int bad = ok;
-    CK(cudaMemcpyAsync(&bad, b->row_bad.get(), 4, cudaMemcpyDeviceToHost, b->stream));
-    CK(cudaStreamSynchronize(b->stream));
-    if (bad != ok) return fail(RSB_ERR_INVALID, what(bad) + "; no row changed");
-    staged = st;
+    rc = stage_checked(b, rows, n * w, n * src_w, where, false, 0, [&](float* out, const float* src, int* bad) { check(out, src, env_count, bad); },
+                       [&](int bad) { return what(bad) + "; no row changed"; }, &staged);
+    if (rc) return rc;
   } else {
     reset = repeat_row(dflt, n);
   }
@@ -743,8 +765,14 @@ static int upload_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_si
   t.x0 = cx - 0.5f * x_size; t.y0 = cy - 0.5f * y_size;
   t.xmax = (float)(xs - 1); t.ymax = (float)(ys - 1);
   t.h = b->hmap.get(); t.env_map = map_of_env ? b->hmap_index.get() : nullptr; t.map_words = xs * ys;
-  t.hmax = h[0];
-  for (size_t i = 1; i < words; i++) t.hmax = std::max(t.hmax, h[i]);
+  b->hmap_max.assign(count, 0.f);
+  for (int m = 0; m < count; m++) {
+    const float* hm = h + (size_t)m * t.map_words;
+    float mx = hm[0];
+    for (int i = 1; i < t.map_words; i++) mx = std::max(mx, hm[i]);
+    b->hmap_max[m] = mx;
+  }
+  t.hmax = *std::max_element(b->hmap_max.begin(), b->hmap_max.end());
   b->ter = t;
   return RSB_OK;
 }
@@ -760,6 +788,63 @@ int rsb_batch_set_heightmaps(rsb_batch* b, int count, int xs, int ys, float x_si
   if ((size_t)count * xs * ys > ((size_t)1 << 30)) return fail(RSB_ERR_INVALID, "height-map atlas too large");
   for (int e = 0; e < b->N; e++) if (map_of_env[e] < 0 || map_of_env[e] >= count) return fail(RSB_ERR_INVALID, "height-map index out of range");
   return upload_heightmaps(b, count, xs, ys, x_size, y_size, cx, cy, h, map_of_env);
+}
+// terrain curriculum: environments [env_begin, env_begin + env_count) move to other maps of the atlas.  The indices are checked in the
+// staging buffer, then copied into the index in stream order: launches enqueued before see the old assignment, later ones the new
+int rsb_batch_set_heightmap_index(rsb_batch* b, const int32_t* map_of_env, int env_begin, int env_count, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (!map_of_env) return fail(RSB_ERR_INVALID, "height-map index: null index list");
+  if (b->ter.type != 2 || !b->ter.env_map) return fail(RSB_ERR_INVALID, "height-map index: no terrain atlas (set one with rsb_batch_set_heightmaps() first)");
+  if (env_count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const int count = (int)b->hmap_max.size();
+  int* staged = nullptr;
+  auto check = [&](int* out, const int* src, int* bad) {
+    const int threads = 256;
+    rsb_heightmap_index_check_kernel<<<(unsigned)((env_count + threads - 1) / threads), threads, 0, b->stream>>>(out, src, env_count, count, bad);
+  };
+  auto what = [&](int bad) {
+    return "height-map index: environment " + std::to_string(env_begin + bad) + " names a map outside [0, " + std::to_string(count) + "); nothing changed";
+  };
+  rc = stage_checked(b, map_of_env, (size_t)env_count, (size_t)env_count, where, true, 0, check, what, &staged); if (rc) return rc;
+  CK(cudaMemcpyAsync(b->hmap_index.get() + env_begin, staged, (size_t)env_count * 4, cudaMemcpyDeviceToDevice, b->stream));
+  return RSB_OK;
+}
+// maps first .. first + count - 1 of the terrain overwritten in place.  The heights are checked, and the largest height of every new map
+// found, in the staging buffer before any map changes; the map pointer stays where it is, and the copy follows earlier launches in
+// stream order
+int rsb_batch_update_heightmaps(rsb_batch* b, int first, int count, const float* heights, int where) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (bad_where(where)) return fail(RSB_ERR_INVALID, "`where` must be RSB_HOST or RSB_DEVICE");
+  if (!heights) return fail(RSB_ERR_INVALID, "update height maps: null heights");
+  if (b->ter.type != 2) return fail(RSB_ERR_INVALID, "update height maps: no height map (set one with rsb_batch_set_heightmap() or rsb_batch_set_heightmaps() first)");
+  const int maps = (int)b->hmap_max.size();
+  if (first < 0 || count < 0 || first > maps - count)
+    return fail(RSB_ERR_INVALID, "update height maps: maps [" + std::to_string(first) + ", " + std::to_string(first) + " + " + std::to_string(count) + ") are not all in the terrain's " + std::to_string(maps));
+  if (count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const int words = b->ter.map_words;
+  float* staged = nullptr;
+  std::vector<int> verdict;
+  auto check = [&](float* out, const float* src, int* v) {
+    const int threads = 256, blocks = std::min((words + threads - 1) / threads, 256);
+    rsb_heightmap_check_kernel<<<dim3((unsigned)blocks, (unsigned)std::min(count, 65535)), threads, 0, b->stream>>>(out, src, words, count, v, v + 1);
+  };
+  auto what = [&](int bad) {
+    const int m = bad / words, i = bad % words;
+    return "update height maps: map " + std::to_string(first + m) + ", sample (" + std::to_string(i % b->ter.xs) + ", " + std::to_string(i / b->ter.xs) + ") is not finite; nothing changed";
+  };
+  const size_t all = (size_t)count * words;
+  int rc = stage_checked(b, heights, all, all, where, true, count, check, what, &staged, &verdict); if (rc) return rc;
+  CK(cudaMemcpyAsync(b->hmap.get() + (size_t)first * words, staged, all * 4, cudaMemcpyDeviceToDevice, b->stream));
+  for (int m = 0; m < count; m++) {   // every value is finite, so each map has a largest one: back from its ordered-integer image
+    const int k = verdict[1 + m], bits = k >= 0 ? k : k ^ 0x7fffffff;
+    float mx;
+    std::memcpy(&mx, &bits, 4);
+    b->hmap_max[first + m] = mx;
+  }
+  b->ter.hmax = *std::max_element(b->hmap_max.begin(), b->hmap_max.end());
+  return RSB_OK;
 }
 int rsb_batch_set_params(rsb_batch* b, const rsb_params* p) {
   if (!b || !p) return fail(RSB_ERR_INVALID, "null argument");
@@ -1475,6 +1560,13 @@ int rsb_internal_launch_config(const rsb_batch* b, int* wpc, int* grid) {
 int rsb_internal_launch_instance(const rsb_batch* b, int* spec, int* slots) {
   if (!b || !spec || !slots) return fail(RSB_ERR_INVALID, "null argument");
   *spec = b->cfg.spec; *slots = b->cfg.slots;
+  return RSB_OK;
+}
+// the stage-B cull height of a height-map terrain (TerrainDesc::hmax) the next launch uses (tests: it must stay the exact maximum over all maps)
+int rsb_internal_terrain_hmax(const rsb_batch* b, float* hmax) {
+  if (!b || !hmax) return fail(RSB_ERR_INVALID, "null argument");
+  if (b->ter.type != 2) return fail(RSB_ERR_INVALID, "no height map");
+  *hmax = b->ter.hmax;
   return RSB_OK;
 }
 void rsb_internal_set_error(const char* msg) { g_err = msg ? msg : ""; }

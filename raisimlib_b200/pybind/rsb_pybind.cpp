@@ -133,6 +133,21 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void set_actuator_params(uintptr_t rows_dev, int env_begin, int env_count) {
     check(rsb_batch_set_actuator_params(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_actuator_params");
   }
+  // terrain atlas: heights [count * ys * xs] and the map of every environment [num_envs], host lists
+  void set_heightmaps(int count, int xs, int ys, float x_size, float y_size, float cx, float cy, const std::vector<float>& heights,
+                      const std::vector<int32_t>& map_of_env) {
+    if ((int64_t)heights.size() != (int64_t)count * xs * ys || (int)map_of_env.size() != view_.num_envs)
+      throw std::runtime_error("set_heightmaps: need count * ys * xs heights and one map index per environment");
+    check(rsb_batch_set_heightmaps(b_, count, xs, ys, x_size, y_size, cx, cy, heights.data(), map_of_env.data()), "set_heightmaps");
+  }
+  // terrain curriculum: atlas map index of environments [env_begin, env_begin + env_count) ([env_count] int32) from a device address
+  void set_heightmap_index(uintptr_t map_of_env_dev, int env_begin, int env_count) {
+    check(rsb_batch_set_heightmap_index(b_, reinterpret_cast<const int32_t*>(map_of_env_dev), env_begin, env_count, RSB_DEVICE), "set_heightmap_index");
+  }
+  // maps first .. first + count - 1 of the terrain overwritten with [count, ys, xs] float32 heights from a device address
+  void update_heightmaps(uintptr_t heights_dev, int first, int count) {
+    check(rsb_batch_update_heightmaps(b_, first, count, reinterpret_cast<const float*>(heights_dev), RSB_DEVICE), "update_heightmaps");
+  }
   int num_envs() const { return view_.num_envs; }
   int nq() const { return view_.nq; }
   int nv() const { return view_.nv; }
@@ -174,6 +189,10 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_contact_friction", &Batch::set_contact_friction, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_actuator_params", &Batch::set_actuator_params, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
+      .def("set_heightmaps", &Batch::set_heightmaps, py::arg("count"), py::arg("xs"), py::arg("ys"), py::arg("x_size"), py::arg("y_size"),
+           py::arg("cx"), py::arg("cy"), py::arg("heights"), py::arg("map_of_env"))
+      .def("set_heightmap_index", &Batch::set_heightmap_index, py::arg("map_of_env_dev"), py::arg("env_begin"), py::arg("env_count"))
+      .def("update_heightmaps", &Batch::update_heightmaps, py::arg("heights_dev"), py::arg("first"), py::arg("count"))
       .def("sync", &Batch::sync)
       .def_property_readonly("num_envs", &Batch::num_envs)
       .def_property_readonly("nq", &Batch::nq)
