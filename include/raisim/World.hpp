@@ -113,6 +113,9 @@ struct LockStep {
   std::vector<float> actuator;              // [n][nv][3] kp, kd, effort limit (setPdGains / setActuationLimits; -1: the batch's); empty until the first one
   bool actuatorDirty = false;
   std::vector<float> scan, scanXy;          // [n][P], [n][P][2] heights and sample locations of the height scan (ArticulatedSystem::setHeightScan)
+  size_t actHistWords = 0;                  // words of one environment's actuator-network history (0: no network, or history 1)
+  std::vector<char> actHistReset;           // [n] ArticulatedSystem::resetActuatorHistory() since the last upload
+  bool actHistDirty = false;
   int scanPoints = 0;
   bool scanValid = false;
   // terrain of every environment (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding the same heights
@@ -192,6 +195,7 @@ struct LockStep {
     if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
     if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
     pushTerrain();
+    pushActuatorHistory();
     stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
@@ -207,7 +211,28 @@ struct LockStep {
     if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
     if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
     pushTerrain();
+    pushActuatorHistory();
     stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
+  }
+  // environment env's actuator-network history goes to zero before the next launch (ArticulatedSystem::resetActuatorHistory)
+  void resetActuatorHistory(int env) {
+    sync(env);
+    if (actHistReset.empty()) actHistReset.assign(n, 0);
+    actHistReset[env] = 1;
+    actHistDirty = true;
+  }
+  // the marked environments' history rows zeroed: one get and one set of all rows, only when some environment reset
+  void pushActuatorHistory() {
+    if (!actHistDirty) return;
+    actHistDirty = false;
+    if (actHistWords > 0) {
+      std::vector<float> h(size_t(n) * actHistWords);
+      rsbCheck(rsb_batch_get_actuator_history(batch, h.data(), 0, n, RSB_HOST), "resetActuatorHistory");
+      for (int e = 0; e < n; e++)
+        if (actHistReset[e]) std::fill(h.begin() + size_t(e) * actHistWords, h.begin() + size_t(e + 1) * actHistWords, 0.f);
+      rsbCheck(rsb_batch_set_actuator_history(batch, h.data(), 0, n, RSB_HOST), "resetActuatorHistory");
+    }
+    std::fill(actHistReset.begin(), actHistReset.end(), 0);
   }
   // environment env's height map (World::addHeightMap), uploaded with the next flush() or pushWrites(): environments holding the same
   // heights share one entry, found by a hash and confirmed by comparison
@@ -370,6 +395,25 @@ class BatchedWorld {
     if (ls_) { ls_->scanPoints = int(bodies.size()); ls_->scanValid = false; }
   }
   size_t numHeightScanPoints() const { return scanBodies_.size(); }
+  // the learned actuator network (ArticulatedSystem::setActuatorNetwork): one for the batch.  Setting it zeroes every history, so a
+  // repeat of the network already set (every environment of a VectorizedEnvironment sets it in its constructor) is not passed on
+  void setActuatorNetwork(const std::vector<int32_t>& dofs, int history, int layers, int width, const std::vector<float>& params) {
+    if (dofs == anDofs_ && history == anH_ && layers == anL_ && width == anW_ && params == anParams_) return;
+    if (!dofs.empty()) {
+      const size_t count = size_t(2 * history) * width + width + size_t(layers - 1) * (size_t(width) * width + width) + width + 1;
+      if (history < 1 || layers < 1 || width < 1 || params.size() != count)
+        throw std::runtime_error("setActuatorNetwork: " + std::to_string(params.size()) + " parameters for history " + std::to_string(history) +
+                                 ", " + std::to_string(layers) + " layers of width " + std::to_string(width));
+    }
+    rsbCheck(rsb_batch_set_actuator_network(batch_, dofs.data(), int(dofs.size()), history, layers, width, params.data()), "setActuatorNetwork");
+    anDofs_ = dofs; anH_ = history; anL_ = layers; anW_ = width; anParams_ = params;
+    if (ls_) { ls_->actHistWords = dofs.empty() ? 0 : dofs.size() * 2 * size_t(history - 1); ls_->actHistDirty = false; ls_->actHistReset.clear(); }
+  }
+  // zero environment env's actuator history: at once in a stand-alone World, before the next launch in a VectorizedEnvironment
+  void resetActuatorHistory(int env) {
+    if (ls_) { ls_->resetActuatorHistory(env); return; }
+    if (!anDofs_.empty()) rsbCheck(rsb_batch_set_actuator_history(batch_, nullptr, env, 1, RSB_HOST), "resetActuatorHistory");
+  }
   const std::string& urdf() const { return urdf_; }
   void rememberUrdf(const std::string& u) { urdf_ = u; }
  private:
@@ -377,6 +421,9 @@ class BatchedWorld {
   std::vector<size_t> contactBodies_;
   std::vector<int32_t> scanBodies_;
   std::vector<float> scanXy_;
+  std::vector<int32_t> anDofs_;
+  int anH_ = 0, anL_ = 0, anW_ = 0;
+  std::vector<float> anParams_;
   bool scanYaw_ = true;
   std::string urdf_;
   rsb_model* model_ = nullptr;
@@ -987,6 +1034,14 @@ class ArticulatedSystem {
     for (size_t i = 0; i < offsets.size(); i++) { xy[2 * i] = float(offsets[i][0]); xy[2 * i + 1] = float(offsets[i][1]); }
     w_->setHeightScan(b, xy, yawAligned);
   }
+  // setActuatorNetwork: the learned actuator network of rsb_batch_set_actuator_network (include/rsb.h) for the dofs listed (generalized
+  // velocity indices of joints), with params in torch.nn.Linear order.  The network belongs to the batch: every environment shares it,
+  // and each environment of a VectorizedEnvironment may set the same one in its constructor.  Setting it zeroes every history.
+  void setActuatorNetwork(const std::vector<size_t>& dofs, int history, int layers, int width, const std::vector<float>& params) {
+    w_->setActuatorNetwork(std::vector<int32_t>(dofs.begin(), dofs.end()), history, layers, width, params);
+  }
+  // zero this environment's actuator-network history (setState keeps it): call it in reset()
+  void resetActuatorHistory() { w_->resetActuatorHistory(env_); }
   // the world z of the collision surface under every point at the current state, in setHeightScan order, and (samples, optional) the
   // world (x, y) each was taken at.  In a VectorizedEnvironment one call scans every environment for the control step; a stand-alone
   // World scans this environment

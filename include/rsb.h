@@ -262,6 +262,38 @@ int rsb_batch_clear_body_inertia(rsb_batch* b);
 int rsb_batch_set_actuator_params(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
 /* drop all per-environment actuator rows: every later launch runs as if none had been set */
 int rsb_batch_clear_actuator_params(rsb_batch* b);
+/* Learned actuator network (Hwangbo et al., Science Robotics 2019): the torque of each listed dof is an MLP of its own recent
+ * position errors and velocities, evaluated by the step kernel at every sub-step from that sub-step's state.
+ *   One network per batch, shared by dofs[n_dofs] (batch gv order; a floating robot's six base dofs are refused).
+ *   Input: 2H features [e_t, e_{t-1}, ..., e_{t-H+1}, v_t, v_{t-1}, ..., v_{t-H+1}] with e = ptarget[q(d)] - gc[q(d)] (the float32
+ *   subtraction of the PD law) and v = gv[d], the current ones taken at the start of the sub-step.  L hidden layers of width W, each
+ *   affine then softsign x / (1 + |x|), then one linear output.  params are packed in torch.nn.Linear order: W1[W][2H], b1[W], ...,
+ *   WL[W][W], bL[W], Wout[1][W], bout[1] (2HW + W + (L - 1)(W^2 + W) + W + 1 floats, host memory).  There are no scaling parameters:
+ *   input normalisation and output scale fold exactly into the first and last layers (INTEGRATION.md).
+ *   History: per environment and listed dof, (e, v) of the last H - 1 sub-steps.  Every launch that advances the state (integrate,
+ *   integrate2, control_step, gym_step) shifts it once per sub-step, so 4 launches of 1 sub-step equal 1 launch of 4 sub-steps bit for
+ *   bit; integrate1, the kinematics pass, the getters and the height scan neither evaluate the network nor shift the history.  The
+ *   network and its history act in RSB_PD_PLUS_FEEDFORWARD_TORQUE mode only: in RSB_FORCE_AND_TORQUE mode the listed dofs get their
+ *   feed-forward torque as every dof does and the history stays as it is.
+ *   Torque: for a listed dof the network replaces the PD law (kp, kd and the velocity target of that dof are ignored).  The commanded
+ *   torque tau_ff + net is explicit, constant over the sub-step (nothing is folded into the mass matrix), saturated at the dof's effort
+ *   limit (URDF or rsb_batch_set_actuator_params row) and reported by rsb_batch_get_generalized_force as applied.  Unlisted dofs are
+ *   unchanged.  A set network counts as PD gains for rsb_batch_gym_step.
+ *   Resets: every rsb_batch_set_actuator_network call and rsb_batch_gym_reset zero all histories; a termination in rsb_batch_gym_step
+ *   zeroes that environment's history.  rsb_batch_set_state does not touch it (set it with rsb_batch_set_actuator_history).
+ *   n_dofs = 0 clears the network (the other arguments are then not read).  Refused with RSB_ERR_INVALID, changing nothing (the old
+ *   network and history stay): a null batch, n_dofs outside [0, nv], a NULL, out-of-range, duplicated or base dof, history, layers or
+ *   width out of range, NULL params with n_dofs > 0, a parameter that is not finite. */
+#define RSB_ACTNET_MAX_HISTORY 4
+#define RSB_ACTNET_MAX_LAYERS 4
+#define RSB_ACTNET_MAX_WIDTH 32
+int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs, int history, int layers, int width, const float* params);
+/* History rows [env_count][n_dofs][2][H - 1] float32 (errors then velocities, most recent first), host or device (`where`).  rows ==
+ * NULL zeroes the range.  The rows are checked on the device in the batch's staging buffer before any of them is committed; the call
+ * waits for that check.  With H = 1 the rows have no words and both calls succeed without doing anything.  Refused with
+ * RSB_ERR_INVALID, changing nothing: a null batch, no network, a bad range or `where`, a value that is not finite. */
+int rsb_batch_set_actuator_history(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
+int rsb_batch_get_actuator_history(rsb_batch* b, float* rows, int env_begin, int env_count, int where);
 /* ArticulatedSystem::getGeneralizedForce(): feed-forward + PD force applied over the last integrate() */
 int rsb_batch_get_generalized_force(rsb_batch* b, float* tau, int env_begin, int env_count, int where);
 
@@ -278,6 +310,7 @@ int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int 
 int rsb_batch_get_contact_points(rsb_batch* b, int32_t* pt_index, int env_begin, int env_count, int where);          /* [n][RSB_KMAX] candidate-point ids */
 int rsb_batch_get_solver_iterations(rsb_batch* b, int32_t* iters, int env_begin, int env_count, int where);          /* getContactSolver().getLoopCounter() */
 int rsb_batch_get_diverged(rsb_batch* b, int32_t* flags, int env_begin, int env_count, int where);                   /* 1 = state went non-finite in the last step: reset it */
+/* a diverged environment with an actuator network also carries NaN in its actuator history until that is set (rsb_batch_set_actuator_history) */
 /* how the last contact solve of every environment ended */
 #define RSB_SOLVER_CONVERGED 0           /* largest impulse update < threshold                                         */
 #define RSB_SOLVER_CONVERGED_COMPLIANT 1 /* ... on the compliant contact set entered after a failed stagnation check   */
@@ -425,8 +458,8 @@ int rsb_batch_gym_configure(rsb_batch* b, const float* gc_init, const float* gv_
                             const int32_t* foot_bodies, int n_foot, float torque_coeff, float forward_vel_coeff, float terminal_reward);
 int rsb_batch_gym_reset(rsb_batch* b);                                             /* VectorizedEnvironment::reset() */
 /* ::step() + ::observe() in ONE launch of the step kernel: action rows -> PD targets, `substeps` x World::integrate(), reward,
- * isTerminalState(), reset() of the terminated environments, observation rows of the resulting state.  Needs rsb_batch_set_pd_gains()
- * or active per-environment actuator rows (rsb_batch_set_actuator_params). */
+ * isTerminalState(), reset() of the terminated environments, observation rows of the resulting state.  Needs rsb_batch_set_pd_gains(),
+ * active per-environment actuator rows (rsb_batch_set_actuator_params) or an actuator network (rsb_batch_set_actuator_network). */
 int rsb_batch_gym_step(rsb_batch* b, const float* action, int where_in, int substeps, float* obs, float* reward, unsigned char* done,
                        int where_out);
 

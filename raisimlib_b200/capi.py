@@ -98,7 +98,7 @@ EXPORTED = [
     "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_set_heightmap_index", "rsb_batch_update_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
     "rsb_batch_set_collision_friction", "rsb_batch_set_self_collision",
     "rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_gains", "rsb_batch_set_pd_target",
-    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_actuator_params", "rsb_batch_clear_actuator_params", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
+    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_actuator_params", "rsb_batch_clear_actuator_params", "rsb_batch_set_actuator_network", "rsb_batch_set_actuator_history", "rsb_batch_get_actuator_history", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
     "rsb_batch_integrate1", "rsb_batch_integrate2", "rsb_batch_integrate",
     "rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities", "rsb_batch_get_body_poses", "rsb_batch_get_contacts",
     "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
@@ -194,6 +194,10 @@ def lib():
         if hasattr(L, "rsb_batch_set_actuator_params"):    # absent from an older build loaded through RSB_LIB_PATH (tools/actuator_params_probe.py)
             L.rsb_batch_set_actuator_params.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
             L.rsb_batch_clear_actuator_params.argtypes = [C.c_void_p]
+        if hasattr(L, "rsb_batch_set_actuator_network"):   # absent from an older build loaded through RSB_LIB_PATH (tools/actuator_network_probe.py)
+            L.rsb_batch_set_actuator_network.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+            L.rsb_batch_set_actuator_history.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+            L.rsb_batch_get_actuator_history.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
         if hasattr(L, "rsb_batch_set_height_scan"):        # absent from an older build loaded through RSB_LIB_PATH (tools/height_scan_probe.py)
             L.rsb_batch_set_height_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
             L.rsb_batch_get_height_scan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
@@ -238,6 +242,28 @@ def _ptr(a):
         assert a.is_contiguous()
         return C.c_void_p(a.data_ptr()), (DEVICE if a.is_cuda else HOST)
     raise TypeError(type(a))
+
+
+def _network_layers(layers):
+    """[(W, b)] float32 numpy pairs of an actuator network given as such pairs or as a torch.nn.Sequential of Linear and Softsign"""
+    if hasattr(layers, "named_children") and hasattr(layers, "__iter__"):
+        mods = list(layers)
+        kinds = [type(m).__name__ for m in mods]
+        ok = len(mods) % 2 == 1 and all(k == ("Linear" if i % 2 == 0 else "Softsign") for i, k in enumerate(kinds))
+        if not ok:
+            raise ValueError(f"actuator network: a Sequential must be Linear, Softsign, ..., Linear; got {kinds}")
+        pairs = []
+        for m in mods[::2]:
+            if m.bias is None:
+                raise ValueError("actuator network: every Linear needs a bias")
+            pairs.append((m.weight.detach().cpu().numpy(), m.bias.detach().cpu().numpy()))
+        layers = pairs
+    out = []
+    for p in layers:
+        if len(p) != 2:
+            raise ValueError("actuator network: layers must be (W, b) pairs")
+        out.append((np.asarray(p[0], np.float32), np.asarray(p[1], np.float32)))
+    return out
 
 
 class Model:
@@ -304,6 +330,7 @@ class Batch:
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
         self.device, self.nframes, self.ncontact_bodies, self.nscan = device, 0, 0, 0
         self.hm_shape = None                 # (ys, xs) of the height map(s) set through this object
+        self.an_shape = None                 # (listed dofs, history) of the actuator network set through this object
 
     def __del__(self):
         if getattr(self, "h", None) and lib is not None and _lib is not None:
@@ -735,6 +762,72 @@ class Batch:
     def clear_actuator_params(self):
         """drop every per-environment actuator row: later steps run as if none had been set"""
         _ck(lib().rsb_batch_clear_actuator_params(self.h))
+
+    # learned actuator network
+    def set_actuator_network(self, dofs_or_joint_names, layers, history):
+        """One network for the batch, evaluated by the step kernel at every sub-step for each listed dof (gv indices, or joint names)
+        from its last `history` position errors (ptarget - q) and velocities, in place of the PD law of those dofs.  layers: a list of
+        (W, b) numpy pairs, torch.nn.Linear order (W [width, 2 * history], b [width], ..., W [1, width], b [1]), or a torch.nn.Sequential
+        of Linear and Softsign only (Linear, Softsign, ..., Linear).  Input features: [e_t .. e_{t-H+1}, v_t .. v_{t-H+1}].  An empty
+        dof list clears the network.  Every call zeroes all histories; a refused call changes nothing."""
+        names = list(dofs_or_joint_names)
+        if any(isinstance(d, str) for d in names):
+            t = self.model.tables()
+            by_name = {nm: int(t["vidx"][i]) for i, nm in enumerate(t["joint_names"]) if i > 0}
+            missing = [d for d in names if isinstance(d, str) and d not in by_name]
+            if missing:
+                raise ValueError(f"set_actuator_network: unknown joints {missing}")
+            names = [by_name[d] if isinstance(d, str) else d for d in names]
+        dofs = np.ascontiguousarray(names, np.int32).reshape(-1)
+        if len(dofs) == 0:
+            _ck(lib().rsb_batch_set_actuator_network(self.h, None, 0, 0, 0, 0, None))
+            self.an_shape = None
+            return
+        pairs = _network_layers(layers)
+        H = int(history)
+        if len(pairs) < 2:
+            raise ValueError("set_actuator_network: need at least one hidden layer and the output layer")
+        width = pairs[0][0].shape[0]
+        for l, (w, b) in enumerate(pairs):
+            want = (1 if l == len(pairs) - 1 else width, 2 * H if l == 0 else width)
+            if w.shape != want or b.shape != (want[0],):
+                raise ValueError(f"set_actuator_network: layer {l}: need W {want} and b ({want[0]},), got {w.shape} and {b.shape}")
+        params = np.ascontiguousarray(np.concatenate([np.concatenate([w.ravel(), b.ravel()]) for w, b in pairs]), np.float32)
+        _ck(lib().rsb_batch_set_actuator_network(self.h, dofs.ctypes.data_as(C.c_void_p), len(dofs), H, len(pairs) - 1, width,
+                                                 params.ctypes.data_as(C.c_void_p)))
+        self.an_shape = (len(dofs), H)
+
+    def _an_rows(self):
+        if self.an_shape is None:
+            raise ValueError("actuator history: no actuator network set through this object")
+        return (self.an_shape[0], 2, self.an_shape[1] - 1)
+
+    def actuator_history(self, env_begin=0, env_count=None):
+        """[n, dofs, 2, H - 1] float32: errors then velocities of the last H - 1 sub-steps of every listed dof, most recent first"""
+        return self._read(lib().rsb_batch_get_actuator_history, self._an_rows(), np.float32, env_begin, env_count)
+
+    def actuator_history_into(self, rows, env_begin=0, env_count=None):
+        """actuator_history() copied into a torch CUDA tensor [n, dofs, 2, H - 1], in the batch's stream order"""
+        n = self._count(env_begin, env_count)
+        _ck(lib().rsb_batch_get_actuator_history(self.h, self._device_out(rows, (n,) + self._an_rows(), "rows"), env_begin, n, DEVICE))
+
+    def set_actuator_history(self, rows, env_begin=0, env_count=None):
+        """rows [n, dofs, 2, H - 1] (numpy) for environments [env_begin, env_begin + n); rows None zeroes env_count environments
+        (default: to the end of the batch).  A refused call (NaN or +-inf anywhere) changes nothing."""
+        shape = self._an_rows()
+        if rows is None:
+            _ck(lib().rsb_batch_set_actuator_history(self.h, None, env_begin, self._count(env_begin, env_count), HOST))
+            return
+        r = np.ascontiguousarray(rows, np.float32)
+        if r.ndim != 4 or r.shape[1:] != shape:
+            raise ValueError(f"rows: need shape [n, {shape[0]}, {shape[1]}, {shape[2]}], got {r.shape}")
+        _ck(lib().rsb_batch_set_actuator_history(self.h, r.ctypes.data_as(C.c_void_p), env_begin, r.shape[0], HOST))
+
+    def set_actuator_history_from(self, rows, env_begin=0):
+        """set_actuator_history() from a contiguous float32 torch tensor [n, dofs, 2, H - 1] on the batch's device, checked there"""
+        shape = self._an_rows()
+        n = rows.shape[0] if hasattr(rows, "shape") and len(rows.shape) > 0 else -1
+        _ck(lib().rsb_batch_set_actuator_history(self.h, self._device_out(rows, (n,) + shape, "rows"), env_begin, n, DEVICE))
 
     def control_step(self, ptarget, substeps, obs_out, vtarget=None):
         """one RaisimGym control step for the whole batch: targets in, fused sub-steps, observations out"""

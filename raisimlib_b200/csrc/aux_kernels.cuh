@@ -60,9 +60,10 @@ __global__ void rsb_body_inertia_pack_kernel(float* __restrict__ out, const floa
   if (fault) atomicMin(bad, r * 4 + fault);
 }
 
-// per-environment terrain friction rows (rsb_batch_set_contact_friction, StepArgs::contact_friction): `n` values of the caller copied as
-// they are.  A value that is NaN or +-inf lowers *bad to its index; *bad is left alone when every value is accepted
-__global__ void rsb_contact_friction_check_kernel(float* __restrict__ out, const float* __restrict__ src, int n, int* bad) {
+// per-environment terrain friction rows (rsb_batch_set_contact_friction, StepArgs::contact_friction) and actuator history rows
+// (rsb_batch_set_actuator_history, ActNetDesc::hist): `n` values of the caller copied as they are.  A value that is NaN or +-inf lowers
+// *bad to its index; *bad is left alone when every value is accepted
+__global__ void rsb_finite_rows_check_kernel(float* __restrict__ out, const float* __restrict__ src, int n, int* bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float v = src[i];
@@ -290,12 +291,15 @@ namespace rsb {
 // terminated environments, observe() -- is ONE launch of rsb_step_kernel (StepArgs::gym_action); only reset() of the whole batch is a kernel here.
 
 // ENVIRONMENT::reset() for every environment
-__global__ void rsb_gym_reset_kernel(float* gc, float* gv, float* ptarget, float* vtarget, GymConfig cfg, int gc_stride, int gv_stride, int nq, int nv, int num_envs) {
+// an_hist: the actuator network's history rows of an_words words per environment, zeroed (null: no network)
+__global__ void rsb_gym_reset_kernel(float* gc, float* gv, float* ptarget, float* vtarget, GymConfig cfg, int gc_stride, int gv_stride, int nq, int nv, int num_envs,
+                                     float* an_hist, int an_words) {
   const int lane = threadIdx.x & 31;
   const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (env >= num_envs) return;
   for (int i = lane; i < nq; i += 32) { gc[(size_t)env * gc_stride + i] = cfg.gc_init[i]; ptarget[(size_t)env * gc_stride + i] = cfg.gc_init[i]; }
   for (int i = lane; i < nv; i += 32) { gv[(size_t)env * gv_stride + i] = cfg.gv_init[i]; vtarget[(size_t)env * gv_stride + i] = 0.f; }
+  if (an_hist) for (int i = lane; i < an_words; i += 32) an_hist[(size_t)env * an_words + i] = 0.f;
 }
 
 }  // namespace rsb

@@ -142,11 +142,20 @@ struct rsb_batch {
   // of the check a call's rows pass before they replace any of them
   EnvRows body_inertia, contact_friction, actuator;
   DevBuf<int> row_bad;
+  // learned actuator network of rsb_batch_set_actuator_network (an_dofs empty: none): its parameters as the step kernel reads them
+  // (ActNetDesc::params) and the history rows [N][n][2][H - 1]
+  std::vector<int32_t> an_dofs;
+  int an_H = 0, an_L = 0, an_W = 0;
+  DevBuf<float> an_params, an_hist;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
-// the step kernel applies PD laws: PD mode, and gains from rsb_batch_set_pd_gains or per-environment actuator rows
-static bool pd_active(const rsb_batch* b) { return b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && (b->pd_set || b->actuator.active); }
+// the step kernel applies PD laws: PD mode, and gains from rsb_batch_set_pd_gains, per-environment actuator rows or an actuator network
+static bool pd_active(const rsb_batch* b) {
+  return b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && (b->pd_set || b->actuator.active || !b->an_dofs.empty());
+}
+// words of one environment's actuator history rows
+static size_t an_hist_words(const rsb_batch* b) { return b->an_dofs.size() * 2 * (size_t)std::max(0, b->an_H - 1); }
 
 // ------------------------------------------------------------------ blob ------------------------
 static void build_blob(const Model& md, const Overrides& ov, LaunchConfig& cfg) {
@@ -296,7 +305,7 @@ static void build_blob(const Model& md, const Overrides& ov, LaunchConfig& cfg) 
 // ------------------------------------------------------------------ launches --------------------
 template <int WPC, int SLOTS, int SPEC>
 static cudaError_t launch_step(const StepArgs& a, int grid, size_t smem, cudaStream_t s) {
-  auto kern = rsb_step_kernel<WPC, SLOTS, SPEC>;
+  auto kern = a.an.params ? rsb_step_kernel<WPC, SLOTS, SPEC, true> : rsb_step_kernel<WPC, SLOTS, SPEC, false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   kern<<<grid, WPC * 32, smem, s>>>(a);
@@ -421,6 +430,11 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
   a.body_inertia = b->body_inertia.active ? b->body_inertia.rows.get() : nullptr;
   a.contact_friction = b->contact_friction.active ? b->contact_friction.rows.get() : nullptr;
   a.actuator = b->actuator.active ? b->actuator.rows.get() : nullptr;
+  if (!b->an_dofs.empty() && a.use_pd) {   // the network and its history act in PD mode only
+    a.an.params = b->an_params.get(); a.an.hist = b->an_hist.get();
+    a.an.n = (int)b->an_dofs.size(); a.an.H = b->an_H; a.an.L = b->an_L; a.an.W = b->an_W;
+    for (int s = 0; s < a.an.n; s++) { a.an.dof[s] = (uint8_t)b->an_dofs[s]; a.an.mask |= 1ull << b->an_dofs[s]; }
+  }
   a.obs = io.obs; a.ob_dim = rsb_batch_ob_dim(b);
   if (io.gym_action) {   // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
     a.gym_action = io.gym_action; a.gym = b->gym; a.gym_reward = io.gym_reward; a.gym_done = io.gym_done;
@@ -1013,7 +1027,7 @@ int rsb_batch_set_contact_friction(rsb_batch* b, const float* rows, int env_begi
   const int ncoll = md.ncoll();
   auto check = [&](float* out, const float* src, int n, int* bad) {
     const int words = n * ncoll, threads = 128;
-    rsb_contact_friction_check_kernel<<<(unsigned)((words + threads - 1) / threads), threads, 0, b->stream>>>(out, src, words, bad);
+    rsb_finite_rows_check_kernel<<<(unsigned)((words + threads - 1) / threads), threads, 0, b->stream>>>(out, src, words, bad);
   };
   auto what = [&](int bad) {
     const int env = env_begin + bad / ncoll, c = bad % ncoll;
@@ -1049,6 +1063,79 @@ int rsb_batch_clear_actuator_params(rsb_batch* b) {
   if (!b) return fail(RSB_ERR_INVALID, "null batch");
   b->actuator.active = false;
   return RSB_OK;
+}
+// ---- learned actuator network (one per batch, shared by the listed dofs): checked and repacked on the host, the history on the device
+int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs, int history, int layers, int width, const float* params) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  const int nv = b->nv, nbase = b->model->md.floating ? 6 : 0;
+  if (n_dofs < 0 || n_dofs > nv) return fail(RSB_ERR_INVALID, "actuator network: n_dofs " + std::to_string(n_dofs) + " outside [0, " + std::to_string(nv) + "]");
+  if (n_dofs == 0) { b->an_dofs.clear(); return RSB_OK; }
+  if (!dofs) return fail(RSB_ERR_INVALID, "actuator network: null dof list");
+  std::vector<char> seen(nv, 0);
+  for (int s = 0; s < n_dofs; s++) {
+    const int d = dofs[s];
+    if (d < nbase || d >= nv) return fail(RSB_ERR_INVALID, "actuator network: dof " + std::to_string(d) + " outside the actuated dofs [" + std::to_string(nbase) + ", " + std::to_string(nv) + ")");
+    if (seen[d]) return fail(RSB_ERR_INVALID, "actuator network: dof " + std::to_string(d) + " listed twice");
+    seen[d] = 1;
+  }
+  if (history < 1 || history > RSB_ACTNET_MAX_HISTORY || layers < 1 || layers > RSB_ACTNET_MAX_LAYERS || width < 1 || width > RSB_ACTNET_MAX_WIDTH)
+    return fail(RSB_ERR_INVALID, "actuator network: history, layers and width must lie in [1, " + std::to_string(RSB_ACTNET_MAX_HISTORY) + "], [1, " +
+                                 std::to_string(RSB_ACTNET_MAX_LAYERS) + "] and [1, " + std::to_string(RSB_ACTNET_MAX_WIDTH) + "]");
+  if (!params) return fail(RSB_ERR_INVALID, "actuator network: null parameters");
+  const int F = 2 * history, W = width;
+  const size_t count = (size_t)W * F + W + (size_t)(layers - 1) * (W * W + W) + W + 1;
+  for (size_t k = 0; k < count; k++)
+    if (!std::isfinite(params[k])) return fail(RSB_ERR_INVALID, "actuator network: parameter " + std::to_string(k) + " is not finite; nothing changed");
+  // torch.nn.Linear order -> ActNetDesc::params: every hidden layer's weights transposed to [n_in][W], then its bias
+  std::vector<float> pk(count);
+  size_t so = 0;
+  for (int l = 0; l < layers; l++) {
+    const int nin = l == 0 ? F : W;
+    for (int j = 0; j < W; j++) for (int k = 0; k < nin; k++) pk[so + (size_t)k * W + j] = params[so + (size_t)j * nin + k];
+    so += (size_t)W * nin;
+    for (int j = 0; j < W; j++) pk[so + j] = params[so + j];
+    so += W;
+  }
+  for (size_t k = so; k < count; k++) pk[k] = params[k];   // output weights [W] and bias
+  CK(cudaSetDevice(b->device));
+  const size_t hist_words = (size_t)b->N * n_dofs * 2 * (history - 1);
+  CK(b->an_params.ensure(count * 4, b->stream));
+  CK(b->an_hist.ensure(std::max<size_t>(hist_words, 1) * 4, b->stream));
+  CK(cudaMemcpyAsync(b->an_params.get(), pk.data(), count * 4, cudaMemcpyHostToDevice, b->stream));
+  if (hist_words > 0) CK(cudaMemsetAsync(b->an_hist.get(), 0, hist_words * 4, b->stream));
+  CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
+  b->an_dofs.assign(dofs, dofs + n_dofs);
+  b->an_H = history; b->an_L = layers; b->an_W = width;
+  return RSB_OK;
+}
+int rsb_batch_set_actuator_history(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (b->an_dofs.empty()) return fail(RSB_ERR_INVALID, "actuator history: no actuator network (rsb_batch_set_actuator_network)");
+  const size_t w = an_hist_words(b), words = w * env_count;
+  if (words == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  float* const at = b->an_hist.get() + (size_t)env_begin * w;
+  if (!rows) { CK(cudaMemsetAsync(at, 0, words * 4, b->stream)); return RSB_OK; }
+  float* staged = nullptr;
+  auto check = [&](float* out, const float* src, int* bad) {
+    const int threads = 256;
+    rsb_finite_rows_check_kernel<<<(unsigned)((words + threads - 1) / threads), threads, 0, b->stream>>>(out, src, (int)words, bad);
+  };
+  auto what = [&](int bad) {
+    return "actuator history: environment " + std::to_string(env_begin + bad / (int)w) + ", word " + std::to_string(bad % (int)w) + " is not finite; nothing changed";
+  };
+  rc = stage_checked(b, rows, words, words, where, false, 0, check, what, &staged); if (rc) return rc;
+  CK(cudaMemcpyAsync(at, staged, words * 4, cudaMemcpyDeviceToDevice, b->stream));
+  return RSB_OK;
+}
+int rsb_batch_get_actuator_history(rsb_batch* b, float* rows, int env_begin, int env_count, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (b->an_dofs.empty()) return fail(RSB_ERR_INVALID, "actuator history: no actuator network (rsb_batch_set_actuator_network)");
+  const size_t w = an_hist_words(b), words = w * env_count;
+  if (words == 0) return RSB_OK;
+  if (!rows) return fail(RSB_ERR_INVALID, "actuator history: null rows");
+  CK(cudaSetDevice(b->device));
+  return copy_out(b, rows, b->an_hist.get() + (size_t)env_begin * w, words * 4, where);
 }
 int rsb_batch_set_control_mode(rsb_batch* b, int mode) {
   if (!b || (mode != RSB_FORCE_AND_TORQUE && mode != RSB_PD_PLUS_FEEDFORWARD_TORQUE)) return fail(RSB_ERR_INVALID, "bad control mode");
@@ -1428,7 +1515,8 @@ int rsb_batch_gym_reset(rsb_batch* b) {
   if (!b || !b->gym_ready) return fail(RSB_ERR_INVALID, "call rsb_batch_gym_configure() first");
   CK(cudaSetDevice(b->device));
   int threads = 128, blocks = (b->N * 32 + threads - 1) / threads;
-  rsb_gym_reset_kernel<<<blocks, threads, 0, b->stream>>>(b->gc.get(), b->gv.get(), b->pt.get(), b->vt.get(), b->gym, b->gc_stride, b->gv_stride, b->nq, b->nv, b->N);
+  rsb_gym_reset_kernel<<<blocks, threads, 0, b->stream>>>(b->gc.get(), b->gv.get(), b->pt.get(), b->vt.get(), b->gym, b->gc_stride, b->gv_stride, b->nq, b->nv, b->N,
+                                                          b->an_dofs.empty() ? nullptr : b->an_hist.get(), (int)an_hist_words(b));
   CK(cudaGetLastError());
   b->kin_dirty = true;
   b->launches++;
@@ -1462,7 +1550,7 @@ int rsb_batch_gym_step(rsb_batch* b, const float* action, int where_in, int subs
   unsigned char* d_done = a_done ? a_done : (host_out || !done) ? b->gym_done.get() : done;
   // ONE launch: action rows -> PD targets, `substeps` x World::integrate(), reward, isTerminalState(), reset() of the terminated
   // environments and the observation rows of the resulting state (the task used to be an action kernel and a post kernel around the step)
-  if (!pd_active(b)) return fail(RSB_ERR_INVALID, "the gym task drives the robot through PD targets: call rsb_batch_set_pd_gains() or rsb_batch_set_actuator_params() first");
+  if (!pd_active(b)) return fail(RSB_ERR_INVALID, "the gym task drives the robot through PD targets: call rsb_batch_set_pd_gains(), rsb_batch_set_actuator_params() or rsb_batch_set_actuator_network() first");
   LaunchIO io;
   io.obs = d_obs; io.gym_action = act; io.gym_reward = d_rew; io.gym_done = d_done;
   int rc = do_launch(b, substeps, 0, false, io); if (rc) return rc;

@@ -194,6 +194,17 @@ struct GymConfig {
   float torque_coeff, forward_vel_coeff, terminal_reward;
 };
 
+// learned actuator network (rsb_batch_set_actuator_network), read by stage C; params == null: no network, or a launch that applies no
+// PD laws (force mode)
+constexpr int AN_MAX_DOFS = 64;          // >= nv of every model (32 bodies)
+struct ActNetDesc {
+  const float* params;   // per hidden layer: weights transposed [n_in][W] (lanes read consecutive words), bias [W]; output weights [W], bias
+  float* hist;           // [num_envs][n][2][H - 1]: errors then velocities of the last H - 1 sub-steps, most recent first
+  unsigned long long mask;   // bit i: dof i is listed
+  int n, H, L, W;
+  uint8_t dof[AN_MAX_DOFS];
+};
+
 // StepArgs::phase_mask bits of the launches that stop early (the host's getters and integrate1())
 constexpr int PHASE_NO_UPDATE = 1;    // stop after stage B (integrate1: no state update)
 constexpr int PHASE_KINEMATICS = 4;   // stop after stage A (stage A + the getters' buffers; the contact records of the last integrate() stay)
@@ -256,6 +267,7 @@ struct StepArgs {
   int phase_mask;      // 0 (a full step) or PHASE_NO_UPDATE, optionally with PHASE_KINEMATICS
   int substep_barrier; // non-zero: re-align the CTA's warps of one round at every sub-step
   int pair_stage_a;    // 1: quadruped instance, CTAs that keep the sub-step barrier: one warp runs stage A of two environments
+  ActNetDesc an;       // learned actuator network (stages C and E, the gym epilogue); an.params null = none
 };
 
 // ------------------------------------------------------------------ small device math ----------
@@ -769,6 +781,69 @@ __device__ __forceinline__ void apply_row_bias(float& u_c, const rsb_params& prm
   }
 }
 
+// Stage C: the actuator network of every listed dof of environment env at the start of the sub-step; net[i] = its output for listed dof i.
+// Lane j is hidden unit j.  The listed dofs go through in groups of AN_G, each lane carrying one accumulator per dof of the group, so
+// that every weight load (read-only path, transposed: the lanes read consecutive words) serves AN_G dofs.  A layer's inputs sit in s_x
+// as [input][AN_G]: one 16-byte broadcast load gives one input of the whole group.  This sub-step's (e, v) go in front of the
+// environment's history, which is shifted in place.  s_x: RSB_ACTNET_MAX_WIDTH * AN_G words of scratch (16-byte aligned), dead outside
+// this call.
+constexpr int AN_G = 4;
+static_assert(RSB_ACTNET_MAX_WIDTH * AN_G <= HIST_WORDS, "the network's scratch is the Anderson history");
+__device__ __forceinline__ void actuator_network(const ActNetDesc& an, int env, int lane, const float* s_gc, const float* s_gv, const float* s_pt,
+                                                 const int* dofq, float* s_x, float* net) {
+  const int H = an.H, W = an.W, F = 2 * H, hw = H - 1, n = an.n;
+  float* const hist = an.hist + (size_t)env * n * 2 * hw;
+#pragma unroll 1
+  for (int g0 = 0; g0 < n; g0 += AN_G) {
+    // features of the group: lane = (dof d of the group, feature k), AN_G * 2H <= 32; 0 past the end of the list
+    float x = 0.f;
+    int hi = -1;
+    if (lane < AN_G * F) {
+      const int d = lane / F, k = lane - d * F, s = g0 + d;
+      if (s < n) {
+        const int c = k >= H ? 1 : 0, t = k - c * H;   // c: 0 error, 1 velocity; t: sub-steps back
+        const int i = an.dof[s];
+        if (t > 0) x = hist[(s * 2 + c) * hw + t - 1];
+        else if (c) x = s_gv[i];
+        else { const int q = dofq[i]; x = s_pt[q] - s_gc[q]; }
+        if (t < hw) hi = (s * 2 + c) * hw + t;
+      }
+      s_x[k * AN_G + d] = x;
+    }
+    __syncwarp();
+    if (hi >= 0) hist[hi] = x;   // every lane has read the old history above
+    const float* p = an.params;
+    float h0 = 0.f, h1 = 0.f, h2 = 0.f, h3 = 0.f;
+#pragma unroll 1
+    for (int l = 0, nin = F; l < an.L; l++, nin = W) {
+      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+      if (lane < W) { a0 = a1 = a2 = a3 = __ldg(p + nin * W + lane); }
+#pragma unroll 4
+      for (int k = 0; k < nin; k++) {
+        const float w = lane < W ? __ldg(p + k * W + lane) : 0.f;
+        const float4 xk = *reinterpret_cast<const float4*>(s_x + k * AN_G);
+        a0 = fmaf(w, xk.x, a0); a1 = fmaf(w, xk.y, a1); a2 = fmaf(w, xk.z, a2); a3 = fmaf(w, xk.w, a3);
+      }
+      p += nin * W + W;
+      h0 = a0 / (1.f + fabsf(a0)); h1 = a1 / (1.f + fabsf(a1)); h2 = a2 / (1.f + fabsf(a2)); h3 = a3 / (1.f + fabsf(a3));
+      __syncwarp();   // every lane has read this layer's inputs
+      if (lane < W) *reinterpret_cast<float4*>(s_x + lane * AN_G) = make_float4(h0, h1, h2, h3);
+      __syncwarp();
+    }
+    // output layer: a butterfly sum over the hidden units (lanes >= W hold 0)
+    const float wo = lane < W ? __ldg(p + lane) : 0.f;
+    float o0 = wo * h0, o1 = wo * h1, o2 = wo * h2, o3 = wo * h3;
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) {
+      o0 += __shfl_xor_sync(FULL, o0, m); o1 += __shfl_xor_sync(FULL, o1, m);
+      o2 += __shfl_xor_sync(FULL, o2, m); o3 += __shfl_xor_sync(FULL, o3, m);
+    }
+    const float o = lane == 0 ? o0 : lane == 1 ? o1 : lane == 2 ? o2 : o3;
+    if (lane < AN_G && g0 + lane < n) net[an.dof[g0 + lane]] = __ldg(p + W) + o;
+    __syncwarp();   // s_x is refilled by the next group
+  }
+}
+
 // Stages C and E: kp, kd and effort limit of dof i in environment env.  The blob's value (gain: kp | kd | effort, nvp each) unless the
 // environment has a row (StepArgs::actuator) whose entry is >= 0; the gains are 0 outside PD mode (use_pd), the effort limit holds in
 // both control modes
@@ -819,7 +894,8 @@ __host__ __device__ constexpr bool operator==(const Dims& a, const Dims& b) {
   return a.nb == b.nb && a.nq == b.nq && a.nv == b.nv && a.floating == b.floating && a.maxdepth == b.maxdepth && a.maxdd == b.maxdd;
 }
 
-template <int WPC, int SLOTS, int SPEC>
+// AN: the instance with the actuator network (launched only while one is set and PD laws apply); without it the step is what it was
+template <int WPC, int SLOTS, int SPEC, bool AN>
 __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel(const __grid_constant__ StepArgs args) {
   extern __shared__ __align__(128) uint32_t smem[];
   __shared__ __align__(8) uint64_t tma_bar;
@@ -1246,14 +1322,20 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           for (int i = lane; i < nv; i += 32) args.vt_store[(size_t)env * args.gv_stride + i] = s_vt[i];
         }
       }
+      // actuator network: a listed dof has no PD law and the feed-forward torque tau_ff + net, its network torque kept in s_vt (its
+      // velocity target, which it does not use; reloaded by every launch) for stage E.  Scratch: the Anderson history of stage D
+      if constexpr (AN) { actuator_network(args.an, env, lane, s_gc, s_gv, s_pt, dofq, s_hist, s_vt); __syncwarp(); }
 #pragma unroll 1
       for (int i = lane; i < nv; i += 32) {
-        float bi = s_tau[i] - s_h[i];
+        const bool an = AN && ((args.an.mask >> i) & 1ull);
+        const float tff = an ? s_tau[i] + s_vt[i] : s_tau[i];
+        float bi = tff - s_h[i];
         // actuator effort limit (oracle step()): when feed-forward + PD law at the current state exceed it, the joint is driven by the
         // constant limit torque over this step and gets no implicit PD terms
-        float te = s_tau[i];
+        float te = tff;
         float kpi, kdi, emi;
         dof_actuator(args, gain, nvp, env, nv, i, kpi, kdi, emi);
+        if (an) { kpi = 0.f; kdi = 0.f; }
         const bool pd = kpi != 0.f || kdi != 0.f;
         const int qi = pd ? dofq[i] : 0;
         if (pd) te += kpi * (s_pt[qi] - s_gc[qi]) + kdi * (s_vt[i] - s_gv[i]);
@@ -1261,7 +1343,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         const float soft = args.prm.dt * kdi + args.prm.dt * args.prm.dt * kpi;
         const bool sat = fabsf(te) > emi * (1.f + soft / s_L[i * DLP + ddepth[i]]);
         s_sat[i] = sat ? 1.f : 0.f;          // remembered for stage E (generalized force applied)
-        if (sat) bi += copysignf(emi, te) - s_tau[i];
+        if (sat) bi += copysignf(emi, te) - tff;
         else if (pd) {
           bi += kpi * (s_pt[qi] - s_gc[qi] - args.prm.dt * s_gv[i]) + kdi * (s_vt[i] - s_gv[i]);
           s_L[i * DLP + ddepth[i]] += args.prm.dt * kdi + args.prm.dt * args.prm.dt * kpi;
@@ -1685,9 +1767,11 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         const float v0 = s_gv[i], vp = v0 + s_rhs[i];
         s_gv[i] = vp;
         // generalized force applied over this step (implicit PD evaluated at q + dt v+, v+; the effort limit where it was hit): getGeneralizedForce()
-        float ta = s_tau[i];
+        const bool an = AN && ((args.an.mask >> i) & 1ull);   // network dof: the explicit torque of stage C
+        float ta = an ? s_tau[i] + s_vt[i] : s_tau[i];
         float kpi, kdi, emi;
         dof_actuator(args, gain, nvp, env, nv, i, kpi, kdi, emi);
+        if (an) { kpi = 0.f; kdi = 0.f; }
         const bool pd = kpi != 0.f || kdi != 0.f;
         const int qi = pd ? dofq[i] : 0;
         float te = ta;
@@ -1775,6 +1859,11 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         for (int i = lane; i < nq; i += 32) { const float g0 = args.gym.gc_init[i]; s_gc[i] = g0; if (args.pt_store) args.pt_store[(size_t)env * args.gc_stride + i] = g0; }
 #pragma unroll 1
         for (int i = lane; i < nv; i += 32) s_gv[i] = args.gym.gv_init[i];
+        if constexpr (AN) {
+          const int hw = args.an.n * 2 * (args.an.H - 1);
+#pragma unroll 1
+          for (int i = lane; i < hw; i += 32) args.an.hist[(size_t)env * hw + i] = 0.f;
+        }
       }
       if (lane == 0) { args.gym_reward[env] = r; args.gym_done[env] = term ? 1 : 0; }
       __syncwarp();

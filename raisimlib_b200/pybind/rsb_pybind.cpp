@@ -133,6 +133,24 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void set_actuator_params(uintptr_t rows_dev, int env_begin, int env_count) {
     check(rsb_batch_set_actuator_params(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_actuator_params");
   }
+  // learned actuator network: dofs (gv indices), parameters in torch.nn.Linear order (host); an empty dof list clears it
+  void set_actuator_network(const std::vector<int32_t>& dofs, int history, int layers, int width, const std::vector<float>& params) {
+    if (!dofs.empty()) {   // the library reads exactly this many floats
+      const size_t count = (history < 1 || layers < 1 || width < 1) ? 0
+                         : size_t(2 * history) * width + width + size_t(layers - 1) * (size_t(width) * width + width) + width + 1;
+      if (count == 0 || params.size() != count)
+        throw std::runtime_error("set_actuator_network: " + std::to_string(params.size()) + " parameters for history " + std::to_string(history) + ", " +
+                                 std::to_string(layers) + " layers of width " + std::to_string(width) + " (need " + std::to_string(count) + ")");
+    }
+    check(rsb_batch_set_actuator_network(b_, dofs.data(), (int)dofs.size(), history, layers, width, params.data()), "set_actuator_network");
+  }
+  // its history rows [env_count, dofs, 2, history - 1] float32 at a device address (0: zeroes the range)
+  void set_actuator_history(uintptr_t rows_dev, int env_begin, int env_count) {
+    check(rsb_batch_set_actuator_history(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_actuator_history");
+  }
+  void actuator_history(uintptr_t rows_dev, int env_begin, int env_count) {
+    check(rsb_batch_get_actuator_history(b_, reinterpret_cast<float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "actuator_history");
+  }
   // terrain atlas: heights [count * ys * xs] and the map of every environment [num_envs], host lists
   void set_heightmaps(int count, int xs, int ys, float x_size, float y_size, float cx, float cy, const std::vector<float>& heights,
                       const std::vector<int32_t>& map_of_env) {
@@ -189,6 +207,9 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_contact_friction", &Batch::set_contact_friction, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_actuator_params", &Batch::set_actuator_params, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
+      .def("set_actuator_network", &Batch::set_actuator_network, py::arg("dofs"), py::arg("history"), py::arg("layers"), py::arg("width"), py::arg("params"))
+      .def("set_actuator_history", &Batch::set_actuator_history, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
+      .def("actuator_history", &Batch::actuator_history, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_heightmaps", &Batch::set_heightmaps, py::arg("count"), py::arg("xs"), py::arg("ys"), py::arg("x_size"), py::arg("y_size"),
            py::arg("cx"), py::arg("cy"), py::arg("heights"), py::arg("map_of_env"))
       .def("set_heightmap_index", &Batch::set_heightmap_index, py::arg("map_of_env_dev"), py::arg("env_begin"), py::arg("env_count"))
