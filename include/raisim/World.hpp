@@ -116,6 +116,8 @@ struct LockStep {
   size_t actHistWords = 0;                  // words of one environment's actuator-network history (0: no network, or history 1)
   std::vector<char> actHistReset;           // [n] ArticulatedSystem::resetActuatorHistory() since the last upload
   bool actHistDirty = false;
+  std::vector<int32_t> delay;               // [n] ArticulatedSystem::setActuationDelay since the last upload (-1: unchanged); empty until the first one
+  bool delayDirty = false;
   int scanPoints = 0;
   bool scanValid = false;
   // terrain of every environment (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding the same heights
@@ -196,6 +198,7 @@ struct LockStep {
     if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
     pushTerrain();
     pushActuatorHistory();
+    pushActuationDelay();
     stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
@@ -212,6 +215,7 @@ struct LockStep {
     if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
     pushTerrain();
     pushActuatorHistory();
+    pushActuationDelay();
     stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
   }
   // environment env's actuator-network history goes to zero before the next launch (ArticulatedSystem::resetActuatorHistory)
@@ -220,6 +224,20 @@ struct LockStep {
     if (actHistReset.empty()) actHistReset.assign(n, 0);
     actHistReset[env] = 1;
     actHistDirty = true;
+  }
+  // environment env's actuation delay, set (and its command history emptied) before the next launch
+  void setActuationDelay(int env, int subSteps) {
+    sync(env);
+    if (delay.empty()) delay.assign(n, -1);
+    delay[env] = subSteps;
+    delayDirty = true;
+  }
+  // the delays set since the last upload in one call, only when some environment set one; the other entries are -1 (unchanged)
+  void pushActuationDelay() {
+    if (!delayDirty) return;
+    delayDirty = false;
+    rsbCheck(rsb_batch_set_actuation_delay(batch, delay.data(), 0, n, RSB_HOST), "setActuationDelay");
+    std::fill(delay.begin(), delay.end(), -1);
   }
   // the marked environments' history rows zeroed: one get and one set of all rows, only when some environment reset
   void pushActuatorHistory() {
@@ -413,6 +431,13 @@ class BatchedWorld {
   void resetActuatorHistory(int env) {
     if (ls_) { ls_->resetActuatorHistory(env); return; }
     if (!anDofs_.empty()) rsbCheck(rsb_batch_set_actuator_history(batch_, nullptr, env, 1, RSB_HOST), "resetActuatorHistory");
+  }
+  // environment env's actuation delay in sub-steps (ArticulatedSystem::setActuationDelay): at once in a stand-alone World, before the
+  // next launch in a VectorizedEnvironment
+  void setActuationDelay(int env, int subSteps) {
+    if (ls_) { ls_->setActuationDelay(env, subSteps); return; }
+    const int32_t d = subSteps;
+    rsbCheck(rsb_batch_set_actuation_delay(batch_, &d, env, 1, RSB_HOST), "setActuationDelay");
   }
   const std::string& urdf() const { return urdf_; }
   void rememberUrdf(const std::string& u) { urdf_ = u; }
@@ -1042,6 +1067,15 @@ class ArticulatedSystem {
   }
   // zero this environment's actuator-network history (setState keeps it): call it in reset()
   void resetActuatorHistory() { w_->resetActuatorHistory(env_); }
+  // setActuationDelay: from now on every joint command (PD targets, feed-forward torque) of this robot takes effect subSteps physics
+  // sub-steps after it was set (rsb_batch_set_actuation_delay, include/rsb.h); setting it empties the command history, so the first
+  // command then holds for subSteps + 1 sub-steps.  Call it in reset() to draw a delay per episode.  In a VectorizedEnvironment the
+  // delays of all environments go up with the next launch in one call.
+  void setActuationDelay(size_t subSteps) {
+    if (subSteps > RSB_MAX_ACTUATION_DELAY)
+      throw std::runtime_error("setActuationDelay: " + std::to_string(subSteps) + " sub-steps, at most " + std::to_string(RSB_MAX_ACTUATION_DELAY));
+    w_->setActuationDelay(env_, int(subSteps));
+  }
   // the world z of the collision surface under every point at the current state, in setHeightScan order, and (samples, optional) the
   // world (x, y) each was taken at.  In a VectorizedEnvironment one call scans every environment for the control step; a stand-alone
   // World scans this environment

@@ -294,6 +294,31 @@ int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs
  * RSB_ERR_INVALID, changing nothing: a null batch, no network, a bad range or `where`, a value that is not finite. */
 int rsb_batch_set_actuator_history(rsb_batch* b, const float* rows, int env_begin, int env_count, int where);
 int rsb_batch_get_actuator_history(rsb_batch* b, float* rows, int env_begin, int env_count, int where);
+/* Actuation delay: a joint command takes effect a chosen number of physics sub-steps after it was issued, per environment (a real
+ * robot applies a policy's command some milliseconds late; training draws the delay per environment at every episode reset).
+ *   Command: at every advancing sub-step, the triple (ptarget[q(d)], vtarget[d], tau_ff[d]) the step would use for every dof d that is
+ *   not one of a floating base's six, whatever its source: rsb_batch_set_pd_target, a bound buffer (rsb_batch_bind_pd_target),
+ *   rsb_batch_control_step targets (pinned rows read in place included), the gym task's action * std + mean, rsb_batch_set_generalized_force.
+ *   It is recorded in both control modes.
+ *   Delay and history: each environment has a delay d in [0, RSB_MAX_ACTUATION_DELAY] sub-steps and a command history.  With t the
+ *   advancing sub-steps since the history was last emptied, counted from 0, sub-step t applies cmd(max(t - d, 0)): after an emptying
+ *   the first command holds for the first d + 1 sub-steps.  The applied command is what the implicit PD law and its saturation test,
+ *   the actuator network's error and rsb_batch_get_generalized_force use.  Gains, effort limits and the network are not delayed; the
+ *   batch's target rows keep the commanded values, so targets persist across launches as they do without a delay.
+ *   Only launches that advance the state record a command: integrate, integrate2, control_step, gym_step.  integrate1, the kinematics
+ *   pass, the getters, the frame calls and the height scan do not, so 1 launch of 4 sub-steps equals 4 launches of 1 bit for bit.
+ *   Emptying: setting an environment's delay, rsb_batch_gym_reset (every environment) and a termination in rsb_batch_gym_step (that
+ *   environment) empty its history; the last two keep the delay.  rsb_batch_set_state and rsb_batch_set_pd_target do not.
+ * delays [env_count] int32, host or device (`where`): an entry d >= 0 sets that environment's delay and empties its history, an entry
+ * -1 leaves the environment as it is (so a trainer may pass where(done, new_delay, -1) from the device).  delays == NULL sets 0 and
+ * empties the whole range.  The first call, and the first after rsb_batch_clear_actuation_delay, starts every environment at delay 0
+ * with an empty history; delays of 0 give results bit-identical to no delay.  The entries are checked on the device in the batch's
+ * staging buffer before any is committed; the call waits for that check.  Refused with RSB_ERR_INVALID, changing nothing: a null
+ * batch, a bad range or `where`, an entry < -1 or > RSB_MAX_ACTUATION_DELAY. */
+#define RSB_MAX_ACTUATION_DELAY 16
+int rsb_batch_set_actuation_delay(rsb_batch* b, const int32_t* delays, int env_begin, int env_count, int where);
+/* drop the delays and the histories: every later launch runs exactly as if none had been set */
+int rsb_batch_clear_actuation_delay(rsb_batch* b);
 /* ArticulatedSystem::getGeneralizedForce(): feed-forward + PD force applied over the last integrate() */
 int rsb_batch_get_generalized_force(rsb_batch* b, float* tau, int env_begin, int env_count, int where);
 

@@ -14,6 +14,7 @@ HOST, DEVICE = 0, 1
 FORCE_AND_TORQUE, PD_PLUS_FEEDFORWARD_TORQUE = 0, 1
 SCAN_YAW, SCAN_WORLD = 0, 1
 MAX_SCAN_POINTS = 1024
+ACTUATION_DELAY_MAX = 16   # RSB_MAX_ACTUATION_DELAY: sub-steps
 
 
 class RsbError(RuntimeError):
@@ -98,7 +99,7 @@ EXPORTED = [
     "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_set_heightmap_index", "rsb_batch_update_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
     "rsb_batch_set_collision_friction", "rsb_batch_set_self_collision",
     "rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_gains", "rsb_batch_set_pd_target",
-    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_actuator_params", "rsb_batch_clear_actuator_params", "rsb_batch_set_actuator_network", "rsb_batch_set_actuator_history", "rsb_batch_get_actuator_history", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
+    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_actuator_params", "rsb_batch_clear_actuator_params", "rsb_batch_set_actuator_network", "rsb_batch_set_actuator_history", "rsb_batch_get_actuator_history", "rsb_batch_set_actuation_delay", "rsb_batch_clear_actuation_delay", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
     "rsb_batch_integrate1", "rsb_batch_integrate2", "rsb_batch_integrate",
     "rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities", "rsb_batch_get_body_poses", "rsb_batch_get_contacts",
     "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
@@ -198,6 +199,9 @@ def lib():
             L.rsb_batch_set_actuator_network.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
             L.rsb_batch_set_actuator_history.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
             L.rsb_batch_get_actuator_history.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+        if hasattr(L, "rsb_batch_set_actuation_delay"):    # absent from an older build loaded through RSB_LIB_PATH (tools/actuation_delay_probe.py)
+            L.rsb_batch_set_actuation_delay.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+            L.rsb_batch_clear_actuation_delay.argtypes = [C.c_void_p]
         if hasattr(L, "rsb_batch_set_height_scan"):        # absent from an older build loaded through RSB_LIB_PATH (tools/height_scan_probe.py)
             L.rsb_batch_set_height_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
             L.rsb_batch_get_height_scan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
@@ -828,6 +832,30 @@ class Batch:
         shape = self._an_rows()
         n = rows.shape[0] if hasattr(rows, "shape") and len(rows.shape) > 0 else -1
         _ck(lib().rsb_batch_set_actuator_history(self.h, self._device_out(rows, (n,) + shape, "rows"), env_begin, n, DEVICE))
+
+    # actuation delay
+    def set_actuation_delay(self, delays, env_begin=0):
+        """environments [env_begin, env_begin + len(delays)) apply each joint command delays [n] (numpy int32) physics sub-steps late:
+        an entry d in [0, ACTUATION_DELAY_MAX] sets the delay and empties the environment's command history, -1 leaves the environment
+        as it is.  delays None sets 0 and empties every environment from env_begin on.  A refused call changes nothing."""
+        if delays is None:
+            _ck(lib().rsb_batch_set_actuation_delay(self.h, None, env_begin, self.n - env_begin, HOST))
+            return
+        d = np.asarray(delays)
+        if d.dtype != np.int32 or d.ndim != 1:
+            raise ValueError(f"delays: need a 1-D numpy int32 array, got {d.dtype} of shape {d.shape}")
+        d = np.ascontiguousarray(d)
+        _ck(lib().rsb_batch_set_actuation_delay(self.h, d.ctypes.data_as(C.c_void_p), env_begin, len(d), HOST))
+
+    def set_actuation_delay_from(self, delays, env_begin=0):
+        """set_actuation_delay() from a contiguous int32 torch tensor [n] on the batch's device, checked there: a trainer passes
+        torch.where(done, new_delay, -1) without a host round trip"""
+        n = delays.shape[0] if hasattr(delays, "shape") and len(delays.shape) == 1 else -1
+        _ck(lib().rsb_batch_set_actuation_delay(self.h, self._device_out(delays, (n,), "delays", "int32"), env_begin, n, DEVICE))
+
+    def clear_actuation_delay(self):
+        """drop every delay and command history: later steps run as if none had been set"""
+        _ck(lib().rsb_batch_clear_actuation_delay(self.h))
 
     def control_step(self, ptarget, substeps, obs_out, vtarget=None):
         """one RaisimGym control step for the whole batch: targets in, fused sub-steps, observations out"""

@@ -90,15 +90,25 @@ __global__ void rsb_actuator_params_check_kernel(float* __restrict__ out, const 
   }
 }
 
-// atlas map index of a range of environments (rsb_batch_set_heightmap_index, TerrainDesc::env_map): `n` indices of the caller copied as
-// they are (out may be src: the check runs in place on a host source's staged copy).  An index outside [0, count) lowers *bad to its
-// position; *bad is left alone when every index is accepted
-__global__ void rsb_heightmap_index_check_kernel(int* out, const int* src, int n, int count, int* bad) {
+// int32 entries of a range of environments: atlas map indices (rsb_batch_set_heightmap_index, TerrainDesc::env_map) and actuation
+// delays (rsb_batch_set_actuation_delay): `n` entries of the caller copied as they are (out may be src: the check runs in place on a
+// host source's staged copy).  An entry outside [lo, hi] lowers *bad to its position; *bad is left alone when every entry is accepted
+__global__ void rsb_int_rows_check_kernel(int* out, const int* src, int n, int lo, int hi, int* bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int v = src[i];
   out[i] = v;
-  if (v < 0 || v >= count) atomicMin(bad, i);
+  if (v < lo || v > hi) atomicMin(bad, i);
+}
+
+// actuation delays of `n` environments (rsb_batch_set_actuation_delay) committed to their [n][2] (delay, sub-steps since the history
+// was emptied) rows, StepArgs::delay_state: an entry d >= 0 sets the delay and empties the history, -1 leaves the row; delays == null
+// sets 0 and empties every row
+__global__ void rsb_actuation_delay_commit_kernel(int* state, const int* delays, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int d = delays ? delays[i] : 0;
+  if (d >= 0) { state[2 * i] = d; state[2 * i + 1] = 0; }
 }
 
 // ordered-integer image of a float: signed integer order is the float order (-0 just below +0), so atomicMax on it takes the largest
@@ -291,15 +301,17 @@ namespace rsb {
 // terminated environments, observe() -- is ONE launch of rsb_step_kernel (StepArgs::gym_action); only reset() of the whole batch is a kernel here.
 
 // ENVIRONMENT::reset() for every environment
-// an_hist: the actuator network's history rows of an_words words per environment, zeroed (null: no network)
+// an_hist: the actuator network's history rows of an_words words per environment, zeroed (null: no network); delay_state: the
+// actuation delay rows (StepArgs::delay_state), whose command histories are emptied and delays kept (null: no delay)
 __global__ void rsb_gym_reset_kernel(float* gc, float* gv, float* ptarget, float* vtarget, GymConfig cfg, int gc_stride, int gv_stride, int nq, int nv, int num_envs,
-                                     float* an_hist, int an_words) {
+                                     float* an_hist, int an_words, int* delay_state) {
   const int lane = threadIdx.x & 31;
   const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (env >= num_envs) return;
   for (int i = lane; i < nq; i += 32) { gc[(size_t)env * gc_stride + i] = cfg.gc_init[i]; ptarget[(size_t)env * gc_stride + i] = cfg.gc_init[i]; }
   for (int i = lane; i < nv; i += 32) { gv[(size_t)env * gv_stride + i] = cfg.gv_init[i]; vtarget[(size_t)env * gv_stride + i] = 0.f; }
   if (an_hist) for (int i = lane; i < an_words; i += 32) an_hist[(size_t)env * an_words + i] = 0.f;
+  if (delay_state && lane == 0) delay_state[2 * env + 1] = 0;
 }
 
 }  // namespace rsb

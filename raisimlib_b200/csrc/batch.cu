@@ -147,6 +147,11 @@ struct rsb_batch {
   std::vector<int32_t> an_dofs;
   int an_H = 0, an_L = 0, an_W = 0;
   DevBuf<float> an_params, an_hist;
+  // actuation delays of rsb_batch_set_actuation_delay while delay_active: (delay, sub-steps since the history was emptied) rows [N][2]
+  // and the command rings [N][DELAY_SLOTS][3][nv - nbase] (StepArgs::delay_state, delay_ring)
+  DevBuf<int> delay_state;
+  DevBuf<float> delay_ring;
+  bool delay_active = false;
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
@@ -305,7 +310,8 @@ static void build_blob(const Model& md, const Overrides& ov, LaunchConfig& cfg) 
 // ------------------------------------------------------------------ launches --------------------
 template <int WPC, int SLOTS, int SPEC>
 static cudaError_t launch_step(const StepArgs& a, int grid, size_t smem, cudaStream_t s) {
-  auto kern = a.an.params ? rsb_step_kernel<WPC, SLOTS, SPEC, true> : rsb_step_kernel<WPC, SLOTS, SPEC, false>;
+  auto kern = a.delay_state ? (a.an.params ? rsb_step_kernel<WPC, SLOTS, SPEC, true, true> : rsb_step_kernel<WPC, SLOTS, SPEC, false, true>)
+                            : (a.an.params ? rsb_step_kernel<WPC, SLOTS, SPEC, true, false> : rsb_step_kernel<WPC, SLOTS, SPEC, false, false>);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   kern<<<grid, WPC * 32, smem, s>>>(a);
@@ -435,6 +441,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
     a.an.n = (int)b->an_dofs.size(); a.an.H = b->an_H; a.an.L = b->an_L; a.an.W = b->an_W;
     for (int s = 0; s < a.an.n; s++) { a.an.dof[s] = (uint8_t)b->an_dofs[s]; a.an.mask |= 1ull << b->an_dofs[s]; }
   }
+  if (b->delay_active && phase_mask == 0) { a.delay_state = b->delay_state.get(); a.delay_ring = b->delay_ring.get(); }   // only advancing launches record a command
   a.obs = io.obs; a.ob_dim = rsb_batch_ob_dim(b);
   if (io.gym_action) {   // targets come from the action rows and are kept in the batch's own rows; terminated environments get their reset target there too
     a.gym_action = io.gym_action; a.gym = b->gym; a.gym_reward = io.gym_reward; a.gym_done = io.gym_done;
@@ -815,7 +822,7 @@ int rsb_batch_set_heightmap_index(rsb_batch* b, const int32_t* map_of_env, int e
   int* staged = nullptr;
   auto check = [&](int* out, const int* src, int* bad) {
     const int threads = 256;
-    rsb_heightmap_index_check_kernel<<<(unsigned)((env_count + threads - 1) / threads), threads, 0, b->stream>>>(out, src, env_count, count, bad);
+    rsb_int_rows_check_kernel<<<(unsigned)((env_count + threads - 1) / threads), threads, 0, b->stream>>>(out, src, env_count, 0, count - 1, bad);
   };
   auto what = [&](int bad) {
     return "height-map index: environment " + std::to_string(env_begin + bad) + " names a map outside [0, " + std::to_string(count) + "); nothing changed";
@@ -1136,6 +1143,37 @@ int rsb_batch_get_actuator_history(rsb_batch* b, float* rows, int env_begin, int
   if (!rows) return fail(RSB_ERR_INVALID, "actuator history: null rows");
   CK(cudaSetDevice(b->device));
   return copy_out(b, rows, b->an_hist.get() + (size_t)env_begin * w, words * 4, where);
+}
+// ---- actuation delay: the entries checked in the staging buffer, then committed by a kernel in stream order
+int rsb_batch_set_actuation_delay(rsb_batch* b, const int32_t* delays, int env_begin, int env_count, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (env_count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const int threads = 256, blocks = (env_count + threads - 1) / threads;
+  int* staged = nullptr;
+  if (delays) {
+    auto check = [&](int* out, const int* src, int* bad) {
+      rsb_int_rows_check_kernel<<<(unsigned)blocks, threads, 0, b->stream>>>(out, src, env_count, -1, RSB_MAX_ACTUATION_DELAY, bad);
+    };
+    auto what = [&](int bad) {
+      return "actuation delay: environment " + std::to_string(env_begin + bad) + ": an entry must be -1 (unchanged) or a delay in [0, " +
+             std::to_string(RSB_MAX_ACTUATION_DELAY) + "] sub-steps; nothing changed";
+    };
+    rc = stage_checked(b, delays, (size_t)env_count, (size_t)env_count, where, true, 0, check, what, &staged); if (rc) return rc;
+  }
+  const int nj = b->nv - (b->model->md.floating ? 6 : 0);
+  CK(b->delay_state.ensure((size_t)b->N * 2 * 4, b->stream));
+  CK(b->delay_ring.ensure(std::max<size_t>((size_t)b->N * DELAY_SLOTS * 3 * nj, 1) * 4, b->stream));
+  if (!b->delay_active) CK(cudaMemsetAsync(b->delay_state.get(), 0, (size_t)b->N * 2 * 4, b->stream));   // delay 0, history empty
+  rsb_actuation_delay_commit_kernel<<<(unsigned)blocks, threads, 0, b->stream>>>(b->delay_state.get() + 2 * (size_t)env_begin, staged, env_count);
+  CK(cudaGetLastError());
+  b->delay_active = true;
+  return RSB_OK;
+}
+int rsb_batch_clear_actuation_delay(rsb_batch* b) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  b->delay_active = false;
+  return RSB_OK;
 }
 int rsb_batch_set_control_mode(rsb_batch* b, int mode) {
   if (!b || (mode != RSB_FORCE_AND_TORQUE && mode != RSB_PD_PLUS_FEEDFORWARD_TORQUE)) return fail(RSB_ERR_INVALID, "bad control mode");
@@ -1516,7 +1554,8 @@ int rsb_batch_gym_reset(rsb_batch* b) {
   CK(cudaSetDevice(b->device));
   int threads = 128, blocks = (b->N * 32 + threads - 1) / threads;
   rsb_gym_reset_kernel<<<blocks, threads, 0, b->stream>>>(b->gc.get(), b->gv.get(), b->pt.get(), b->vt.get(), b->gym, b->gc_stride, b->gv_stride, b->nq, b->nv, b->N,
-                                                          b->an_dofs.empty() ? nullptr : b->an_hist.get(), (int)an_hist_words(b));
+                                                          b->an_dofs.empty() ? nullptr : b->an_hist.get(), (int)an_hist_words(b),
+                                                          b->delay_active ? b->delay_state.get() : nullptr);
   CK(cudaGetLastError());
   b->kin_dirty = true;
   b->launches++;

@@ -268,6 +268,11 @@ struct StepArgs {
   int substep_barrier; // non-zero: re-align the CTA's warps of one round at every sub-step
   int pair_stage_a;    // 1: quadruped instance, CTAs that keep the sub-step barrier: one warp runs stage A of two environments
   ActNetDesc an;       // learned actuator network (stages C and E, the gym epilogue); an.params null = none
+  // actuation delay (rsb_batch_set_actuation_delay), read by the DL instances only; null = none, or a launch that does not advance the
+  // state.  delay_state [num_envs][2]: the delay d and the advancing sub-steps t since the history was emptied (actuation_delay);
+  // delay_ring [num_envs][DELAY_SLOTS][3][nv - nbase]: the command ring
+  int* delay_state;
+  float* delay_ring;
 };
 
 // ------------------------------------------------------------------ small device math ----------
@@ -844,6 +849,39 @@ __device__ __forceinline__ void actuator_network(const ActNetDesc& an, int env, 
   }
 }
 
+// Stage C: the actuation delay of environment env at one advancing sub-step.  The command of a joint dof j (nbase + j) is the triple
+// (ptarget[q], vtarget, tau_ff); it goes into ring slot t % DELAY_SLOTS, and the one of sub-step max(t - d, 0) replaces it in s_pt,
+// s_vt and s_tau, where the PD law, the actuator network and stage E read it.  At sub-step 0 of a launch the command is what the
+// prologue fetched; later sub-steps of the launch repeat it, from the slot the sub-step before wrote, since s_* then hold applied values.
+// A slot is overwritten DELAY_SLOTS sub-steps after it was written, later than any delay reads it.  t is kept in [0, 2 DELAY_SLOTS):
+// from DELAY_SLOTS on, t - d >= 0 and only t % DELAY_SLOTS matters.  Each lane touches its own ring words only, but its s_* words are
+// read by other lanes: the first __syncwarp orders the pt_store / vt_store copies of sub-step 0 (lane i reads word i) before this
+// lane's writes, the second orders every lane's read of t and of s_* before the counter and the PD law move on.
+constexpr int DELAY_SLOTS = RSB_MAX_ACTUATION_DELAY + 1;
+__device__ __forceinline__ void actuation_delay(int* state, float* rings, int env, int sub, int nbase, int nv, const int* dofq, float* s_pt,
+                                                float* s_vt, float* s_tau, int lane) {
+  __syncwarp();
+  const int nj = nv - nbase, row = 3 * nj;
+  int* const st = state + 2 * env;
+  float* const ring = rings + (size_t)env * DELAY_SLOTS * row;
+  const int2 dt = *reinterpret_cast<const int2*>(st);
+  const int d = dt.x, t = dt.y;
+  float* const cur = ring + (t % DELAY_SLOTS) * row;
+  const float* const prev = ring + ((t + DELAY_SLOTS - 1) % DELAY_SLOTS) * row;
+  const float* const app = ring + (max(t - d, 0) % DELAY_SLOTS) * row;
+#pragma unroll 1
+  for (int j = lane; j < nj; j += 32) {
+    const int i = nbase + j, q = dofq[i];
+    float p, v, f;
+    if (sub == 0) { p = s_pt[q]; v = s_vt[i]; f = s_tau[i]; }
+    else { p = prev[j]; v = prev[nj + j]; f = prev[2 * nj + j]; }
+    cur[j] = p; cur[nj + j] = v; cur[2 * nj + j] = f;
+    s_pt[q] = app[j]; s_vt[i] = app[nj + j]; s_tau[i] = app[2 * nj + j];
+  }
+  __syncwarp();
+  if (lane == 0) st[1] = t + 1 < 2 * DELAY_SLOTS ? t + 1 : t + 1 - DELAY_SLOTS;
+}
+
 // Stages C and E: kp, kd and effort limit of dof i in environment env.  The blob's value (gain: kp | kd | effort, nvp each) unless the
 // environment has a row (StepArgs::actuator) whose entry is >= 0; the gains are 0 outside PD mode (use_pd), the effort limit holds in
 // both control modes
@@ -894,8 +932,10 @@ __host__ __device__ constexpr bool operator==(const Dims& a, const Dims& b) {
   return a.nb == b.nb && a.nq == b.nq && a.nv == b.nv && a.floating == b.floating && a.maxdepth == b.maxdepth && a.maxdd == b.maxdd;
 }
 
-// AN: the instance with the actuator network (launched only while one is set and PD laws apply); without it the step is what it was
-template <int WPC, int SLOTS, int SPEC, bool AN>
+// AN: the instance with the actuator network (launched only while one is set and PD laws apply); DL: the one with actuation delays
+// (launched only while they are set, by the launches that advance the state).  Without them the step is what it was: inlined into
+// every instance, either one changed the register allocation of many of them (ptxas, CUDA 12.9; DESIGN.md §2)
+template <int WPC, int SLOTS, int SPEC, bool AN, bool DL>
 __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel(const __grid_constant__ StepArgs args) {
   extern __shared__ __align__(128) uint32_t smem[];
   __shared__ __align__(8) uint64_t tma_bar;
@@ -1021,9 +1061,10 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       for (int i = lane; i < nv; i += 32) s_gv[i] = g_gv[i];
 #pragma unroll 1
       for (int i = lane; i < nv; i += 32) s_tau[i] = args.tau ? args.tau[(size_t)env * args.gv_stride + i] : 0.f;
-      if (args.use_pd) {
+      if (args.use_pd || DL) {
         // PD targets are first needed in stage C: fetch them asynchronously (cp.async, global -> shared) so that a
-        // caller buffer in pinned host memory (zero-copy control step) is read over PCIe behind stages A and B
+        // caller buffer in pinned host memory (zero-copy control step) is read over PCIe behind stages A and B.  With an actuation
+        // delay they are fetched in force mode too: the command history records them in both control modes
         // gym task: the joint part of the position target is action * actionStd + actionMean (ENVIRONMENT::step(), first half); the base
         // part comes from the batch's own rows like every other target
         const int nfetch = args.gym_action ? 7 : nq;
@@ -1310,7 +1351,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
         __syncwarp();
       }
       const int C3 = C, CR = C3 + Lm;   // contact rows, all constraint rows
-      if (sub == 0 && args.use_pd) {     // the asynchronous target fetch of the prologue lands here
+      if (sub == 0 && (args.use_pd || DL)) {     // the asynchronous target fetch of the prologue lands here
         asm volatile("cp.async.wait_all;" ::: "memory");
         __syncwarp();
         if (args.pt_store) {
@@ -1322,6 +1363,8 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           for (int i = lane; i < nv; i += 32) args.vt_store[(size_t)env * args.gv_stride + i] = s_vt[i];
         }
       }
+      // actuation delay: the commanded rows were stored above; from here on s_pt, s_vt and s_tau hold the applied command
+      if constexpr (DL) actuation_delay(args.delay_state, args.delay_ring, env, sub, nbase, nv, dofq, s_pt, s_vt, s_tau, lane);
       // actuator network: a listed dof has no PD law and the feed-forward torque tau_ff + net, its network torque kept in s_vt (its
       // velocity target, which it does not use; reloaded by every launch) for stage E.  Scratch: the Anderson history of stage D
       if constexpr (AN) { actuator_network(args.an, env, lane, s_gc, s_gv, s_pt, dofq, s_hist, s_vt); __syncwarp(); }
@@ -1864,6 +1907,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 #pragma unroll 1
           for (int i = lane; i < hw; i += 32) args.an.hist[(size_t)env * hw + i] = 0.f;
         }
+        if (DL && lane == 0) args.delay_state[2 * env + 1] = 0;   // the command history is emptied, the delay kept
       }
       if (lane == 0) { args.gym_reward[env] = r; args.gym_done[env] = term ? 1 : 0; }
       __syncwarp();

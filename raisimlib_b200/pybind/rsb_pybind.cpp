@@ -162,6 +162,12 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void set_heightmap_index(uintptr_t map_of_env_dev, int env_begin, int env_count) {
     check(rsb_batch_set_heightmap_index(b_, reinterpret_cast<const int32_t*>(map_of_env_dev), env_begin, env_count, RSB_DEVICE), "set_heightmap_index");
   }
+  // actuation delays of environments [env_begin, env_begin + env_count) ([env_count] int32, -1: unchanged) from a device address
+  // (0: delay 0 and an empty history for the whole range)
+  void set_actuation_delay(uintptr_t delays_dev, int env_begin, int env_count) {
+    check(rsb_batch_set_actuation_delay(b_, reinterpret_cast<const int32_t*>(delays_dev), env_begin, env_count, RSB_DEVICE), "set_actuation_delay");
+  }
+  void clear_actuation_delay() { check(rsb_batch_clear_actuation_delay(b_), "clear_actuation_delay"); }
   // maps first .. first + count - 1 of the terrain overwritten with [count, ys, xs] float32 heights from a device address
   void update_heightmaps(uintptr_t heights_dev, int first, int count) {
     check(rsb_batch_update_heightmaps(b_, first, count, reinterpret_cast<const float*>(heights_dev), RSB_DEVICE), "update_heightmaps");
@@ -214,6 +220,8 @@ PYBIND11_MODULE(_rsb_py, m) {
            py::arg("cx"), py::arg("cy"), py::arg("heights"), py::arg("map_of_env"))
       .def("set_heightmap_index", &Batch::set_heightmap_index, py::arg("map_of_env_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("update_heightmaps", &Batch::update_heightmaps, py::arg("heights_dev"), py::arg("first"), py::arg("count"))
+      .def("set_actuation_delay", &Batch::set_actuation_delay, py::arg("delays_dev"), py::arg("env_begin"), py::arg("env_count"))
+      .def("clear_actuation_delay", &Batch::clear_actuation_delay)
       .def("sync", &Batch::sync)
       .def_property_readonly("num_envs", &Batch::num_envs)
       .def_property_readonly("nq", &Batch::nq)
