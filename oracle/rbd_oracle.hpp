@@ -454,46 +454,56 @@ template <typename T> class Sim {
     if (n.z < T(0)) inv = -inv;
     return inv * n;
   }
-  // cells [ix0, ix1] x [iy0, iy1] under the axis-aligned box [lo, hi], at most 3 x 3 around the cell of the centre
+  // cells [ix0, ix1] x [iy0, iy1] under the axis-aligned box [lo, hi] (all of them, clamped to the map); false: the shape's centre
+  // (cxp, cyp) is off the map, no contact
   static bool cell_range(const HmGrid& g, T lox, T hix, T loy, T hiy, T cxp, T cyp, int& ix0, int& ix1, int& iy0, int& iy1) {
     const T gx = (cxp - g.x0) / g.dx, gy = (cyp - g.y0) / g.dy;
     if (!(gx >= T(0)) || !(gy >= T(0)) || !(gx < T(g.xs - 1)) || !(gy < T(g.ys - 1))) return false;
-    const int cx = int(gx), cy = int(gy);
-    ix0 = std::max(std::max(int(std::floor((lox - g.x0) / g.dx)), cx - 1), 0); ix1 = std::min(std::min(int(std::floor((hix - g.x0) / g.dx)), cx + 1), g.xs - 2);
-    iy0 = std::max(std::max(int(std::floor((loy - g.y0) / g.dy)), cy - 1), 0); iy1 = std::min(std::min(int(std::floor((hiy - g.y0) / g.dy)), cy + 1), g.ys - 2);
+    ix0 = std::max(int(std::floor((lox - g.x0) / g.dx)), 0); ix1 = std::min(int(std::floor((hix - g.x0) / g.dx)), g.xs - 2);
+    iy0 = std::max(int(std::floor((loy - g.y0) / g.dy)), 0); iy1 = std::min(int(std::floor((hiy - g.y0) / g.dy)), g.ys - 2);
     return true;
   }
-  // sphere (centre C, radius r > 0) against the eight triangles of the 2 x 2 block of cells nearest to its centre (everything
-  // within half a cell of the centre horizontally: exact for radii up to half the grid pitch): the terrain point closest to
-  // the centre decides.  Centre above the surface (the usual case): depth = r - distance, pushed out along the line to that point
-  // (face, edge or vertex); centre under the surface (deep penetration): depth = r + distance, along that triangle's normal.
-  // Of several triangles within 1e-6 m of the smallest distance (they share the touched edge or vertex) the lowest pair index wins.
+  // sphere (centre C, radius r > 0) against the triangles under its footprint [C +- r]: the terrain point closest to the centre decides.
+  // Centre above the surface (the usual case): depth = r - distance, pushed out along the line to that point (face, edge or vertex);
+  // centre under the surface (deep penetration; inside / outside from the triangle directly beneath the centre): depth = r + distance,
+  // along that triangle's normal.  The cells are visited in 2 x 2 blocks, eight triangles per block (slot k: cell (k >> 1) & 1, k >> 2
+  // of the block, triangle k & 1; the kernel gives each slot a lane): when the footprint fits in the 2 x 2 block nearest to the centre
+  // (always for radii up to half the pitch) that block alone, else the blocks from the footprint's first cell on, in steps of two
+  // cells, iy-major.  Each slot keeps its closest triangle (a later block's only when strictly closer); of the slots within 1e-6 m of
+  // the smallest distance (they share the touched edge or vertex) the lowest pair index wins.
   void sphere_vs_heightmap(const HmGrid& g, V3<T> C, T r, Best& best) const {
     const T gx = (C.x - g.x0) / g.dx, gy = (C.y - g.y0) / g.dy;
     if (!(gx >= T(0)) || !(gy >= T(0)) || !(gx < T(g.xs - 1)) || !(gy < T(g.ys - 1))) return;
     const int ccx = int(gx), ccy = int(gy);
-    const int bx = std::min(std::max(int(std::floor(gx - T(0.5))), 0), std::max(g.xs - 3, 0)), by = std::min(std::max(int(std::floor(gy - T(0.5))), 0), std::max(g.ys - 3, 0));
+    int bx = std::min(std::max(int(std::floor(gx - T(0.5))), 0), std::max(g.xs - 3, 0)), by = std::min(std::max(int(std::floor(gy - T(0.5))), 0), std::max(g.ys - 3, 0));
+    const int fx0 = std::max(int(std::floor(gx - r / g.dx)), 0), fx1 = std::min(int(std::floor(gx + r / g.dx)), g.xs - 2);
+    const int fy0 = std::max(int(std::floor(gy - r / g.dy)), 0), fy1 = std::min(int(std::floor(gy + r / g.dy)), g.ys - 2);
+    int nbx = 1, nby = 1;
+    if (fx0 < bx || fx1 > bx + 1 || fy0 < by || fy1 > by + 1) { bx = fx0; by = fy0; nbx = (fx1 - fx0 + 2) >> 1; nby = (fy1 - fy0 + 2) >> 1; }
     T dist[8]; V3<T> vv[8], nn[8]; int pr[8]; bool ok[8];
+    for (int k = 0; k < 8; k++) ok[k] = false;
     bool inside = false; T dmin = T(3.0e38);
-    for (int k = 0; k < 8; k++) {
-      const int ix = bx + ((k >> 1) & 1), iy = by + (k >> 2), tri = k & 1;
-      ok[k] = false;
-      if (ix > g.xs - 2 || iy > g.ys - 2) continue;
-      const V3<T> a = vertex(g, ix, iy), b = tri == 0 ? vertex(g, ix + 1, iy) : vertex(g, ix + 1, iy + 1), c = tri == 0 ? vertex(g, ix + 1, iy + 1) : vertex(g, ix, iy + 1);
-      const V3<T> nt = tri_normal(a, b, c);
-      const T side = dot(C - a, nt);
-      if (ix == ccx && iy == ccy) {                            // the triangle directly beneath the centre tells inside from outside
-        const T fx = gx - T(ccx), fy = gy - T(ccy);
-        if ((fx >= fy) == (tri == 0)) inside = side < T(0);
+    for (int p = 0; p < nbx * nby; p++)
+      for (int k = 0; k < 8; k++) {
+        const int ix = bx + 2 * (p % nbx) + ((k >> 1) & 1), iy = by + 2 * (p / nbx) + (k >> 2), tri = k & 1;
+        if (ix > g.xs - 2 || iy > g.ys - 2) continue;
+        const V3<T> a = vertex(g, ix, iy), b = tri == 0 ? vertex(g, ix + 1, iy) : vertex(g, ix + 1, iy + 1), c = tri == 0 ? vertex(g, ix + 1, iy + 1) : vertex(g, ix, iy + 1);
+        const V3<T> nt = tri_normal(a, b, c);
+        const T side = dot(C - a, nt);
+        if (ix == ccx && iy == ccy) {                            // the triangle directly beneath the centre tells inside from outside
+          const T fx = gx - T(ccx), fy = gy - T(ccy);
+          if ((fx >= fy) == (tri == 0)) inside = side < T(0);
+        }
+        if (side - r > T(0)) continue;                           // the whole sphere is above this triangle's plane
+        const V3<T> Q = closest_on_triangle(C, a, b, c);
+        const V3<T> v = C - Q;
+        const T d = std::sqrt(dot(v, v));
+        if (ok[k] && !(d < dist[k])) continue;                   // the slot keeps its closest triangle
+        vv[k] = v; nn[k] = nt; dist[k] = d;
+        pr[k] = 2 * (iy * (g.xs - 1) + ix) + tri;
+        ok[k] = true;
+        dmin = std::min(dmin, d);
       }
-      if (side - r > T(0)) continue;                           // the whole sphere is above this triangle's plane
-      const V3<T> Q = closest_on_triangle(C, a, b, c);
-      vv[k] = C - Q; nn[k] = nt;
-      dist[k] = std::sqrt(dot(vv[k], vv[k]));
-      pr[k] = 2 * (iy * (g.xs - 1) + ix) + tri;
-      ok[k] = true;
-      dmin = std::min(dmin, dist[k]);
-    }
     int win = -1;
     for (int k = 0; k < 8; k++) if (ok[k] && dist[k] <= dmin + T(1e-6) && (win < 0 || pr[k] < pr[win])) win = k;
     if (win < 0) return;

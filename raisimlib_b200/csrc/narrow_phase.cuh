@@ -4,7 +4,9 @@
 // contact candidate.  Included by step_kernel.cuh inside namespace rsb, after the f3 helpers and TerrainDesc.
 //
 // Cell (ix, iy) holds two triangles split along the diagonal P00-P11: tri 0 = (P00, P10, P11), tri 1 = (P00, P11, P01);
-// pair index = 2 * cell + tri.  At most 3 x 3 cells around the cell under the candidate's centre are visited.
+// pair index = 2 * cell + tri.  Every cell under the shape's horizontal reach is visited, whatever its size against the pitch
+// (a sphere: its footprint [C +- r]; a capsule side or a box face: its axis-aligned bounding box); a shape whose centre is off the
+// map has no contact.
 #pragma once
 
 struct HmBest { bool hit; float depth; f3 n, pos; int pair; };
@@ -32,9 +34,8 @@ __device__ __forceinline__ f3 hm_tri_normal(f3 a, f3 b, f3 c) {
 __device__ __forceinline__ bool hm_cell_range(const TerrainDesc& t, float lox, float hix, float loy, float hiy, float cxp, float cyp, int& ix0, int& ix1, int& iy0, int& iy1) {
   const float gx = (cxp - t.x0) / t.dx, gy = (cyp - t.y0) / t.dy;
   if (!(gx >= 0.f) || !(gy >= 0.f) || !(gx < t.xmax) || !(gy < t.ymax)) return false;
-  const int cx = (int)gx, cy = (int)gy;
-  ix0 = max(max((int)floorf((lox - t.x0) / t.dx), cx - 1), 0); ix1 = min(min((int)floorf((hix - t.x0) / t.dx), cx + 1), t.xs - 2);
-  iy0 = max(max((int)floorf((loy - t.y0) / t.dy), cy - 1), 0); iy1 = min(min((int)floorf((hiy - t.y0) / t.dy), cy + 1), t.ys - 2);
+  ix0 = max((int)floorf((lox - t.x0) / t.dx), 0); ix1 = min((int)floorf((hix - t.x0) / t.dx), t.xs - 2);
+  iy0 = max((int)floorf((loy - t.y0) / t.dy), 0); iy1 = min((int)floorf((hiy - t.y0) / t.dy), t.ys - 2);
   return true;
 }
 // closest point of triangle (a, b, c) to p: Voronoi regions of the triangle (Ericson, Real-Time Collision Detection 5.1.5)
@@ -72,10 +73,14 @@ __device__ __forceinline__ void closest_segments(f3 p1, f3 d1, f3 p2, f3 d2, flo
   else if (t > 1.f) { t = 1.f; s = fminf(fmaxf((b - c) / a, 0.f), 1.f); }
 }
 
-// Sphere (centre C, radius r > 0) against the eight triangles of the 2 x 2 block of cells nearest to its centre (oracle
-// sphere_vs_heightmap).  EIGHT LANES share one sphere, one triangle each (sub = lane & 7: cell (sub >> 1) & 1, sub >> 2 of the block,
-// triangle sub & 1); the group reduces to the closest terrain point with xor shuffles inside its aligned 8-lane segment.  Of several
-// triangles within 1e-6 m of the smallest distance (they share the touched edge or vertex) the lowest pair index wins.
+// Sphere (centre C, radius r > 0) against the triangles under its footprint [C +- r] (oracle sphere_vs_heightmap), in 2 x 2 cell
+// blocks of eight triangles.  EIGHT LANES share one sphere, one triangle of each block each (sub = lane & 7: cell (sub >> 1) & 1,
+// sub >> 2 of the block, triangle sub & 1).  When the footprint fits in the 2 x 2 block nearest to the centre (always for radii up to
+// half the pitch) that block is the only pass; else the group steps over the blocks from the footprint's first cell on, two cells at
+// a time, iy-major, and each lane keeps its closest triangle (a later block's only when strictly closer).  The pass count is the
+// warp's largest, so the shuffles below see every lane.  The group then reduces to the closest terrain point with xor shuffles inside
+// its aligned 8-lane segment; of several lanes within 1e-6 m of the smallest distance (they share the touched edge or vertex) the
+// lowest pair index wins.
 // Every lane returns the contact ITS triangle would give (depth, normal, pair) and the lane of its group whose triangle won
 // (winner, the same in all eight lanes; -1 = no contact): the lane that owns the sphere fetches the winner's answer with shuffles.
 // `valid` = this group holds a sphere at all.
@@ -84,28 +89,38 @@ __device__ __forceinline__ SphereTri sphere_vs_heightmap_group(const TerrainDesc
   const float gx = (C.x - t.x0) * t.inv_dx, gy = (C.y - t.y0) * t.inv_dy;
   const bool in_map = valid && gx >= 0.f && gy >= 0.f && gx < t.xmax && gy < t.ymax;
   const int ccx = (int)gx, ccy = (int)gy;
-  const int bx = min(max((int)floorf(gx - 0.5f), 0), max(t.xs - 3, 0)), by = min(max((int)floorf(gy - 0.5f), 0), max(t.ys - 3, 0));
+  int bx = min(max((int)floorf(gx - 0.5f), 0), max(t.xs - 3, 0)), by = min(max((int)floorf(gy - 0.5f), 0), max(t.ys - 3, 0));
+  const int fx0 = max((int)floorf(gx - r * t.inv_dx), 0), fx1 = min((int)floorf(gx + r * t.inv_dx), t.xs - 2);
+  const int fy0 = max((int)floorf(gy - r * t.inv_dy), 0), fy1 = min((int)floorf(gy + r * t.inv_dy), t.ys - 2);
+  int nbx = 1, npass = in_map ? 1 : 0;
+  if (in_map && (fx0 < bx || fx1 > bx + 1 || fy0 < by || fy1 > by + 1)) { bx = fx0; by = fy0; nbx = (fx1 - fx0 + 2) >> 1; npass = nbx * ((fy1 - fy0 + 2) >> 1); }
   const int sub = lane & 7, tri = sub & 1;
-  const int ix = bx + ((sub >> 1) & 1), iy = by + (sub >> 2);
   float dist = 3.0e38f; f3 v = mk(0.f, 0.f, 0.f), nt = mk(0.f, 0.f, 1.f); int pair = 0x7fffffff; bool beneath_inside = false;
-  if (in_map && ix <= t.xs - 2 && iy <= t.ys - 2) {
-    const float* H = t.h + hm_offset + iy * t.xs + ix;
-    const float h00 = __ldg(H), h11 = __ldg(H + t.xs + 1), h3 = __ldg(tri == 0 ? H + 1 : H + t.xs);
-    const float X0 = t.x0 + (float)ix * t.dx, X1 = t.x0 + (float)(ix + 1) * t.dx, Y0 = t.y0 + (float)iy * t.dy, Y1 = t.y0 + (float)(iy + 1) * t.dy;
-    const f3 a = mk(X0, Y0, h00), p11 = mk(X1, Y1, h11), p3 = tri == 0 ? mk(X1, Y0, h3) : mk(X0, Y1, h3);
-    const f3 b = tri == 0 ? p3 : p11, c = tri == 0 ? p11 : p3;      // tri 0 = (P00, P10, P11), tri 1 = (P00, P11, P01)
-    nt = hm_tri_normal(a, b, c);
-    const float side = dot(C - a, nt);
-    if (ix == ccx && iy == ccy) {                               // the triangle directly beneath the centre tells inside from outside
-      const float fx = gx - (float)ccx, fy = gy - (float)ccy;
-      if ((fx >= fy) == (tri == 0)) beneath_inside = side < 0.f;
-    }
-    if (!(side - r > 0.f)) {                                    // else: the whole sphere is above this triangle's plane
-      const f3 Q = closest_on_triangle(C, a, b, c);
-      v = C - Q;
-      const float d2 = dot(v, v);
-      dist = d2 * np_rsqrt(fmaxf(d2, 1e-30f));
-      pair = 2 * (iy * (t.xs - 1) + ix) + tri;
+  const int passes = __reduce_max_sync(0xffffffffu, npass);
+  int qx = 0, qy = 0;                                           // this pass's block: (bx + 2 qx, by + 2 qy), iy-major
+#pragma unroll 1
+  for (int p = 0; p < passes; p++) {
+    const int ix = bx + 2 * qx + ((sub >> 1) & 1), iy = by + 2 * qy + (sub >> 2);
+    if (++qx == nbx) { qx = 0; qy++; }
+    if (p < npass && ix <= t.xs - 2 && iy <= t.ys - 2) {
+      const float* H = t.h + hm_offset + iy * t.xs + ix;
+      const float h00 = __ldg(H), h11 = __ldg(H + t.xs + 1), h3 = __ldg(tri == 0 ? H + 1 : H + t.xs);
+      const float X0 = t.x0 + (float)ix * t.dx, X1 = t.x0 + (float)(ix + 1) * t.dx, Y0 = t.y0 + (float)iy * t.dy, Y1 = t.y0 + (float)(iy + 1) * t.dy;
+      const f3 a = mk(X0, Y0, h00), p11 = mk(X1, Y1, h11), p3 = tri == 0 ? mk(X1, Y0, h3) : mk(X0, Y1, h3);
+      const f3 b = tri == 0 ? p3 : p11, c = tri == 0 ? p11 : p3;      // tri 0 = (P00, P10, P11), tri 1 = (P00, P11, P01)
+      const f3 ntp = hm_tri_normal(a, b, c);
+      const float side = dot(C - a, ntp);
+      if (ix == ccx && iy == ccy) {                             // the triangle directly beneath the centre tells inside from outside
+        const float fx = gx - (float)ccx, fy = gy - (float)ccy;
+        if ((fx >= fy) == (tri == 0)) beneath_inside = side < 0.f;
+      }
+      if (!(side - r > 0.f)) {                                  // else: the whole sphere is above this triangle's plane
+        const f3 Q = closest_on_triangle(C, a, b, c);
+        const f3 vp = C - Q;
+        const float d2 = dot(vp, vp);
+        const float dp = d2 * np_rsqrt(fmaxf(d2, 1e-30f));
+        if (dp < dist) { dist = dp; v = vp; nt = ntp; pair = 2 * (iy * (t.xs - 1) + ix) + tri; }   // the lane keeps its closest triangle
+      }
     }
   }
   const unsigned seg = 0xffu << (lane & 24);

@@ -868,7 +868,8 @@ def test_random_heightmap_sphere_contacts_against_brute_force_sampling():
     """Spheres on a random rough map: the oracle's contact (closest point of the 8 triangles around the centre, Voronoi-region formula)
     against brute force -- every triangle of the 5 x 5 cells around the centre sampled on a dense barycentric grid.  No sampled point
     may be closer to the centre than the oracle's closest point, and the oracle's point must be (nearly) attained by the samples:
-    independent evidence for the closest-feature routine and for the 2 x 2 cell block being enough for a radius below the pitch."""
+    independent evidence for the closest-feature routine (a radius of half the pitch: the 2 x 2 cell block nearest to the centre covers
+    the footprint; wider spheres: tests/test_terrain_contact_cpu.py)."""
     t = load_tables(SPHERE_URDF)
     o = Oracle(t)
     rng = np.random.default_rng(77)
