@@ -22,6 +22,7 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -88,40 +89,48 @@ class Contact {
   rsb_contact c_;
 };
 
-// Lock-step execution of N unmodified per-environment programs on one batch (VectorizedEnvironment<ENVIRONMENT>).
-// Every environment holds World / ArticulatedSystem VIEWS of the same BatchedWorld.  Their setters and getters work on host
-// mirrors of the batch rows, and World::integrate() only counts: the first access that needs the result (getState, getContacts,
-// setPdTarget after an integrate ...) suspends that environment until every environment has reached the same point; then the
-// dirty rows go up in one copy each, ONE launch integrates the counted sub-steps of every environment (the usual RaisimGym loop
-// `for (i < control_dt / simulation_dt) world_->integrate();` becomes a single fused launch), and the mirrors are refilled lazily,
-// one copy per array and control step.
+// Host mirror of one batch's per-environment rows: every World / ArticulatedSystem view writes its environment's row here and reads it
+// after the mirror has made it current.  Two upload policies:
+//  * immediate (a stand-alone World, a view built with World(BatchedWorld*, env)): a write goes up before the setter returns, World::
+//    integrate() launches at once, and a read fetches the reader's row alone -- per call, the C-ABI call of a per-environment accessor;
+//  * deferred (VectorizedEnvironment<ENVIRONMENT>: N unmodified per-environment programs in lock step on one batch): World::integrate()
+//    only counts.  The first access that needs the result (getState, getContacts, setPdTarget after an integrate ...) suspends that
+//    environment until every environment has reached the same point; then the rows written go up in one copy per array, ONE launch
+//    integrates the counted sub-steps of every environment (the usual RaisimGym loop `for (i < control_dt / simulation_dt)
+//    world_->integrate();` becomes a single fused launch), and reads refill every environment's rows, one copy per array and control step.
 struct LockStep {
+  // rows [n][w] of one array and the environments [lo, hi) written since the last upload
+  template <class T> struct Rows {
+    std::vector<T> v;
+    size_t w = 0;
+    int lo = 0, hi = 0;
+    void init(int n, size_t width, T fill) { w = width; v.assign(size_t(n) * w, fill); }
+    T* row(int e) { return v.data() + size_t(e) * w; }
+    bool dirty() const { return hi > lo; }
+    void mark(int e) { lo = dirty() ? std::min(lo, e) : e; hi = std::max(hi, e + 1); }
+    void clean() { lo = hi = 0; }
+  };
   rsb_batch* batch = nullptr;
-  int n = 0, nq = 0, nv = 0;
-  std::vector<float> gc, gv, pt, vt, tau, tauApplied;
-  std::vector<rsb_contact> contacts;
-  std::vector<int32_t> ncontacts;
-  std::vector<float> cfForce;               // [n][S][3], [n][S] of the contact bodies (ArticulatedSystem::setContactBodies), S = cfBodies
-  std::vector<int32_t> cfSteps;
-  int cfBodies = 0;
-  bool cfValid = false;
-  std::vector<float> bodyInertia;           // [n][nb][10] inertial rows (ArticulatedSystem::updateMassInfo); empty until the first one
-  bool bodyInertiaDirty = false;
-  int ncoll = 0;
-  std::vector<float> friction;              // [n][ncoll] terrain friction rows (World material calls; -1: the batch's value); empty until the first one
-  bool frictionDirty = false;
-  std::vector<float> actuator;              // [n][nv][3] kp, kd, effort limit (setPdGains / setActuationLimits; -1: the batch's); empty until the first one
-  bool actuatorDirty = false;
-  std::vector<float> scan, scanXy;          // [n][P], [n][P][2] heights and sample locations of the height scan (ArticulatedSystem::setHeightScan)
+  const rsb_model* model = nullptr;
+  int n = 0, nq = 0, nv = 0, nb = 0, ncoll = 0;
+  bool deferred = false;
+  // rows the views write; pt and vt (setPdTarget), gc and gv (setState) go up in one call each
+  Rows<float> gc, gv, pt, vt, tau;
+  Rows<float> bodyInertia;                  // [nb][10] inertial rows (ArticulatedSystem::updateMassInfo); empty until the first one
+  Rows<float> friction;                     // [ncoll] terrain friction (World materials; -1: the batch's value); empty until the first one
+  Rows<float> actuator;                     // [nv][3] kp, kd, effort limit (setPdGains / setActuationLimits; -1: the batch's); empty until the first one
+  Rows<int32_t> delay;                      // [1] ArticulatedSystem::setActuationDelay since the last upload (-1: unchanged); empty until the first one
+  Rows<char> actHistReset;                  // [1] ArticulatedSystem::resetActuatorHistory() since the last upload
   size_t actHistWords = 0;                  // words of one environment's actuator-network history (0: no network, or history 1)
-  std::vector<char> actHistReset;           // [n] ArticulatedSystem::resetActuatorHistory() since the last upload
-  bool actHistDirty = false;
-  std::vector<int32_t> delay;               // [n] ArticulatedSystem::setActuationDelay since the last upload (-1: unchanged); empty until the first one
-  bool delayDirty = false;
-  int scanPoints = 0;
-  bool scanValid = false;
-  // terrain of every environment (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding the same heights
-  // share one MapEntry; `atlas` is what the device holds, in atlas order (atlasSingle: one map set without an index)
+  // rows the device fills: deferred, every environment's, valid until the next launch (the height scan: until the next state write or
+  // terrain upload); immediate, the reader's row of the last read
+  Rows<float> tauApplied, cfForce, scan, scanXy;   // [nv], [S][3] and [S] of the contact bodies (setContactBodies), [P] and [P][2] of the scan
+  Rows<int32_t> ncontacts, cfSteps;
+  Rows<rsb_contact> contacts;               // [RSB_KMAX]
+  int cfBodies = 0, scanPoints = 0;
+  bool stateValid = false, tauAppliedValid = false, contactsValid = false, cfValid = false, scanValid = false;
+  // terrain of every environment of a deferred mirror (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding
+  // the same heights share one MapEntry; `atlas` is what the device holds, in atlas order (atlasSingle: one map set without an index)
   struct MapEntry {
     int xs = 0, ys = 0;
     double xSize = 0, ySize = 0, cx = 0, cy = 0;
@@ -136,14 +145,14 @@ struct LockStep {
   bool atlasSingle = false, terrainDirty = false;
   long mapUploads = 0, indexUploads = 0;    // terrain calls issued: maps uploaded (rsb_batch_set_heightmap / _heightmaps), index moves
   std::vector<int> pending;                 // World::integrate() calls not executed yet, per environment
-  bool stateValid = false, stateDirty = false, ptDirty = false, vtDirty = false, tauDirty = false, tauAppliedValid = false, contactsValid = false;
   long launches = 0;
   std::function<void(int)> suspend;         // installed by the scheduler: park the calling environment until the batch was flushed
 
-  void init(rsb_batch* b, int n_, int nq_, int nv_) {
-    batch = b; n = n_; nq = nq_; nv = nv_;
-    gc.assign(size_t(n) * nq, 0.f); gv.assign(size_t(n) * nv, 0.f); pt.assign(size_t(n) * nq, 0.f); vt.assign(size_t(n) * nv, 0.f);
-    tau.assign(size_t(n) * nv, 0.f); tauApplied.assign(size_t(n) * nv, 0.f); contacts.resize(size_t(n) * RSB_KMAX); ncontacts.assign(n, 0);
+  void init(rsb_batch* b, const rsb_model* m, int n_) {
+    batch = b; model = m; n = n_;
+    rsbCheck(rsb_model_dims(m, &nq, &nv, &nb, &ncoll, nullptr), "dims");
+    gc.init(n, nq, 0.f); gv.init(n, nv, 0.f); pt.init(n, nq, 0.f); vt.init(n, nv, 0.f); tau.init(n, nv, 0.f);
+    tauApplied.init(n, nv, 0.f); contacts.init(n, RSB_KMAX, rsb_contact{}); ncontacts.init(n, 1, 0);
     pending.assign(n, 0);
     envMap.assign(n, nullptr); envGround.assign(n, 0);
   }
@@ -153,107 +162,145 @@ struct LockStep {
     if (!suspend) throw std::runtime_error("World: state access with integrate() calls pending outside VectorizedEnvironment::step()");
     suspend(env);
   }
-  void needState() {
-    if (stateValid) return;
-    rsbCheck(rsb_batch_get_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "getState");
-    stateValid = true;
+
+  // ---- writes: environment env's row of an array, marked for the next upload; commit() after filling it ----
+  template <class T> T* write(int env, Rows<T>& a) { sync(env); a.mark(env); return a.row(env); }
+  template <class T> T* write(int env, Rows<T>& a, size_t width, T fill) {   // an array kept empty until its first write
+    if (a.v.empty()) a.init(n, width, fill);
+    return write(env, a);
   }
-  void needTauApplied() {
-    if (tauAppliedValid) return;
-    rsbCheck(rsb_batch_get_generalized_force(batch, tauApplied.data(), 0, n, RSB_HOST), "getGeneralizedForce");
-    tauAppliedValid = true;
+  // gc or gv: a deferred upload spans every row between the lowest and the highest environment written, so the mirror must hold the
+  // other environments' rows first; a written state also makes the height scan stale
+  float* stateRow(int env, Rows<float>& a) {
+    sync(env);
+    if (deferred) needState(env);
+    scanValid = false;
+    return write(env, a);
   }
-  void needContacts() {
-    if (contactsValid) return;
-    rsbCheck(rsb_batch_get_contacts(batch, contacts.data(), ncontacts.data(), 0, n, RSB_HOST), "getContacts");
-    contactsValid = true;
+  float* inertiaRow(int env) {               // every environment starts from the model's rows
+    if (bodyInertia.v.empty()) {
+      rsb_model_tables t; rsbCheck(rsb_model_get_tables(model, &t), "getTables");
+      bodyInertia.init(n, size_t(nb) * 10, 0.f);
+      for (int e = 0; e < n; e++)
+        for (int b = 0; b < nb; b++) {
+          float* r = bodyInertia.row(e) + size_t(b) * 10;
+          r[0] = float(t.mass[b]);
+          for (int k = 0; k < 3; k++) r[1 + k] = float(t.com[3 * b + k]);
+          for (int k = 0; k < 6; k++) r[4 + k] = float(t.inertia[6 * b + k]);
+        }
+    }
+    return write(env, bodyInertia);
   }
-  void needContactForces() {
-    if (cfValid) return;
-    cfForce.resize(size_t(n) * cfBodies * 3); cfSteps.resize(size_t(n) * cfBodies);
-    rsbCheck(rsb_batch_get_body_contact_forces(batch, 0, n, cfForce.data(), cfSteps.data(), RSB_HOST), "getBodyContactForce");
-    cfValid = true;
+  float* actuatorRow(int env) { return write(env, actuator, size_t(nv) * 3, -1.f); }
+  void setFriction(int env, size_t collisionBody, double mu) {
+    if (collisionBody >= size_t(ncoll)) throw std::runtime_error("setCollisionBodyFriction: collision body index out of range");
+    write(env, friction, size_t(ncoll), -1.f)[collisionBody] = float(mu);
+    commit();
   }
-  // the height scan of every environment in one call, after the rows written since the last launch went up (a reset() that moved a
-  // robot is seen); valid until the next flush() or state write
-  void needHeightScan() {
+  // environment env's actuator-network history goes to zero, its actuation delay is set (and its command history emptied)
+  void resetActuatorHistory(int env) { *write(env, actHistReset, 1, char(0)) = 1; commit(); }
+  void setActuationDelay(int env, int subSteps) { *write(env, delay, 1, int32_t(-1)) = subSteps; commit(); }
+  // the rows written go up now, unless uploads wait for the next launch or device read
+  void commit() { if (!deferred) pushWrites(); }
+
+  // ---- uploads ----
+  template <class T, class F> void push(Rows<T>& a, F call) {
+    if (!a.dirty()) return;
+    call(a.row(a.lo), a.lo, a.hi - a.lo);
+    a.clean();
+  }
+  // two arrays one call sets: both over the union of their ranges, one nobody wrote as nullptr
+  template <class F> void push(Rows<float>& a, Rows<float>& b, F call) {
+    if (!a.dirty() && !b.dirty()) return;
+    const int lo = !a.dirty() ? b.lo : !b.dirty() ? a.lo : std::min(a.lo, b.lo), hi = std::max(a.hi, b.hi);
+    call(a.dirty() ? a.row(lo) : nullptr, b.dirty() ? b.row(lo) : nullptr, lo, hi - lo);
+    a.clean(); b.clean();
+  }
+  // every row written since the last upload, one call per array over the environments written
+  void pushWrites() {
+    push(gc, gv, [&](float* q, float* v, int lo, int k) { rsbCheck(rsb_batch_set_state(batch, q, v, lo, k, RSB_HOST), "setState"); });
+    push(pt, vt, [&](float* p, float* v, int lo, int k) { rsbCheck(rsb_batch_set_pd_target(batch, p, v, lo, k, RSB_HOST), "setPdTarget"); });
+    push(tau, [&](float* r, int lo, int k) { rsbCheck(rsb_batch_set_generalized_force(batch, r, lo, k, RSB_HOST), "setGeneralizedForce"); });
+    push(bodyInertia, [&](float* r, int lo, int k) { rsbCheck(rsb_batch_set_body_inertia(batch, r, lo, k, RSB_HOST), "updateMassInfo"); });
+    push(friction, [&](float* r, int lo, int k) { rsbCheck(rsb_batch_set_contact_friction(batch, r, lo, k, RSB_HOST), "setMaterialPairProp"); });
+    push(actuator, [&](float* r, int lo, int k) { rsbCheck(rsb_batch_set_actuator_params(batch, r, lo, k, RSB_HOST), "setPdGains"); });
+    pushTerrain();
+    // the marked environments' history rows zeroed: one call when every environment of the range was marked, else one get and one set
+    push(actHistReset, [&](char* m, int lo, int k) {
+      if (actHistWords > 0 && std::all_of(m, m + k, [](char c) { return c != 0; })) {
+        rsbCheck(rsb_batch_set_actuator_history(batch, nullptr, lo, k, RSB_HOST), "resetActuatorHistory");
+      } else if (actHistWords > 0) {
+        std::vector<float> h(size_t(k) * actHistWords);
+        rsbCheck(rsb_batch_get_actuator_history(batch, h.data(), lo, k, RSB_HOST), "resetActuatorHistory");
+        for (int e = 0; e < k; e++)
+          if (m[e]) std::fill(h.begin() + size_t(e) * actHistWords, h.begin() + size_t(e + 1) * actHistWords, 0.f);
+        rsbCheck(rsb_batch_set_actuator_history(batch, h.data(), lo, k, RSB_HOST), "resetActuatorHistory");
+      }
+      std::fill(m, m + k, 0);
+    });
+    push(delay, [&](int32_t* d, int lo, int k) {
+      rsbCheck(rsb_batch_set_actuation_delay(batch, d, lo, k, RSB_HOST), "setActuationDelay");
+      std::fill(d, d + k, -1);
+    });
+  }
+  // upload, then one launch of k sub-steps for every environment
+  void launch(int k) {
     pushWrites();
-    if (scanValid) return;
-    scan.resize(size_t(n) * scanPoints); scanXy.resize(size_t(n) * scanPoints * 2);
-    rsbCheck(rsb_batch_get_height_scan(batch, 0, n, scan.data(), scanXy.data(), RSB_HOST), "getHeightScan");
-    scanValid = true;
+    rsbCheck(rsb_batch_integrate(batch, k), "integrate");
+    launches++;
+    for (int& p : pending) p = 0;
+    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = false;
   }
-  // every environment is parked (or finished) with the same number of integrate() calls pending: upload, one launch, invalidate
+  // every environment is parked (or finished) with the same number of integrate() calls pending
   void flush() {
     int k = 0;
     for (int e = 0; e < n; e++) k = pending[e] > k ? pending[e] : k;
     if (k == 0) return;
     for (int e = 0; e < n; e++)
       if (pending[e] != k) throw std::runtime_error("VectorizedEnvironment: environments disagree on the number of World::integrate() calls between two state accesses");
-    if (stateDirty) rsbCheck(rsb_batch_set_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "setState");
-    if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
-    if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
-    if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
-    if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
-    if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
-    pushTerrain();
-    pushActuatorHistory();
-    pushActuationDelay();
-    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
-    rsbCheck(rsb_batch_integrate(batch, k), "integrate");
-    launches++;
-    for (int& p : pending) p = 0;
-    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = false;
+    launch(k);
   }
-  // rows written outside a step (reset(), init()): push them before anything else reads the device
-  void pushWrites() {
-    if (stateDirty) { rsbCheck(rsb_batch_set_state(batch, gc.data(), gv.data(), 0, n, RSB_HOST), "setState"); scanValid = false; }
-    if (ptDirty || vtDirty) rsbCheck(rsb_batch_set_pd_target(batch, ptDirty ? pt.data() : nullptr, vtDirty ? vt.data() : nullptr, 0, n, RSB_HOST), "setPdTarget");
-    if (tauDirty) rsbCheck(rsb_batch_set_generalized_force(batch, tau.data(), 0, n, RSB_HOST), "setGeneralizedForce");
-    if (bodyInertiaDirty) rsbCheck(rsb_batch_set_body_inertia(batch, bodyInertia.data(), 0, n, RSB_HOST), "updateMassInfo");
-    if (frictionDirty) rsbCheck(rsb_batch_set_contact_friction(batch, friction.data(), 0, n, RSB_HOST), "setMaterialPairProp");
-    if (actuatorDirty) rsbCheck(rsb_batch_set_actuator_params(batch, actuator.data(), 0, n, RSB_HOST), "setPdGains");
-    pushTerrain();
-    pushActuatorHistory();
-    pushActuationDelay();
-    stateDirty = ptDirty = vtDirty = tauDirty = bodyInertiaDirty = frictionDirty = actuatorDirty = false;
-  }
-  // environment env's actuator-network history goes to zero before the next launch (ArticulatedSystem::resetActuatorHistory)
-  void resetActuatorHistory(int env) {
+
+  // ---- reads ----
+  // The gate of every read the device computes from the current state and parameters (M, h, poses, the height scan, the solver's loop
+  // counter): whatever env integrated has happened and every row written since is up
+  void current(int env) { sync(env); pushWrites(); }
+  // rows of the last launch's results, and the state: fetch(lo, count, all) refills rows [lo, lo + count), all of what the mirror keeps
+  // (all) or what the reader asked for.  The mirror holds every write to them, so they need no upload
+  template <class F> void refill(int env, bool& valid, F fetch) {
     sync(env);
-    if (actHistReset.empty()) actHistReset.assign(n, 0);
-    actHistReset[env] = 1;
-    actHistDirty = true;
+    if (valid) return;
+    if (deferred) { fetch(0, n, true); valid = true; }
+    else fetch(env, 1, false);
   }
-  // environment env's actuation delay, set (and its command history emptied) before the next launch
-  void setActuationDelay(int env, int subSteps) {
-    sync(env);
-    if (delay.empty()) delay.assign(n, -1);
-    delay[env] = subSteps;
-    delayDirty = true;
+  void needState(int env) {
+    refill(env, stateValid, [&](int lo, int k, bool) { rsbCheck(rsb_batch_get_state(batch, gc.row(lo), gv.row(lo), lo, k, RSB_HOST), "getState"); });
   }
-  // the delays set since the last upload in one call, only when some environment set one; the other entries are -1 (unchanged)
-  void pushActuationDelay() {
-    if (!delayDirty) return;
-    delayDirty = false;
-    rsbCheck(rsb_batch_set_actuation_delay(batch, delay.data(), 0, n, RSB_HOST), "setActuationDelay");
-    std::fill(delay.begin(), delay.end(), -1);
+  void needTauApplied(int env) {
+    refill(env, tauAppliedValid, [&](int lo, int k, bool) { rsbCheck(rsb_batch_get_generalized_force(batch, tauApplied.row(lo), lo, k, RSB_HOST), "getGeneralizedForce"); });
   }
-  // the marked environments' history rows zeroed: one get and one set of all rows, only when some environment reset
-  void pushActuatorHistory() {
-    if (!actHistDirty) return;
-    actHistDirty = false;
-    if (actHistWords > 0) {
-      std::vector<float> h(size_t(n) * actHistWords);
-      rsbCheck(rsb_batch_get_actuator_history(batch, h.data(), 0, n, RSB_HOST), "resetActuatorHistory");
-      for (int e = 0; e < n; e++)
-        if (actHistReset[e]) std::fill(h.begin() + size_t(e) * actHistWords, h.begin() + size_t(e + 1) * actHistWords, 0.f);
-      rsbCheck(rsb_batch_set_actuator_history(batch, h.data(), 0, n, RSB_HOST), "resetActuatorHistory");
-    }
-    std::fill(actHistReset.begin(), actHistReset.end(), 0);
+  void needContacts(int env) {
+    refill(env, contactsValid, [&](int lo, int k, bool) { rsbCheck(rsb_batch_get_contacts(batch, contacts.row(lo), ncontacts.row(lo), lo, k, RSB_HOST), "getContacts"); });
   }
-  // environment env's height map (World::addHeightMap), uploaded with the next flush() or pushWrites(): environments holding the same
-  // heights share one entry, found by a hash and confirmed by comparison
+  void needContactForces(int env, bool force, bool steps) {
+    if (cfForce.w != size_t(cfBodies) * 3) { cfForce.init(n, size_t(cfBodies) * 3, 0.f); cfSteps.init(n, size_t(cfBodies), 0); cfValid = false; }
+    refill(env, cfValid, [&](int lo, int k, bool all) {
+      rsbCheck(rsb_batch_get_body_contact_forces(batch, lo, k, all || force ? cfForce.row(lo) : nullptr, all || steps ? cfSteps.row(lo) : nullptr, RSB_HOST),
+               "getBodyContactForce");
+    });
+  }
+  // deferred: one call scans every environment, after the rows written since the last launch went up (a reset() that moved a robot is seen)
+  void needHeightScan(int env, bool samples) {
+    current(env);
+    if (scan.w != size_t(scanPoints)) { scan.init(n, size_t(scanPoints), 0.f); scanXy.init(n, size_t(scanPoints) * 2, 0.f); scanValid = false; }
+    refill(env, scanValid, [&](int lo, int k, bool all) {
+      rsbCheck(rsb_batch_get_height_scan(batch, lo, k, scan.row(lo), all || samples ? scanXy.row(lo) : nullptr, RSB_HOST), "getHeightScan");
+    });
+  }
+
+  // ---- terrain of a deferred mirror ----
+  // environment env's height map (World::addHeightMap), uploaded with the next launch or read: environments holding the same heights
+  // share one entry, found by a hash and confirmed by comparison
   void setHeightMap(int env, int xs, int ys, double xSize, double ySize, double cx, double cy, std::vector<float> h) {
     sync(env);
     auto e = std::make_shared<MapEntry>();
@@ -341,21 +388,6 @@ struct LockStep {
     terrainDirty = false;
     scanValid = false;
   }
-  // environment env's terrain friction of one collision body, uploaded with the next flush() or pushWrites() (no launch of its own)
-  void setFriction(int env, size_t collisionBody, double mu) {
-    if (collisionBody >= size_t(ncoll)) throw std::runtime_error("setCollisionBodyFriction: collision body index out of range");
-    sync(env);
-    if (friction.empty()) friction.assign(size_t(n) * ncoll, -1.f);
-    friction[size_t(env) * ncoll + collisionBody] = float(mu);
-    frictionDirty = true;
-  }
-  // environment env's actuator row [nv][3] (batch gv order), written by the caller and uploaded with the next flush() or pushWrites()
-  float* actuatorRow(int env) {
-    sync(env);
-    if (actuator.empty()) actuator.assign(size_t(n) * nv * 3, -1.f);
-    actuatorDirty = true;
-    return &actuator[size_t(env) * nv * 3];
-  }
 };
 
 // One GPU batch of N identical worlds (new; the reference has no equivalent -- its batching is the
@@ -367,6 +399,7 @@ class BatchedWorld {
     rsbCheck(rsb_batch_create(model_, numEnvs, device, &batch_), "BatchedWorld");
     rsbCheck(rsb_model_dims(model_, &nq_, &nv_, &nb_, nullptr, nullptr), "dims");
     n_ = numEnvs;
+    ls_.init(batch_, model_, n_);
   }
   ~BatchedWorld() { if (batch_) rsb_batch_destroy(batch_); if (model_) rsb_model_destroy(model_); }
   BatchedWorld(const BatchedWorld&) = delete;
@@ -384,12 +417,68 @@ class BatchedWorld {
   void integrate2() { rsbCheck(rsb_batch_integrate2(batch_), "integrate2"); worldTime_ += params().dt; }
   double worldTime() const { return worldTime_; }
   void advanceTime(double t) { worldTime_ += t; }
-  // lock-step mode (VectorizedEnvironment<ENVIRONMENT>): per-environment views work on host mirrors, integrate() is deferred
-  LockStep* lockStep() { return ls_.get(); }
-  void enableLockStep() {
-    if (ls_) return;
-    ls_.reset(new LockStep); ls_->init(batch_, n_, nq_, nv_); ls_->cfBodies = int(contactBodies_.size()); ls_->scanPoints = int(scanBodies_.size());
-    rsbCheck(rsb_model_dims(model_, nullptr, nullptr, nullptr, &ls_->ncoll, nullptr), "dims");
+  // the host mirror every view reads and writes through; lock-step mode (VectorizedEnvironment<ENVIRONMENT>) defers its uploads
+  LockStep* lockStep() { return &ls_; }
+  void enableLockStep() { ls_.deferred = true; }
+  // World::integrate() of environment env: deferred, one more sub-step for the next launch (the world time follows environment 0);
+  // immediate, one launch now.  Returns whether it launched
+  bool integrateEnv(int env) {
+    if (ls_.deferred) {
+      ls_.pending[env]++;
+      if (env == 0) advanceTime(params().dt);
+      return false;
+    }
+    ls_.launch(1);
+    advanceTime(params().dt);
+    return true;
+  }
+  // ---- what a stand-alone World sets for its batch and a VectorizedEnvironment per environment ----
+  // PD gains in the batch's gv order: a stand-alone World's are its batch's; in a VectorizedEnvironment each environment's are its own,
+  // kept in its actuator row and uploaded before the next launch (no launch of their own), as upstream's per-World gains are
+  void setPdGains(int env, const std::vector<float>& kp, const std::vector<float>& kd) {
+    if (!ls_.deferred) { rsbCheck(rsb_batch_set_pd_gains(batch_, kp.data(), kd.data()), "setPdGains"); return; }
+    float* r = ls_.actuatorRow(env);
+    for (int i = 0; i < nv_; i++) { r[3 * i] = kp[size_t(i)]; r[3 * i + 1] = kd[size_t(i)]; }
+  }
+  // friction of one collision body against the terrain (mu < 0: the default material): a stand-alone World sets it for its batch; in a
+  // VectorizedEnvironment it is environment env's own, kept in its friction row and uploaded with the next launch
+  // (include/rsb.h rsb_batch_set_contact_friction)
+  void setCollisionFriction(int env, size_t collisionBody, double mu) {
+    if (ls_.deferred) ls_.setFriction(env, collisionBody, mu);
+    else rsbCheck(rsb_batch_set_collision_friction(batch_, int(collisionBody), float(mu)), "setCollisionBodyFriction");
+  }
+  // World's materials of environment env: pairMu holds each collision body with a material and the friction of its pair with the
+  // terrain's material (none: no such pair), defaultMu the environment's setDefaultMaterial friction (< 0: not set).  A stand-alone World
+  // sets the friction of those bodies for its batch (-1 without a pair); in a VectorizedEnvironment they fill environment env's whole
+  // friction row, the default where a body has no pair
+  void setMaterialFriction(int env, const std::map<size_t, std::optional<double>>& pairMu, double defaultMu) {
+    if (!ls_.deferred) {
+      for (const auto& kv : pairMu) setCollisionFriction(env, kv.first, kv.second ? *kv.second : -1.0);
+      return;
+    }
+    if (ls_.friction.v.empty() && pairMu.empty() && defaultMu < 0) return;   // every entry -1: no rows needed
+    for (int c = 0; c < ls_.ncoll; c++) {
+      auto m = pairMu.find(size_t(c));
+      setCollisionFriction(env, size_t(c), m != pairMu.end() && m->second ? *m->second : defaultMu);
+    }
+  }
+  // setDefaultMaterial: restitution is the batch's.  The friction is rsb_params.mu for a stand-alone World, which self-collision pairs
+  // use too; in a VectorizedEnvironment it is environment env's own, through its friction row, and self pairs keep the batch's mu
+  void setDefaultMaterial(int env, double friction, double restitution, double resThreshold, const std::map<size_t, std::optional<double>>& pairMu) {
+    rsb_params p = params(); p.restitution = float(restitution); p.rest_threshold = float(resThreshold);
+    if (!ls_.deferred) p.mu = float(friction);
+    setParams(p);
+    if (ls_.deferred) setMaterialFriction(env, pairMu, friction);
+  }
+  // terrain: a stand-alone World, or a view, sets it for the whole batch at once; in a VectorizedEnvironment each environment's map is
+  // its own, uploaded with the next launch or read (LockStep::pushTerrain), and a ground is set at once
+  void setHeightMap(int env, int xs, int ys, double xSize, double ySize, double cx, double cy, const std::vector<float>& h) {
+    if (ls_.deferred) ls_.setHeightMap(env, xs, ys, xSize, ySize, cx, cy, h);
+    else rsbCheck(rsb_batch_set_heightmap(batch_, xs, ys, float(xSize), float(ySize), float(cx), float(cy), h.data()), "addHeightMap");
+  }
+  void setGround(int env, double z) {
+    if (ls_.deferred) ls_.setGround(env);
+    rsbCheck(rsb_batch_set_ground(batch_, float(z)), "addGround");
   }
   // bodies whose contact force every integrate() gathers (ArticulatedSystem::setContactBodies): one list for all environments
   void setContactBodies(const std::vector<size_t>& bodies) {
@@ -397,7 +486,7 @@ class BatchedWorld {
     std::vector<int32_t> b(bodies.begin(), bodies.end());
     rsbCheck(rsb_batch_set_contact_bodies(batch_, b.data(), int(b.size())), "setContactBodies");
     contactBodies_ = bodies;
-    if (ls_) { ls_->cfBodies = int(bodies.size()); ls_->cfValid = false; }
+    ls_.cfBodies = int(bodies.size()); ls_.cfValid = false;
   }
   size_t contactBodySlot(size_t bodyIdx) const {
     for (size_t s = 0; s < contactBodies_.size(); s++) if (contactBodies_[s] == bodyIdx) return s;
@@ -410,7 +499,7 @@ class BatchedWorld {
     if (xy.size() != 2 * bodies.size()) throw std::runtime_error("setHeightScan: one offset per body");
     rsbCheck(rsb_batch_set_height_scan(batch_, bodies.data(), xy.data(), int(bodies.size()), yawAligned ? RSB_SCAN_YAW : RSB_SCAN_WORLD), "setHeightScan");
     scanBodies_ = bodies; scanXy_ = xy; scanYaw_ = yawAligned;
-    if (ls_) { ls_->scanPoints = int(bodies.size()); ls_->scanValid = false; }
+    ls_.scanPoints = int(bodies.size()); ls_.scanValid = false;
   }
   size_t numHeightScanPoints() const { return scanBodies_.size(); }
   // the learned actuator network (ArticulatedSystem::setActuatorNetwork): one for the batch.  Setting it zeroes every history, so a
@@ -425,24 +514,22 @@ class BatchedWorld {
     }
     rsbCheck(rsb_batch_set_actuator_network(batch_, dofs.data(), int(dofs.size()), history, layers, width, params.data()), "setActuatorNetwork");
     anDofs_ = dofs; anH_ = history; anL_ = layers; anW_ = width; anParams_ = params;
-    if (ls_) { ls_->actHistWords = dofs.empty() ? 0 : dofs.size() * 2 * size_t(history - 1); ls_->actHistDirty = false; ls_->actHistReset.clear(); }
+    ls_.actHistWords = dofs.empty() ? 0 : dofs.size() * 2 * size_t(history - 1); ls_.actHistReset = {};
   }
-  // zero environment env's actuator history: at once in a stand-alone World, before the next launch in a VectorizedEnvironment
-  void resetActuatorHistory(int env) {
-    if (ls_) { ls_->resetActuatorHistory(env); return; }
-    if (!anDofs_.empty()) rsbCheck(rsb_batch_set_actuator_history(batch_, nullptr, env, 1, RSB_HOST), "resetActuatorHistory");
-  }
-  // environment env's actuation delay in sub-steps (ArticulatedSystem::setActuationDelay): at once in a stand-alone World, before the
-  // next launch in a VectorizedEnvironment
-  void setActuationDelay(int env, int subSteps) {
-    if (ls_) { ls_->setActuationDelay(env, subSteps); return; }
-    const int32_t d = subSteps;
-    rsbCheck(rsb_batch_set_actuation_delay(batch_, &d, env, 1, RSB_HOST), "setActuationDelay");
+  // zero environment env's actuator history, and set its actuation delay in sub-steps (ArticulatedSystem::setActuationDelay)
+  void resetActuatorHistory(int env) { ls_.resetActuatorHistory(env); }
+  void setActuationDelay(int env, int subSteps) { ls_.setActuationDelay(env, subSteps); }
+  // getContactSolver().getLoopCounter() of environment env
+  int solverIterations(int env) {
+    ls_.current(env);
+    int32_t it = 0;
+    rsbCheck(rsb_batch_get_solver_iterations(batch_, &it, env, 1, RSB_HOST), "getLoopCounter");
+    return it;
   }
   const std::string& urdf() const { return urdf_; }
   void rememberUrdf(const std::string& u) { urdf_ = u; }
  private:
-  std::unique_ptr<LockStep> ls_;
+  LockStep ls_;
   std::vector<size_t> contactBodies_;
   std::vector<int32_t> scanBodies_;
   std::vector<float> scanXy_;
@@ -520,18 +607,17 @@ struct TerrainProperties {
 // raisim::ArticulatedSystem -- a view of one environment's robot
 class ArticulatedSystem {
  public:
-  ArticulatedSystem(BatchedWorld* w, int env) : w_(w), env_(env) {}
+  ArticulatedSystem(BatchedWorld* w, int env) : w_(w), m_(*w->lockStep()), env_(env) { setJointOrder({}); }
   // upstream addArticulatedSystem(urdf, resDir, jointOrder): the order of the joints in gc / gv as the caller wants it.  The batch keeps
   // its depth-first order; this view permutes on the way in and out (base coordinates first, as always).
   void setJointOrder(const std::vector<std::string>& jointOrder) {
-    qmap_.clear(); vmap_.clear();
+    qmap_.resize(size_t(w_->nq())); vmap_.resize(size_t(w_->nv()));
+    for (size_t i = 0; i < qmap_.size(); i++) qmap_[i] = int(i);
+    for (size_t i = 0; i < vmap_.size(); i++) vmap_[i] = int(i);
     if (jointOrder.empty()) return;
     rsb_model_tables t; rsbCheck(rsb_model_get_tables(w_->model(), &t), "getTables");
     const int nj = t.nb - 1, q0 = t.floating ? 7 : 0, v0 = t.floating ? 6 : 0;
     if (int(jointOrder.size()) != nj) throw std::runtime_error("addArticulatedSystem: jointOrder must name every movable joint exactly once");
-    qmap_.resize(size_t(t.nq)); vmap_.resize(size_t(t.nv));
-    for (int i = 0; i < q0; i++) qmap_[i] = i;
-    for (int i = 0; i < v0; i++) vmap_[i] = i;
     std::vector<bool> seen(size_t(t.nb), false);
     for (int k = 0; k < nj; k++) {
       int body = -1;
@@ -546,92 +632,28 @@ class ArticulatedSystem {
   void setName(const std::string& n) { name_ = n; }
   const std::string& getName() const { return name_; }
 
+  // State, targets and forces go through this environment's rows of the batch's host mirror (LockStep), permuted between the caller's
+  // joint order and the batch's by fromBatch / toBatch
   void getState(VecDyn& gc, VecDyn& gv) const {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needState();
-      gc.resize(size_t(ls->nq)); gv.resize(size_t(ls->nv));
-      for (int i = 0; i < ls->nq; i++) gc[i] = ls->gc[size_t(env_) * ls->nq + qi(i)];
-      for (int i = 0; i < ls->nv; i++) gv[i] = ls->gv[size_t(env_) * ls->nv + vi(i)];
-      return;
-    }
-    std::vector<float> q(w_->nq()), v(w_->nv());
-    rsbCheck(rsb_batch_get_state(w_->batch(), q.data(), v.data(), env_, 1, RSB_HOST), "getState");
-    gc.resize(q.size()); gv.resize(v.size());
-    for (size_t i = 0; i < q.size(); i++) gc[i] = q[qi(i)];
-    for (size_t i = 0; i < v.size(); i++) gv[i] = v[vi(i)];
+    m_.needState(env_);
+    gc = fromBatch(m_.gc.row(env_), qmap_); gv = fromBatch(m_.gv.row(env_), vmap_);
   }
   VecDyn getGeneralizedCoordinate() const { VecDyn q, v; getState(q, v); return q; }
   VecDyn getGeneralizedVelocity() const { VecDyn q, v; getState(q, v); return v; }
   template <class VQ, class VV> void setState(const VQ& gc, const VV& gv) {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needState();           // the other environments' rows of the mirror must be current before the whole array goes up
-      for (int i = 0; i < ls->nq; i++) ls->gc[size_t(env_) * ls->nq + qi(i)] = float(gc[i]);
-      for (int i = 0; i < ls->nv; i++) ls->gv[size_t(env_) * ls->nv + vi(i)] = float(gv[i]);
-      ls->stateDirty = true;
-      return;
-    }
-    std::vector<float> q(w_->nq()), v(w_->nv());
-    for (size_t i = 0; i < q.size(); i++) q[qi(i)] = float(gc[i]);
-    for (size_t i = 0; i < v.size(); i++) v[vi(i)] = float(gv[i]);
-    rsbCheck(rsb_batch_set_state(w_->batch(), q.data(), v.data(), env_, 1, RSB_HOST), "setState");
+    toBatch(gc, qmap_, m_.stateRow(env_, m_.gc)); toBatch(gv, vmap_, m_.stateRow(env_, m_.gv)); m_.commit();
   }
-  template <class VQ> void setGeneralizedCoordinate(const VQ& gc) {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needState();
-      for (int i = 0; i < ls->nq; i++) ls->gc[size_t(env_) * ls->nq + qi(i)] = float(gc[i]);
-      ls->stateDirty = true;
-      return;
-    }
-    std::vector<float> q(w_->nq());
-    for (size_t i = 0; i < q.size(); i++) q[qi(i)] = float(gc[i]);
-    rsbCheck(rsb_batch_set_state(w_->batch(), q.data(), nullptr, env_, 1, RSB_HOST), "setGeneralizedCoordinate");
-  }
-  template <class VV> void setGeneralizedVelocity(const VV& gv) {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needState();
-      for (int i = 0; i < ls->nv; i++) ls->gv[size_t(env_) * ls->nv + vi(i)] = float(gv[i]);
-      ls->stateDirty = true;
-      return;
-    }
-    std::vector<float> v(w_->nv());
-    for (size_t i = 0; i < v.size(); i++) v[vi(i)] = float(gv[i]);
-    rsbCheck(rsb_batch_set_state(w_->batch(), nullptr, v.data(), env_, 1, RSB_HOST), "setGeneralizedVelocity");
-  }
-  template <class VV> void setGeneralizedForce(const VV& tau) {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_);
-      for (int i = 0; i < ls->nv; i++) ls->tau[size_t(env_) * ls->nv + vi(i)] = float(tau[i]);
-      ls->tauDirty = true;
-      return;
-    }
-    std::vector<float> t(w_->nv());
-    for (size_t i = 0; i < t.size(); i++) t[vi(i)] = float(tau[i]);
-    rsbCheck(rsb_batch_set_generalized_force(w_->batch(), t.data(), env_, 1, RSB_HOST), "setGeneralizedForce");
-  }
-  // A stand-alone World sets the gains of its batch.  In a VectorizedEnvironment they are this environment's own: they go to its
-  // actuator row of the host mirror and up before the next launch (no launch of their own), as upstream's per-World gains do.
+  template <class VQ> void setGeneralizedCoordinate(const VQ& gc) { toBatch(gc, qmap_, m_.stateRow(env_, m_.gc)); m_.commit(); }
+  template <class VV> void setGeneralizedVelocity(const VV& gv) { toBatch(gv, vmap_, m_.stateRow(env_, m_.gv)); m_.commit(); }
+  template <class VV> void setGeneralizedForce(const VV& tau) { toBatch(tau, vmap_, m_.write(env_, m_.tau)); m_.commit(); }
+  // A stand-alone World sets the gains of its batch; in a VectorizedEnvironment they are this environment's own (BatchedWorld::setPdGains)
   template <class VV> void setPdGains(const VV& p, const VV& d) {
-    if (LockStep* ls = w_->lockStep()) {
-      float* r = ls->actuatorRow(env_);
-      for (int i = 0; i < ls->nv; i++) { r[3 * vi(i)] = float(p[i]); r[3 * vi(i) + 1] = float(d[i]); }
-      return;
-    }
-    std::vector<float> kp(w_->nv()), kd(w_->nv());
-    for (size_t i = 0; i < kp.size(); i++) { kp[vi(i)] = float(p[i]); kd[vi(i)] = float(d[i]); }
-    rsbCheck(rsb_batch_set_pd_gains(w_->batch(), kp.data(), kd.data()), "setPdGains");
+    std::vector<float> kp(size_t(w_->nv())), kd(size_t(w_->nv()));
+    toBatch(p, vmap_, kp.data()); toBatch(d, vmap_, kd.data());
+    w_->setPdGains(env_, kp, kd);
   }
   template <class VQ, class VV> void setPdTarget(const VQ& posTarget, const VV& velTarget) {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_);
-      for (int i = 0; i < ls->nq; i++) ls->pt[size_t(env_) * ls->nq + qi(i)] = float(posTarget[i]);
-      for (int i = 0; i < ls->nv; i++) ls->vt[size_t(env_) * ls->nv + vi(i)] = float(velTarget[i]);
-      ls->ptDirty = ls->vtDirty = true;
-      return;
-    }
-    std::vector<float> q(w_->nq()), v(w_->nv());
-    for (size_t i = 0; i < q.size(); i++) q[qi(i)] = float(posTarget[i]);
-    for (size_t i = 0; i < v.size(); i++) v[vi(i)] = float(velTarget[i]);
-    rsbCheck(rsb_batch_set_pd_target(w_->batch(), q.data(), v.data(), env_, 1, RSB_HOST), "setPdTarget");
+    toBatch(posTarget, qmap_, m_.write(env_, m_.pt)); toBatch(velTarget, vmap_, m_.write(env_, m_.vt)); m_.commit();
   }
   void setControlMode(ControlMode::Type m) { rsbCheck(rsb_batch_set_control_mode(w_->batch(), int(m)), "setControlMode"); }
 
@@ -639,6 +661,7 @@ class ArticulatedSystem {
   MatDyn getMassMatrix() const {
     const int nv = w_->nv();
     std::vector<float> m(size_t(nv) * nv);
+    m_.current(env_);
     rsbCheck(rsb_batch_get_mass_matrix(w_->batch(), env_, 1, m.data(), RSB_HOST), "getMassMatrix");
     MatDyn M; M.resize(nv, nv);
     for (int i = 0; i < nv; i++) for (int j = 0; j < nv; j++) M(i, j) = m[vi(size_t(i)) * size_t(nv) + vi(size_t(j))];   // the caller's dof order (jointOrder)
@@ -670,19 +693,7 @@ class ArticulatedSystem {
     }
     return Minv;
   }
-  VecDyn getGeneralizedForce() const {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needTauApplied();
-      VecDyn r(size_t(ls->nv));
-      for (int i = 0; i < ls->nv; i++) r[i] = ls->tauApplied[size_t(env_) * ls->nv + vi(i)];
-      return r;
-    }
-    std::vector<float> t(w_->nv());
-    rsbCheck(rsb_batch_get_generalized_force(w_->batch(), t.data(), env_, 1, RSB_HOST), "getGeneralizedForce");
-    VecDyn r(t.size());
-    for (size_t i = 0; i < t.size(); i++) r[i] = t[vi(i)];
-    return r;
-  }
+  VecDyn getGeneralizedForce() const { m_.needTauApplied(env_); return fromBatch(m_.tauApplied.row(env_), vmap_); }
   // upstream: setExternalForce(localIdx, force) acts at the body COM, setExternalForce(localIdx, pos_in_body, force) at a
   // point fixed in the body, setExternalTorque(localIdx, torque); world frame, valid for the next integrate() only.
   // One wrench (force + torque on the same body) per environment.
@@ -723,12 +734,9 @@ class ArticulatedSystem {
   bool materialsDirty() const { return materialsDirty_; }
   void materialsApplied() { materialsDirty_ = false; }
   // friction of one collision body against the terrain (upstream: getCollisionBody(name).setMaterial + setMaterialPairProp); mu < 0:
-  // the default material.  A stand-alone World sets it for its batch; in a VectorizedEnvironment it is this environment's own, kept in
-  // the host mirror's friction row and uploaded with the next launch (include/rsb.h rsb_batch_set_contact_friction)
-  void setCollisionBodyFriction(size_t collisionBodyIdx, double mu) {
-    if (LockStep* ls = w_->lockStep()) { ls->setFriction(env_, collisionBodyIdx, mu); return; }
-    rsbCheck(rsb_batch_set_collision_friction(w_->batch(), int(collisionBodyIdx), float(mu)), "setCollisionBodyFriction");
-  }
+  // the default material.  A stand-alone World sets it for its batch; in a VectorizedEnvironment it is this environment's own
+  // (BatchedWorld::setCollisionFriction)
+  void setCollisionBodyFriction(size_t collisionBodyIdx, double mu) { w_->setCollisionFriction(env_, collisionBodyIdx, mu); }
   // Self-collision.  Upstream checks the bodies of an articulated system against each other and user code switches single pairs off
   // with ignoreCollisionBetween; here self-collision is OFF until explicit pairs of collision bodies are enabled ("LINK/k" names as in
   // getCollisionBody; at most RSB_MAX_SELF_PAIRS; sphere / capsule pairs and sphere-box), optionally each with its own friction.  The
@@ -760,10 +768,9 @@ class ArticulatedSystem {
   size_t getNumberOfSelfCollisionPairs() const { return selfMu_.size(); }
   VecDyn getNonlinearities() const {
     std::vector<float> h(w_->nv());
+    m_.current(env_);
     rsbCheck(rsb_batch_get_nonlinearities(w_->batch(), env_, 1, h.data(), RSB_HOST), "getNonlinearities");
-    VecDyn r(h.size());
-    for (size_t i = 0; i < h.size(); i++) r[i] = h[vi(i)];
-    return r;
+    return fromBatch(h.data(), vmap_);
   }
   size_t getBodyIdx(const std::string& name) const {
     int i = rsb_model_body_index(w_->model(), name.c_str());
@@ -776,9 +783,9 @@ class ArticulatedSystem {
     return size_t(i);
   }
   void getPosition(size_t bodyIdx, const Vec<3>& pointInBody, Vec<3>& out) const {
-    std::vector<float> R(size_t(w_->nb()) * 9), p(size_t(w_->nb()) * 3);
-    rsbCheck(rsb_batch_get_body_poses(w_->batch(), env_, 1, R.data(), p.data(), RSB_HOST), "getPosition");
-    for (int r = 0; r < 3; r++) out[r] = p[bodyIdx * 3 + r] + R[bodyIdx * 9 + 3 * r] * pointInBody[0] + R[bodyIdx * 9 + 3 * r + 1] * pointInBody[1] + R[bodyIdx * 9 + 3 * r + 2] * pointInBody[2];
+    const Poses P = poses();
+    const float* R = &P.R[bodyIdx * 9]; const float* p = &P.p[bodyIdx * 3];
+    for (int r = 0; r < 3; r++) out[r] = p[r] + R[3 * r] * pointInBody[0] + R[3 * r + 1] * pointInBody[1] + R[3 * r + 2] * pointInBody[2];
   }
   // ---- kinematic getters (host algebra on body poses the kernel computes for the current state) ----
   // upstream: getBodyPosition/Orientation, getFramePosition/Orientation/Velocity/AngularVelocity,
@@ -855,41 +862,22 @@ class ArticulatedSystem {
   // Upstream's idiom for changing a robot's inertial parameters: edit getMass()[i], getBodyCOM_B()[i] (body frame) and getInertia()[i]
   // (about the centre of mass, body frame; symmetric), then updateMassInfo().  The vectors are this environment's editable copy,
   // filled from the model on first use.  updateMassInfo() makes them the parameters this environment integrates: a stand-alone World
-  // uploads them at once; in a VectorizedEnvironment they go to the host mirror and up before the next launch (no launch of their
-  // own).  The batch refuses a copy that is not finite, has a negative mass or an inertia that is not positive semidefinite
+  // uploads them at once; in a VectorizedEnvironment they go up before the next launch (no launch of their own).  The batch refuses a copy that is not finite, has a negative mass or an inertia that is not positive semidefinite
   // (include/rsb.h) when it arrives: at once stand-alone, at the upload in a VectorizedEnvironment.
   std::vector<double>& getMass() { initMassInfo(); return mass_; }
   std::vector<Vec<3>>& getBodyCOM_B() { initMassInfo(); return com_; }
   std::vector<Mat<3, 3>>& getInertia() { initMassInfo(); return inertia_; }
   void updateMassInfo() {
     initMassInfo();
-    const size_t nb = mass_.size();
-    std::vector<float> row(nb * 10);
-    for (size_t b = 0; b < nb; b++) {
+    float* row = m_.inertiaRow(env_);
+    for (size_t b = 0; b < mass_.size(); b++) {
       float* r = &row[b * 10];
       const Mat<3, 3>& I = inertia_[b];
       r[0] = float(mass_[b]);
       for (size_t k = 0; k < 3; k++) r[1 + k] = float(com_[b][k]);
       r[4] = float(I(0, 0)); r[5] = float(I(0, 1)); r[6] = float(I(0, 2)); r[7] = float(I(1, 1)); r[8] = float(I(1, 2)); r[9] = float(I(2, 2));
     }
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_);
-      if (ls->bodyInertia.empty()) {             // every environment starts from the model's rows
-        std::vector<float> model(nb * 10);
-        const rsb_model_tables t = tables();
-        for (size_t b = 0; b < nb; b++) {
-          model[b * 10] = float(t.mass[b]);
-          for (size_t k = 0; k < 3; k++) model[b * 10 + 1 + k] = float(t.com[3 * b + k]);
-          for (size_t k = 0; k < 6; k++) model[b * 10 + 4 + k] = float(t.inertia[6 * b + k]);
-        }
-        ls->bodyInertia.resize(size_t(ls->n) * nb * 10);
-        for (int e = 0; e < ls->n; e++) std::copy(model.begin(), model.end(), ls->bodyInertia.begin() + size_t(e) * nb * 10);
-      }
-      std::copy(row.begin(), row.end(), ls->bodyInertia.begin() + size_t(env_) * nb * 10);
-      ls->bodyInertiaDirty = true;
-    } else {
-      rsbCheck(rsb_batch_set_body_inertia(w_->batch(), row.data(), env_, 1, RSB_HOST), "updateMassInfo");
-    }
+    m_.commit();
     appliedMass_ = mass_; appliedCom_ = com_;
   }
   std::vector<Vec<3>> getBodyCOM_W() const {
@@ -983,19 +971,16 @@ class ArticulatedSystem {
   }
   // This environment's actuator effort limits, per generalized velocity index: the commanded torque (feed-forward + PD) saturates at
   // +-upper.  The step saturates symmetrically, so lower must be -upper with upper >= 0 (+inf: no limit); anything else fails loudly.
-  // The base dofs of a floating robot are not actuated and their entries are ignored.  A stand-alone World uploads the limits at once;
-  // in a VectorizedEnvironment they go to this environment's actuator row of the host mirror and up before the next launch.
+  // The base dofs of a floating robot are not actuated and their entries are ignored.  They go to this environment's actuator row: up
+  // at once from a stand-alone World, before the next launch in a VectorizedEnvironment.
   template <class VV> void setActuationLimits(const VV& upper, const VV& lower) {
     const int nv = w_->nv();
     for (int i = 0; i < nv; i++)
       if (!(upper[i] >= 0.0) || !(lower[i] == -upper[i]))
         throw std::runtime_error("setActuationLimits: dof " + std::to_string(i) + ": only symmetric limits (lower = -upper, upper >= 0) are implemented by the batched step");
-    float* r = nullptr;
-    std::vector<float> own;
-    if (LockStep* ls = w_->lockStep()) r = ls->actuatorRow(env_);
-    else { own.assign(size_t(nv) * 3, -1.f); r = own.data(); }       // gains -1: the batch's (setPdGains)
+    float* r = m_.actuatorRow(env_);      // gains -1 until this environment sets its own: the batch's
     for (int i = 0; i < nv; i++) r[3 * vi(i) + 2] = float(upper[i]);
-    if (!w_->lockStep()) rsbCheck(rsb_batch_set_actuator_params(w_->batch(), own.data(), env_, 1, RSB_HOST), "setActuationLimits");
+    m_.commit();
     effort_.assign(size_t(nv), 0.0);
     for (int i = 0; i < nv; i++) effort_[size_t(i)] = upper[i];
   }
@@ -1006,16 +991,9 @@ class ArticulatedSystem {
   }
 
   std::vector<Contact>& getContacts() {
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needContacts();
-      contacts_.clear();
-      for (int i = 0; i < ls->ncontacts[env_]; i++) contacts_.emplace_back(ls->contacts[size_t(env_) * RSB_KMAX + i]);
-      return contacts_;
-    }
-    rsb_contact c[RSB_KMAX]; int32_t n = 0;
-    rsbCheck(rsb_batch_get_contacts(w_->batch(), c, &n, env_, 1, RSB_HOST), "getContacts");
+    m_.needContacts(env_);
     contacts_.clear();
-    for (int i = 0; i < n; i++) contacts_.emplace_back(c[i]);
+    for (int i = 0; i < *m_.ncontacts.row(env_); i++) contacts_.emplace_back(m_.contacts.row(env_)[i]);
     return contacts_;
   }
   // ---- Extensions upstream does not have.  Under upstream an ENVIRONMENT calls World::integrate() once per simulation step and sees
@@ -1027,26 +1005,15 @@ class ArticulatedSystem {
   // mean contact force on the body [N, world frame] over the integrate() calls since the last state access (the fused launch); over
   // the one step of a stand-alone integrate()
   void getBodyContactForce(size_t bodyIdx, Vec<3>& out) {
-    const size_t S = w_->numContactBodies(), s = w_->contactBodySlot(bodyIdx);
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needContactForces();
-      for (int k = 0; k < 3; k++) out[k] = ls->cfForce[(size_t(env_) * S + s) * 3 + k];
-      return;
-    }
-    std::vector<float> f(S * 3);
-    rsbCheck(rsb_batch_get_body_contact_forces(w_->batch(), env_, 1, f.data(), nullptr, RSB_HOST), "getBodyContactForce");
-    for (int k = 0; k < 3; k++) out[k] = f[s * 3 + k];
+    const size_t s = w_->contactBodySlot(bodyIdx);
+    m_.needContactForces(env_, true, false);
+    for (int k = 0; k < 3; k++) out[k] = m_.cfForce.row(env_)[s * 3 + k];
   }
   // the number of those integrate() calls in which the body had a contact (> 0: it touched something during the control step)
   int getBodyContactSteps(size_t bodyIdx) {
-    const size_t S = w_->numContactBodies(), s = w_->contactBodySlot(bodyIdx);
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needContactForces();
-      return ls->cfSteps[size_t(env_) * S + s];
-    }
-    std::vector<int32_t> n(S);
-    rsbCheck(rsb_batch_get_body_contact_forces(w_->batch(), env_, 1, nullptr, n.data(), RSB_HOST), "getBodyContactSteps");
-    return n[s];
+    const size_t s = w_->contactBodySlot(bodyIdx);
+    m_.needContactForces(env_, false, true);
+    return m_.cfSteps.row(env_)[s];
   }
   // setHeightScan: terrain height samples at horizontal offsets (x, y) from bodies (getBodyIdx order, at most RSB_MAX_SCAN_POINTS),
   // turned with each body's heading (yawAligned) or along the world axes: what an upstream observe() builds with one
@@ -1082,16 +1049,8 @@ class ArticulatedSystem {
   void getHeightScan(VecDyn& heights, std::vector<Vec<2>>* samples = nullptr) {
     const size_t P = w_->numHeightScanPoints();
     if (P == 0) throw std::runtime_error("getHeightScan: call setHeightScan() first");
-    const float *h, *xy;
-    std::vector<float> own;
-    if (LockStep* ls = w_->lockStep()) {
-      ls->sync(env_); ls->needHeightScan();
-      h = &ls->scan[size_t(env_) * P]; xy = &ls->scanXy[size_t(env_) * P * 2];
-    } else {
-      own.resize(3 * P);
-      rsbCheck(rsb_batch_get_height_scan(w_->batch(), env_, 1, own.data(), samples ? own.data() + P : nullptr, RSB_HOST), "getHeightScan");
-      h = own.data(); xy = own.data() + P;
-    }
+    m_.needHeightScan(env_, samples != nullptr);
+    const float *h = m_.scan.row(env_), *xy = m_.scanXy.row(env_);
     heights.resize(P);
     for (size_t i = 0; i < P; i++) heights[i] = h[i];
     if (samples) {
@@ -1120,7 +1079,7 @@ class ArticulatedSystem {
   struct FrameW { int body; Vec<3> pos; Mat<3, 3> rot; };
   Poses poses() const {
     Poses P; P.R.resize(size_t(w_->nb()) * 9); P.p.resize(size_t(w_->nb()) * 3);
-    if (LockStep* ls = w_->lockStep()) { ls->sync(env_); ls->pushWrites(); }
+    m_.current(env_);
     // the C-ABI getter is lazy: it runs a kinematics-only pass when the state changed (upstream's updateKinematics()); the contact
     // records and impulses of the last integrate() stay valid across kinematic getters, as upstream's getContacts() does
     rsbCheck(rsb_batch_get_body_poses(w_->batch(), env_, 1, P.R.data(), P.p.data(), RSB_HOST), "getBodyPoses");
@@ -1166,10 +1125,18 @@ class ArticulatedSystem {
     VecDyn gv = getGeneralizedVelocity();
     for (int r = 0; r < 3; r++) { double s = 0; for (size_t c = 0; c < J.cols(); c++) s += J(r, c) * gv[c]; out[r] = s; }
   }
-  size_t qi(size_t i) const { return qmap_.empty() ? i : size_t(qmap_[i]); }     // caller's coordinate index -> the batch's
-  size_t vi(size_t i) const { return vmap_.empty() ? i : size_t(vmap_[i]); }
+  size_t qi(size_t i) const { return size_t(qmap_[i]); }     // caller's coordinate index -> the batch's
+  size_t vi(size_t i) const { return size_t(vmap_[i]); }
+  // a row in the batch's order from the caller's values (map: qmap_ or vmap_), and back
+  template <class V> static void toBatch(const V& x, const std::vector<int>& map, float* row) {
+    for (size_t i = 0; i < map.size(); i++) row[map[i]] = float(x[i]);
+  }
+  static VecDyn fromBatch(const float* row, const std::vector<int>& map) {
+    VecDyn x(map.size());
+    for (size_t i = 0; i < map.size(); i++) x[i] = row[map[i]];
+    return x;
+  }
   size_t vinv(size_t batchIdx) const {                                            // the batch's velocity index -> the caller's
-    if (vmap_.empty()) return batchIdx;
     for (size_t i = 0; i < vmap_.size(); i++) if (size_t(vmap_[i]) == batchIdx) return i;
     return batchIdx;
   }
@@ -1203,6 +1170,7 @@ class ArticulatedSystem {
   std::vector<double> effort_;                        // the last setActuationLimits() upper limits in the caller's order (empty: the URDF's)
   std::vector<int> qmap_, vmap_;
   BatchedWorld* w_;
+  LockStep& m_;
   int env_;
   std::string name_;
   std::vector<Contact> contacts_;
@@ -1234,21 +1202,15 @@ class World {
         ctx_->batch->enableLockStep();
       } else if (ctx_->batch->urdf() != urdfPathOrXml) throw std::runtime_error("VectorizedEnvironment: every environment must load the same robot description");
       w_ = ctx_->batch.get();
-      rsb_params p = w_->params();
-      p.dt = float(dt_); p.gravity[0] = float(g_[0]); p.gravity[1] = float(g_[1]); p.gravity[2] = float(g_[2]);
-      w_->setParams(p);
-      if (haveGround_) setGround();
-      robot_.reset(new ArticulatedSystem(w_, env_));
-      robot_->setJointOrder(jointOrder);
-      return robot_.get();
+    } else {
+      owned_.reset(new BatchedWorld(urdfPathOrXml, 1));
+      w_ = owned_.get(); env_ = 0;
     }
-    owned_.reset(new BatchedWorld(urdfPathOrXml, 1));
-    w_ = owned_.get(); env_ = 0;
     rsb_params p = w_->params();
     p.dt = float(dt_); p.gravity[0] = float(g_[0]); p.gravity[1] = float(g_[1]); p.gravity[2] = float(g_[2]);
     w_->setParams(p);
-    if (haveGround_) rsbCheck(rsb_batch_set_ground(w_->batch(), float(groundZ_)), "addGround");
-    robot_.reset(new ArticulatedSystem(w_, 0));
+    if (haveGround_) setGround();
+    robot_.reset(new ArticulatedSystem(w_, env_));
     robot_->setJointOrder(jointOrder);
     return robot_.get();
   }
@@ -1303,9 +1265,8 @@ class World {
   // In a VectorizedEnvironment the friction is this environment's own: every collision body without a material pair of its own takes it
   // (through the environment's friction row); restitution, and the default friction of self-collision pairs, stay batch-wide
   void setDefaultMaterial(double friction, double restitution, double resThreshold) {
-    need(); rsb_params p = w_->params(); p.restitution = float(restitution); p.rest_threshold = float(resThreshold);
-    if (w_->lockStep()) { w_->setParams(p); defaultFriction_ = friction; if (robot_) applyMaterials(true); return; }
-    p.mu = float(friction); w_->setParams(p);
+    need(); defaultFriction_ = friction;
+    w_->setDefaultMaterial(env_, friction, restitution, resThreshold, materialFriction());
   }
   // named material pairs: friction of (collision-body material, terrain material); restitution is global (setDefaultMaterial)
   void setMaterialPairProp(const std::string& m1, const std::string& m2, double friction, double /*restitution*/ = 0, double /*resThreshold*/ = 0) {
@@ -1314,7 +1275,7 @@ class World {
   }
   struct ContactSolverView {            // World::getContactSolver().getLoopCounter()
     const World* w;
-    int getLoopCounter() const { int32_t it = 0; rsbCheck(rsb_batch_get_solver_iterations(w->w_->batch(), &it, w->env_, 1, RSB_HOST), "getLoopCounter"); return it; }
+    int getLoopCounter() const { return w->w_->solverIterations(w->env_); }
   };
   ContactSolverView getContactSolver() const { need(); return ContactSolverView{this}; }
   ArticulatedSystem* getObject(const std::string& name) { return (robot_ && robot_->getName() == name) ? robot_.get() : nullptr; }
@@ -1324,14 +1285,8 @@ class World {
   // one World::integrate() of THIS environment's batch.  Views of a shared batch must not call this
   // per environment -- the vectorized wrapper steps the whole batch once (see VectorizedEnvironment.hpp).
   void integrate() {
-    need();
-    if (LockStep* ls = w_->lockStep()) {   // deferred: counted now, executed for every environment at once when the result is first needed
-      applyMaterials(false);
-      ls->pending[env_]++;
-      if (env_ == 0) w_->advanceTime(w_->params().dt);
-      return;
-    }
-    applyMaterials(false); w_->integrate(1); if (robot_) robot_->clearExternalWrench();
+    need(); applyMaterials(false);
+    if (w_->integrateEnv(env_)) robot_->clearExternalWrench();
   }
   void integrate1() { need(); applyMaterials(false); w_->integrate1(); }
   void integrate2() { need(); w_->integrate2(); if (robot_) robot_->clearExternalWrench(); }
@@ -1340,41 +1295,27 @@ class World {
   BatchedWorld* batched() { return w_; }
  private:
   void need() const { if (!w_) throw std::runtime_error("World: call addArticulatedSystem() first (the batch is created with the robot)"); }
-  // the terrain of this environment: in a VectorizedEnvironment its own map goes to the LockStep mirror, which uploads the maps of all
-  // environments before the next launch, getter or scan; a stand-alone World sets it at once.  hm_ holds the float32 heights the batch
-  // collides with, so HeightMap::getHeight answers for them
+  // the terrain of this environment (BatchedWorld::setHeightMap).  hm_ holds the float32 heights the batch collides with, so
+  // HeightMap::getHeight answers for them
   HeightMap* useHeightMap(int xs, int ys, double xSize, double ySize, double cx, double cy, std::vector<float> h) {
-    if (LockStep* ls = w_->lockStep()) ls->setHeightMap(env_, xs, ys, xSize, ySize, cx, cy, h);
-    else rsbCheck(rsb_batch_set_heightmap(w_->batch(), xs, ys, float(xSize), float(ySize), float(cx), float(cy), h.data()), "addHeightMap");
+    w_->setHeightMap(env_, xs, ys, xSize, ySize, cx, cy, h);
     hm_.set(size_t(xs), size_t(ys), xSize, ySize, cx, cy, std::vector<double>(h.begin(), h.end()));
     return &hm_;
   }
-  void setGround() {
-    if (LockStep* ls = w_->lockStep()) ls->setGround(env_);
-    rsbCheck(rsb_batch_set_ground(w_->batch(), float(groundZ_)), "addGround");
-  }
-  void applyMaterials(bool force) {
-    if (!robot_ || (!force && !robot_->materialsDirty())) return;
-    if (LockStep* ls = w_->lockStep()) {   // this environment's whole row: its pair friction, else its default friction (< 0: the batch's)
-      if (ls->friction.empty() && robot_->collisionMaterials().empty() && defaultFriction_ < 0) return;   // every entry -1: no rows needed
-      for (int c = 0; c < ls->ncoll; c++) {
-        auto m = robot_->collisionMaterials().find(size_t(c));
-        double mu = defaultFriction_;
-        if (m != robot_->collisionMaterials().end()) {
-          const std::string& a = m->second; const std::string& b = terrainMaterial_;
-          auto it = pairFriction_.find(a < b ? std::make_pair(a, b) : std::make_pair(b, a));
-          if (it != pairFriction_.end()) mu = it->second;
-        }
-        robot_->setCollisionBodyFriction(size_t(c), mu);
-      }
-      robot_->materialsApplied();
-      return;
-    }
+  void setGround() { w_->setGround(env_, groundZ_); }
+  // the robot's collision bodies with a material -> the friction of their pair with the terrain's material (none: no such pair)
+  std::map<size_t, std::optional<double>> materialFriction() const {
+    std::map<size_t, std::optional<double>> mu;
     for (const auto& kv : robot_->collisionMaterials()) {
       const std::string& a = kv.second; const std::string& b = terrainMaterial_;
       auto it = pairFriction_.find(a < b ? std::make_pair(a, b) : std::make_pair(b, a));
-      robot_->setCollisionBodyFriction(kv.first, it == pairFriction_.end() ? -1.0 : it->second);   // < 0: default material
+      mu[kv.first] = it == pairFriction_.end() ? std::nullopt : std::optional<double>(it->second);
     }
+    return mu;
+  }
+  void applyMaterials(bool force) {
+    if (!robot_ || (!force && !robot_->materialsDirty())) return;
+    w_->setMaterialFriction(env_, materialFriction(), defaultFriction_);
     robot_->materialsApplied();
   }
   std::map<std::pair<std::string, std::string>, double> pairFriction_;

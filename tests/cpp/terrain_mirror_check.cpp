@@ -27,14 +27,14 @@ static void put(LockStep& ls, int env, int k) { ls.setHeightMap(env, XS, YS, SX,
 // every environment's scan against the level it should collide with
 static bool collides(LockStep& ls, const std::vector<int>& want) {
   ls.scanValid = false;
-  ls.needHeightScan();
+  ls.needHeightScan(0, true);
   for (int e = 0; e < ls.n; e++) {
     const std::vector<float> h = level(want[size_t(e)]);
     raisim::HeightMap hm;
     hm.set(XS, YS, SX, SY, CX, CY, std::vector<double>(h.begin(), h.end()));
     for (int p = 0; p < ls.scanPoints; p++) {
       const size_t i = size_t(e) * ls.scanPoints + p;
-      if (!(std::fabs(ls.scan[i] - hm.getHeight(ls.scanXy[2 * i], ls.scanXy[2 * i + 1])) <= 1e-4)) return false;
+      if (!(std::fabs(ls.scan.v[i] - hm.getHeight(ls.scanXy.v[2 * i], ls.scanXy.v[2 * i + 1])) <= 1e-4)) return false;
     }
   }
   return true;
@@ -47,9 +47,7 @@ int main(int argc, char** argv) {
   bw.enableLockStep();
   LockStep& ls = *bw.lockStep();
   bw.setHeightScan({0, 0, 0}, {0.3f, 0.2f, -1.1f, 0.7f, 2.5f, -1.9f}, false);
-  ls.needState();
-  for (int e = 0; e < n; e++) ls.gc[size_t(e) * ls.nq] = float(0.5 * e);   // base x: the environments sample different places
-  ls.stateDirty = true;
+  for (int e = 0; e < n; e++) ls.stateRow(e, ls.gc)[0] = float(0.5 * e);   // base x: the environments sample different places
 
   // environments without terrain of their own share the lowest-numbered environment's map: one common map is one plain upload
   put(ls, 1, 0); put(ls, 3, 0);
