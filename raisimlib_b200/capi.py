@@ -8,7 +8,10 @@ import os
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("RSB_LIB_PATH") or os.path.join(_HERE, "librsb.so")   # RSB_LIB_PATH: another build of the same library (A/B probes in tools/)
+# RSB_LIB_PATH loads another build of the library instead, such as the parent commit's in an A/B cost comparison
+# (tools/feature_cost.py --parent-lib); calls that build does not export are left unbound
+_OTHER_BUILD = os.environ.get("RSB_LIB_PATH")
+LIB_PATH = _OTHER_BUILD or os.path.join(_HERE, "librsb.so")
 KMAX = 8
 HOST, DEVICE = 0, 1
 FORCE_AND_TORQUE, PD_PLUS_FEEDFORWARD_TORQUE = 0, 1
@@ -91,26 +94,102 @@ class DeviceView(C.Structure):
                 [(n, C.c_void_p) for n in ("gc", "gv", "tau_ff", "ptarget", "vtarget", "ncontacts", "contacts")])
 
 
-EXPORTED = [
-    "rsb_last_error", "rsb_version", "rsb_params_default",
-    "rsb_model_create_from_urdf", "rsb_model_destroy", "rsb_model_save", "rsb_model_load", "rsb_model_dims", "rsb_model_get_tables", "rsb_model_body_index",
-    "rsb_model_body_name", "rsb_model_collision_index", "rsb_model_joint_name", "rsb_model_frame_index", "rsb_model_frame",
-    "rsb_batch_create", "rsb_batch_destroy", "rsb_batch_set_stream", "rsb_batch_sync", "rsb_batch_num_envs",
-    "rsb_batch_set_ground", "rsb_batch_set_heightmap", "rsb_batch_set_heightmaps", "rsb_batch_set_heightmap_index", "rsb_batch_update_heightmaps", "rsb_batch_clear_terrain", "rsb_batch_set_params", "rsb_batch_get_params",
-    "rsb_batch_set_collision_friction", "rsb_batch_set_self_collision",
-    "rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_gains", "rsb_batch_set_pd_target",
-    "rsb_batch_set_generalized_force", "rsb_batch_set_external_wrench", "rsb_batch_set_body_inertia", "rsb_batch_clear_body_inertia", "rsb_batch_set_contact_friction", "rsb_batch_clear_contact_friction", "rsb_batch_set_actuator_params", "rsb_batch_clear_actuator_params", "rsb_batch_set_actuator_network", "rsb_batch_set_actuator_history", "rsb_batch_get_actuator_history", "rsb_batch_set_actuation_delay", "rsb_batch_clear_actuation_delay", "rsb_batch_set_control_mode", "rsb_batch_get_generalized_force", "rsb_batch_bind_pd_target",
-    "rsb_batch_integrate1", "rsb_batch_integrate2", "rsb_batch_integrate",
-    "rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities", "rsb_batch_get_body_poses", "rsb_batch_get_contacts",
-    "rsb_batch_get_contact_points", "rsb_batch_get_solver_iterations", "rsb_batch_get_diverged", "rsb_batch_get_solver_residual", "rsb_batch_get_solver_status", "rsb_batch_update_kinematics", "rsb_batch_device_ptrs", "rsb_batch_launch_count",
-    "rsb_batch_set_frames", "rsb_batch_get_frame_states", "rsb_batch_get_frame_jacobians",
-    "rsb_batch_set_contact_bodies", "rsb_batch_get_body_contact_forces",
-    "rsb_batch_set_height_scan", "rsb_batch_get_height_scan",
-    "rsb_batch_ob_dim", "rsb_batch_observe", "rsb_batch_control_step",
-    "rsb_batch_gym_configure", "rsb_batch_gym_reset", "rsb_batch_gym_step",
-    "rsb_peer_buffer_create", "rsb_peer_buffer_open", "rsb_peer_buffer_close", "rsb_peer_buffer_destroy", "rsb_batch_set_observation_peers", "rsb_batch_wait_observation_peers",
-    "rsb_comm_init", "rsb_comm_allgather_obs", "rsb_comm_destroy", "rsb_terrain_generate", "rsb_heightmap_read_text", "rsb_heightmap_read_png",
-]
+_P, _I, _F, _S = C.c_void_p, C.c_int, C.c_float, C.c_char_p
+
+# Every function include/rsb.h declares: symbol -> argtypes, or (argtypes, restype) where it does not return int
+SIGNATURES = {
+    "rsb_last_error": ([], _S),
+    "rsb_version": [],
+    "rsb_params_default": [C.POINTER(Params)],
+    "rsb_model_create_from_urdf": [_S, C.POINTER(_P)],
+    "rsb_model_load": [_S, _P],
+    "rsb_model_save": [_P, _S],
+    "rsb_model_collision_index": [_P, _S],
+    "rsb_model_destroy": [_P],
+    "rsb_model_dims": [_P] + [C.POINTER(_I)] * 5,
+    "rsb_model_get_tables": [_P, C.POINTER(ModelTables)],
+    "rsb_model_body_index": [_P, _S],
+    "rsb_model_body_name": ([_P, _I], _S),
+    "rsb_model_joint_name": ([_P, _I], _S),
+    "rsb_model_frame_index": [_P, _S],
+    "rsb_model_frame": [_P, _I, C.POINTER(_I), _P, _P],
+    "rsb_batch_create": [_P, _I, _I, C.POINTER(_P)],
+    "rsb_batch_destroy": [_P],
+    "rsb_batch_set_stream": [_P, _P],
+    "rsb_batch_sync": [_P],
+    "rsb_batch_num_envs": [_P],
+    "rsb_batch_set_ground": [_P, _F],
+    "rsb_batch_set_heightmap": [_P, _I, _I, _F, _F, _F, _F, _P],
+    "rsb_batch_set_heightmaps": [_P, _I, _I, _I, _F, _F, _F, _F, _P, _P],
+    "rsb_batch_set_heightmap_index": [_P, _P, _I, _I, _I],
+    "rsb_batch_update_heightmaps": [_P, _I, _I, _P, _I],
+    "rsb_batch_clear_terrain": [_P],
+    "rsb_batch_set_collision_friction": [_P, _I, _F],
+    "rsb_batch_set_self_collision": [_P, _P, _I, _P],
+    "rsb_batch_set_params": [_P, C.POINTER(Params)],
+    "rsb_batch_get_params": [_P, C.POINTER(Params)],
+    "rsb_batch_set_state": [_P, _P, _P, _I, _I, _I],
+    "rsb_batch_get_state": [_P, _P, _P, _I, _I, _I],
+    "rsb_batch_set_pd_target": [_P, _P, _P, _I, _I, _I],
+    "rsb_batch_set_pd_gains": [_P, _P, _P],
+    "rsb_batch_set_generalized_force": [_P, _P, _I, _I, _I],
+    "rsb_batch_get_generalized_force": [_P, _P, _I, _I, _I],
+    "rsb_batch_set_control_mode": [_P, _I],
+    "rsb_batch_set_external_wrench": [_P, _I, _P, _P, _P, _I, _I, _I],
+    "rsb_batch_bind_pd_target": [_P, _P, _I],
+    "rsb_batch_set_body_inertia": [_P, _P, _I, _I, _I],
+    "rsb_batch_clear_body_inertia": [_P],
+    "rsb_batch_set_contact_friction": [_P, _P, _I, _I, _I],
+    "rsb_batch_clear_contact_friction": [_P],
+    "rsb_batch_set_actuator_params": [_P, _P, _I, _I, _I],
+    "rsb_batch_clear_actuator_params": [_P],
+    "rsb_batch_set_actuator_network": [_P, _P, _I, _I, _I, _I, _P],
+    "rsb_batch_set_actuator_history": [_P, _P, _I, _I, _I],
+    "rsb_batch_get_actuator_history": [_P, _P, _I, _I, _I],
+    "rsb_batch_set_actuation_delay": [_P, _P, _I, _I, _I],
+    "rsb_batch_clear_actuation_delay": [_P],
+    "rsb_batch_integrate1": [_P],
+    "rsb_batch_integrate2": [_P],
+    "rsb_batch_integrate": [_P, _I],
+    "rsb_batch_get_mass_matrix": [_P, _I, _I, _P, _I],
+    "rsb_batch_get_nonlinearities": [_P, _I, _I, _P, _I],
+    "rsb_batch_get_body_poses": [_P, _I, _I, _P, _P, _I],
+    "rsb_batch_get_contacts": [_P, _P, _P, _I, _I, _I],
+    "rsb_batch_get_contact_points": [_P, _P, _I, _I, _I],
+    "rsb_batch_get_solver_iterations": [_P, _P, _I, _I, _I],
+    "rsb_batch_get_diverged": [_P, _P, _I, _I, _I],
+    "rsb_batch_get_solver_residual": [_P, _P, _I, _I, _I],
+    "rsb_batch_get_solver_status": [_P, _P, _I, _I, _I],
+    "rsb_batch_update_kinematics": [_P],
+    "rsb_batch_device_ptrs": [_P, C.POINTER(DeviceView)],
+    "rsb_batch_launch_count": ([_P], C.c_int64),
+    "rsb_batch_set_frames": [_P, _P, _P, _P, _I],
+    "rsb_batch_get_frame_states": [_P, _I, _I] + [_P] * 4 + [_I],
+    "rsb_batch_get_frame_jacobians": [_P, _I, _I, _P, _I],
+    "rsb_batch_set_contact_bodies": [_P, _P, _I],
+    "rsb_batch_get_body_contact_forces": [_P, _I, _I, _P, _P, _I],
+    "rsb_batch_set_height_scan": [_P, _P, _P, _I, _I],
+    "rsb_batch_get_height_scan": [_P, _I, _I, _P, _P, _I],
+    "rsb_batch_ob_dim": [_P],
+    "rsb_batch_observe": [_P, _P, _I, _I, _I],
+    "rsb_batch_control_step": [_P, _P, _P, _I, _I, _P, _I],
+    "rsb_batch_gym_configure": [_P] + [_P] * 5 + [_I, _F, _F, _F],
+    "rsb_batch_gym_reset": [_P],
+    "rsb_batch_gym_step": [_P, _P, _I, _I, _P, _P, _P, _I],
+    "rsb_peer_buffer_create": [_I, C.c_size_t, C.POINTER(_P), _P],
+    "rsb_peer_buffer_open": [_I, _P, C.POINTER(_P)],
+    "rsb_peer_buffer_close": [_P],
+    "rsb_peer_buffer_destroy": [_P],
+    "rsb_batch_set_observation_peers": [_P, _I, _I, _P, _P],
+    "rsb_batch_wait_observation_peers": [_P, C.POINTER(_I)],
+    "rsb_comm_init": [C.POINTER(_P), _I, C.POINTER(_P)],
+    "rsb_comm_allgather_obs": [_P, C.POINTER(_P)],
+    "rsb_comm_destroy": [_P],
+    "rsb_terrain_generate": [C.POINTER(TerrainProperties), _P],
+    "rsb_heightmap_read_text": [_S, _P, _P, _P, _P, _P, _I],
+    "rsb_heightmap_read_png": [_S, C.c_double, C.c_double, _P, _P, _P, _I],
+}
+EXPORTED = list(SIGNATURES)
 
 _lib = None
 
@@ -126,105 +205,13 @@ def lib():
             except Exception as e:
                 raise RsbError(f"{LIB_PATH} is missing and could not be built ({e}): run `python -c 'import __graft_entry__ as g; g.build()'` (no CPU fallback exists)")
         L = C.CDLL(LIB_PATH)
-        L.rsb_last_error.restype = C.c_char_p
-        L.rsb_model_body_name.restype = C.c_char_p
-        L.rsb_model_joint_name.restype = C.c_char_p
-        L.rsb_batch_launch_count.restype = C.c_int64
-        L.rsb_model_create_from_urdf.argtypes = [C.c_char_p, C.POINTER(C.c_void_p)]
-        L.rsb_model_load.argtypes = [C.c_char_p, C.c_void_p]
-        L.rsb_model_save.argtypes = [C.c_void_p, C.c_char_p]
-        L.rsb_model_collision_index.argtypes = [C.c_void_p, C.c_char_p]
-        L.rsb_model_destroy.argtypes = [C.c_void_p]
-        L.rsb_model_dims.argtypes = [C.c_void_p] + [C.POINTER(C.c_int)] * 5
-        L.rsb_model_get_tables.argtypes = [C.c_void_p, C.POINTER(ModelTables)]
-        L.rsb_model_body_index.argtypes = [C.c_void_p, C.c_char_p]
-        L.rsb_model_body_name.argtypes = [C.c_void_p, C.c_int]
-        L.rsb_model_joint_name.argtypes = [C.c_void_p, C.c_int]
-        L.rsb_model_frame_index.argtypes = [C.c_void_p, C.c_char_p]
-        L.rsb_model_frame.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
-        L.rsb_batch_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
-        L.rsb_batch_destroy.argtypes = [C.c_void_p]
-        L.rsb_batch_set_stream.argtypes = [C.c_void_p, C.c_void_p]
-        L.rsb_batch_sync.argtypes = [C.c_void_p]
-        L.rsb_batch_num_envs.argtypes = [C.c_void_p]
-        L.rsb_batch_set_ground.argtypes = [C.c_void_p, C.c_float]
-        L.rsb_batch_set_heightmap.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p]
-        L.rsb_batch_set_heightmaps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
-        L.rsb_batch_clear_terrain.argtypes = [C.c_void_p]
-        if hasattr(L, "rsb_batch_set_heightmap_index"):    # absent from an older build loaded through RSB_LIB_PATH (tools/terrain_curriculum_probe.py)
-            L.rsb_batch_set_heightmap_index.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-            L.rsb_batch_update_heightmaps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
-        L.rsb_batch_set_collision_friction.argtypes = [C.c_void_p, C.c_int, C.c_float]
-        L.rsb_batch_set_self_collision.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-        L.rsb_batch_set_params.argtypes = [C.c_void_p, C.POINTER(Params)]
-        L.rsb_batch_get_params.argtypes = [C.c_void_p, C.POINTER(Params)]
-        L.rsb_params_default.argtypes = [C.POINTER(Params)]
-        for n in ("rsb_batch_set_state", "rsb_batch_get_state", "rsb_batch_set_pd_target"):
-            getattr(L, n).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_set_pd_gains.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.rsb_batch_set_generalized_force.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_set_control_mode.argtypes = [C.c_void_p, C.c_int]
-        L.rsb_batch_set_external_wrench.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_bind_pd_target.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_batch_get_generalized_force.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_integrate1.argtypes = [C.c_void_p]
-        L.rsb_batch_integrate2.argtypes = [C.c_void_p]
-        L.rsb_batch_integrate.argtypes = [C.c_void_p, C.c_int]
-        for n in ("rsb_batch_get_mass_matrix", "rsb_batch_get_nonlinearities"):
-            getattr(L, n).argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
-        L.rsb_batch_get_body_poses.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_batch_get_contacts.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_get_contact_points.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_get_solver_iterations.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_get_diverged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_get_solver_residual.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_get_solver_status.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_update_kinematics.argtypes = [C.c_void_p]
-        L.rsb_batch_set_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_batch_get_frame_states.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_int]
-        L.rsb_batch_get_frame_jacobians.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
-        if hasattr(L, "rsb_batch_set_contact_bodies"):     # absent from an older build loaded through RSB_LIB_PATH (tools/contact_force_probe.py)
-            L.rsb_batch_set_contact_bodies.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-            L.rsb_batch_get_body_contact_forces.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
-        if hasattr(L, "rsb_batch_set_body_inertia"):       # absent from an older build loaded through RSB_LIB_PATH (tools/body_inertia_probe.py)
-            L.rsb_batch_set_body_inertia.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-            L.rsb_batch_clear_body_inertia.argtypes = [C.c_void_p]
-        if hasattr(L, "rsb_batch_set_contact_friction"):   # absent from an older build loaded through RSB_LIB_PATH (tools/contact_friction_probe.py)
-            L.rsb_batch_set_contact_friction.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-            L.rsb_batch_clear_contact_friction.argtypes = [C.c_void_p]
-        if hasattr(L, "rsb_batch_set_actuator_params"):    # absent from an older build loaded through RSB_LIB_PATH (tools/actuator_params_probe.py)
-            L.rsb_batch_set_actuator_params.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-            L.rsb_batch_clear_actuator_params.argtypes = [C.c_void_p]
-        if hasattr(L, "rsb_batch_set_actuator_network"):   # absent from an older build loaded through RSB_LIB_PATH (tools/actuator_network_probe.py)
-            L.rsb_batch_set_actuator_network.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
-            L.rsb_batch_set_actuator_history.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-            L.rsb_batch_get_actuator_history.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        if hasattr(L, "rsb_batch_set_actuation_delay"):    # absent from an older build loaded through RSB_LIB_PATH (tools/actuation_delay_probe.py)
-            L.rsb_batch_set_actuation_delay.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-            L.rsb_batch_clear_actuation_delay.argtypes = [C.c_void_p]
-        if hasattr(L, "rsb_batch_set_height_scan"):        # absent from an older build loaded through RSB_LIB_PATH (tools/height_scan_probe.py)
-            L.rsb_batch_set_height_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-            L.rsb_batch_get_height_scan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_batch_device_ptrs.argtypes = [C.c_void_p, C.POINTER(DeviceView)]
-        L.rsb_batch_launch_count.argtypes = [C.c_void_p]
-        L.rsb_batch_ob_dim.argtypes = [C.c_void_p]
-        L.rsb_batch_observe.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.rsb_batch_control_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
-        L.rsb_batch_gym_configure.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int, C.c_float, C.c_float, C.c_float]
-        L.rsb_batch_gym_reset.argtypes = [C.c_void_p]
-        L.rsb_batch_gym_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_comm_init.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p)]
-        L.rsb_comm_allgather_obs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        L.rsb_comm_destroy.argtypes = [C.c_void_p]
-        L.rsb_terrain_generate.argtypes = [C.POINTER(TerrainProperties), C.c_void_p]
-        L.rsb_heightmap_read_text.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_heightmap_read_png.argtypes = [C.c_char_p, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.rsb_peer_buffer_create.argtypes = [C.c_int, C.c_size_t, C.POINTER(C.c_void_p), C.c_void_p]
-        L.rsb_peer_buffer_open.argtypes = [C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-        L.rsb_peer_buffer_close.argtypes = [C.c_void_p]
-        L.rsb_peer_buffer_destroy.argtypes = [C.c_void_p]
-        L.rsb_batch_set_observation_peers.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        L.rsb_batch_wait_observation_peers.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
+        for name, sig in SIGNATURES.items():
+            if not hasattr(L, name):
+                if LIB_PATH == _OTHER_BUILD:
+                    continue          # an older build: calling what it lacks raises AttributeError
+                raise RsbError(f"{LIB_PATH} does not export {name}: rebuild it")
+            f = getattr(L, name)
+            f.argtypes, f.restype = sig if isinstance(sig, tuple) else (sig, C.c_int)
         _lib = L
     return _lib
 
