@@ -47,7 +47,9 @@ extern "C" {
 typedef struct rsb_model rsb_model; /* immutable robot description (URDF -> tables) */
 typedef struct rsb_batch rsb_batch; /* N environments of one model on one GPU        */
 
-/* World::setTimeStep, setGravity, setERP, setContactSolverParam, setDefaultMaterial */
+/* World::setTimeStep, setGravity, setERP, setContactSolverParam, setDefaultMaterial.
+ * rsb_batch_set_params refuses (RSB_ERR_INVALID, naming the field; the batch keeps its parameters) a non-finite value in any float
+ * field, dt <= 0, max_iter < 1, mu < 0, accel_m other than 0 or 2, accel_start < 3 with accel_m = 2, and stall_reg < 0. */
 typedef struct rsb_params {
   float dt;          /* World::setTimeStep                               (default 0.0025) */
   float gravity[3];  /* World::setGravity                                (0,0,-9.81)      */

@@ -868,7 +868,17 @@ int rsb_batch_update_heightmaps(rsb_batch* b, int first, int count, const float*
   return RSB_OK;
 }
 int rsb_batch_set_params(rsb_batch* b, const rsb_params* p) {
-  if (!b || !p) return fail(RSB_ERR_INVALID, "null argument");
+  if (!p) return fail(RSB_ERR_INVALID, "null argument");
+  // every float field finite, checked before the batch: a non-finite dt, gravity or relaxation factor turns every state into NaN on
+  // the next launch, a NaN threshold turns the convergence test off
+  const struct { const char* name; float v; } fields[] = {
+      {"dt", p->dt}, {"gravity[0]", p->gravity[0]}, {"gravity[1]", p->gravity[1]}, {"gravity[2]", p->gravity[2]}, {"erp", p->erp},
+      {"alpha_init", p->alpha_init}, {"alpha_min", p->alpha_min}, {"alpha_decay", p->alpha_decay}, {"threshold", p->threshold},
+      {"mu", p->mu}, {"restitution", p->restitution}, {"rest_threshold", p->rest_threshold}, {"stall_ratio", p->stall_ratio},
+      {"stall_reg", p->stall_reg}};
+  for (const auto& f : fields)
+    if (!std::isfinite(f.v)) return fail(RSB_ERR_INVALID, std::string("params: ") + f.name + " is not finite");
+  if (!b) return fail(RSB_ERR_INVALID, "null argument");
   if (!(p->dt > 0) || p->max_iter < 1 || !(p->mu >= 0)) return fail(RSB_ERR_INVALID, "invalid params");
   if (p->accel_m != 0 && p->accel_m != 2) return fail(RSB_ERR_INVALID, "accel_m must be 0 (plain sweeps) or 2");
   if (p->accel_m == 2 && p->accel_start < 3) return fail(RSB_ERR_INVALID, "accel_start must be at least 3");

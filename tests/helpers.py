@@ -390,3 +390,180 @@ def launch_config(capi, bt):
     assert L.rsb_internal_launch_config(bt.h, ctypes.byref(v[0]), ctypes.byref(v[1])) == 0
     assert L.rsb_internal_launch_instance(bt.h, ctypes.byref(v[2]), ctypes.byref(v[3])) == 0
     return dict(zip(("wpc", "grid", "spec", "slots"), [x.value for x in v]))
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Every compiled instance of the step kernel: the models that reach each one, and a batch of robots landing under stiff PD
+
+OPTIONS = (28, 16, 14, 8, 4, 1)          # warps per CTA, as pick_config offers them
+# name, robot description, RSB_FORCE_GENERIC, (spec, slots) it must run, base height, nominal joint positions
+_Q = ANYMAL_GC0[7:]
+_QP = np.where(np.arange(12) % 3 == 2, 0.0, _Q)          # prismatic knees at the middle of their travel
+CASES = {
+    "quad_feet": (QUAD_FEET, False, (1, 1), 0.56, _Q),
+    "anymal": ("anymal_c_like.urdf", False, (1, 2), 0.56, _Q),
+    "quad_prismatic": (QUAD_PRISMATIC, False, (1, 2), 0.62, _QP),
+    "quad_branched": (QUAD_BRANCHED, False, (0, 1), 0.6, None),
+    "atlas": ("atlas_like.urdf", False, (2, 2), 0.95, None),
+    "hexapod": (HEXAPOD, False, (0, 1), 0.22, None),
+    "max32": (MAX32, False, (0, 2), 0.1, None),
+    "anymal_generic": ("anymal_c_like.urdf", True, (0, 2), 0.56, _Q),
+    "atlas_generic": ("atlas_like.urdf", True, (0, 2), 0.95, None),
+}
+# warps per CTA whose CTA (model block + one workspace per warp) fits in the 227 KB of shared memory of an H100
+FITS = {
+    "quad_feet": OPTIONS, "anymal": OPTIONS, "quad_prismatic": OPTIONS, "quad_branched": OPTIONS, "anymal_generic": OPTIONS,
+    "hexapod": (16, 14, 8, 4, 1),
+    "atlas": (16, 14, 8, 4, 1), "atlas_generic": (16, 14, 8, 4, 1),
+    "max32": (16, 14, 8, 4, 1),
+}
+
+
+def _nominal(name, t):
+    urdf, generic, inst, base_z, q = CASES[name]
+    gc0 = np.zeros(t["nq"]); gc0[2] = base_z; gc0[3] = 1.0
+    if q is not None:
+        gc0[7:] = q
+    return gc0
+
+
+def _state(name, t, n, rng):
+    """upright robots with a small random tilt, jittered joints and velocities, spread over the terrain; in every environment two
+    joints of short travel (less than 3 rad or m between the stops) start up to 5 cm or 0.05 rad past a stop"""
+    gc0 = _nominal(name, t)
+    gc = np.tile(gc0, (n, 1))
+    gc[:, :2] = rng.uniform(-2, 2, (n, 2))
+    q = np.c_[np.ones(n), 0.08 * rng.standard_normal((n, 3))]; q /= np.linalg.norm(q, axis=1, keepdims=True)
+    gc[:, 3:7] = q
+    gc[:, 7:] += rng.uniform(-0.15, 0.15, (n, t["nq"] - 7))
+    short = np.where((t["jlimit"][1:, 1] - t["jlimit"][1:, 0]) < 3.0)[0] + 1
+    for e in range(n):
+        for body in rng.choice(short, 2, replace=False):
+            lo, hi = t["jlimit"][body]
+            gc[e, t["qidx"][body]] = hi + rng.uniform(0.01, 0.05) if rng.uniform() < 0.5 else lo - rng.uniform(0.01, 0.05)
+    gv = 0.3 * rng.standard_normal((n, t["nv"]))
+    return gc.astype(np.float32).astype(np.float64), gv.astype(np.float32).astype(np.float64)
+
+
+def _pd(t, n, gc0, rng):
+    """stiff PD towards targets up to 0.6 rad / m off the nominal pose: joints run into their stops and their actuators' effort limits"""
+    kp = np.r_[np.zeros(6), 300.0 * np.ones(t["nv"] - 6)]; kd = np.r_[np.zeros(6), 4.0 * np.ones(t["nv"] - 6)]
+    pt = np.tile(gc0, (n, 1)); pt[:, 7:] += rng.uniform(-0.6, 0.6, (n, t["nq"] - 7))
+    prismatic = t["jtype"][1:] == 2
+    pt[:, 7:][:, prismatic] = np.tile(gc0[7:][prismatic], (n, 1)) + rng.uniform(-0.2, 0.2, (n, prismatic.sum()))
+    return kp, kd, pt.astype(np.float32)
+
+
+def _batch(capi, monkeypatch, name, n, terrain, seed, wpc=None, params=None):
+    urdf, generic, inst, base_z, q = CASES[name]
+    monkeypatch.setenv("RSB_FORCE_GENERIC", "1" if generic else "0")
+    if wpc is None:
+        monkeypatch.delenv("RSB_FORCE_WPC", raising=False)
+    else:
+        monkeypatch.setenv("RSB_FORCE_WPC", str(wpc))
+    t, bt, o64, o32, _, _, _ = setup_batch(capi, urdf, n, seed, terrain=terrain, tau_scale=0.0, params=params)
+    cfg = launch_config(capi, bt)
+    assert (cfg["spec"], cfg["slots"]) == inst, f"{name}: runs instance {cfg}, expected (spec, slots) = {inst}"
+    rng = np.random.default_rng(seed + 1)
+    gc, gv = _state(name, t, n, rng)
+    kp, kd, pt = _pd(t, n, _nominal(name, t), rng)
+    bt.set_state(gc.astype(np.float32), gv.astype(np.float32))
+    bt.set_control_mode(capi.PD_PLUS_FEEDFORWARD_TORQUE)
+    bt.set_generalized_force(np.zeros((n, t["nv"]), np.float32))
+    bt.set_pd_gains(kp, kd)
+    bt.set_pd_target(pt, np.zeros((n, t["nv"]), np.float32))
+    return t, bt, o64, o32, gc, gv, kp, kd, pt, cfg
+
+
+def _at_effort_limit(t, tau_applied):
+    lim = np.array([t["jeffort"][i] for i in range(1, t["nb"])])
+    return np.abs(np.abs(tau_applied[:, 6:]) - lim[None, :]) < 1e-9 * lim[None, :]
+
+
+def _row(name, cfg, n, K, cr, extra):
+    T = cfg["wpc"] * cfg["grid"]
+    rounds = -(-n // T)
+    fill = (n - (rounds - 1) * T) / T
+    print(f"| {name:15s} | spec {cfg['spec']} | slots {cfg['slots']} | WPC {cfg['wpc']:2d} | grid {cfg['grid']:3d} | rounds {rounds:2d} | "
+          f"last round {100 * fill:5.1f} % | K {K:.2f} | CR max {cr if cr >= 0 else '-':>2} | {extra}")
+
+
+def step_and_trajectory(capi, monkeypatch, name, terrain, seed, params=None, n=256, near_threshold="refuse", converged=0.88, flips=0):
+    """one step (contact lists, state, impulses, complementarity, actuators at their effort limits) and 10 steps (state) of CASES[name]
+    against the oracle, PD targets on, joints at their stops and actuators at their effort limits.  params: rsb_params fields (gx, gy,
+    gz for gravity) on both sides; dt, mu and joint_limits set the bounds and the edges the run must reach.  With restitution on
+    (restitution and rest_threshold > 0) the threshold must split the approach speeds; an approach speed within 1e-4 m/s of it fails
+    the run (near_threshold="refuse") or leaves its environment out of the one-step comparison ("exclude").  converged: the least share
+    of environments whose solves converge on both sides with equal contact lists (the one-step comparison's sample).  flips: environments
+    left out of the 10-step quantiles, the worst ones -- on the rough map index parity allows one contact list per step to differ on a
+    tie, and a robot whose contact set changed one step apart from the oracle's follows another trajectory from there.
+    Returns a dict of the run's figures for the caller's table."""
+    prm = dict(params or {})
+    dt, mu, limits = prm.get("dt", 0.0025), prm.get("mu", 0.8), prm.get("joint_limits", 1)
+    t, bt, o64, o32, gc, gv, kp, kd, pt, cfg = _batch(capi, monkeypatch, name, n, terrain, seed=seed, params=prm)
+    ptd, vt = pt.astype(np.float64), np.zeros((n, t["nv"]))
+    bt.integrate(1)
+    g1, v1 = bt.get_state(); ct, cnt = bt.contacts(); pts = bt.contact_points(); st = bt.solver_status(); ta = bt.generalized_force()
+    a, b = gc.copy(), gv.copy()
+    d = o64.step(a, b, ptarget=ptd, vtarget=vt, kp=kp, kd=kd, debug=True)
+    c, e_ = gc.copy(), gv.copy()
+    d32 = o32.step(c, e_, ptarget=ptd, vtarget=vt, kp=kp, kd=kd, debug=True)
+    assert np.isfinite(g1).all() and np.isfinite(v1).all()
+    # the edges this test is meant to reach: contacts, joint-limit rows (none with joint_limits = 0), saturated actuators
+    sat_ref = _at_effort_limit(t, d["tau_applied"])
+    assert cnt.sum() > n // 4 and sat_ref.any()
+    assert d["nlimits"].sum() > 0 if limits else d["nlimits"].sum() == 0
+    # the effort-limit switch (its threshold moves with dt) takes the oracle's side on every actuator not within rounding of it
+    lim = np.array([t["jeffort"][i] for i in range(1, t["nb"])])
+    sat_gpu = np.abs(np.abs(ta[:, 6:].astype(np.float64)) - lim[None, :]) < 1e-6 * lim[None, :]
+    assert (sat_gpu == sat_ref).mean() > 0.999, f"{int((sat_gpu != sat_ref).sum())} actuators switched differently"
+    near = np.zeros(n, bool)
+    if prm.get("restitution", 0.0) > 0 and prm.get("rest_threshold", 0.01) > 0:
+        vn = normal_speeds(t, gc, gv, d)
+        if near_threshold == "refuse":
+            check_restitution_split(vn, prm["rest_threshold"])
+        else:
+            w = vn[np.isfinite(vn)]
+            assert (w < -prm["rest_threshold"]).sum() > 10 and (w > -prm["rest_threshold"]).sum() > 10
+            near = (np.abs(np.nan_to_num(vn, nan=1e9) + prm["rest_threshold"]) < 1e-4).any(1)
+    hard = index_parity(pts, cnt, d32, f"{name} {terrain}")
+    # on the rough map two triangles sharing an edge can tie to 1e-6 m under different rounding
+    # (test_heightmap_narrow_phase_matches_oracle_on_rough_terrain): at most one environment in 256
+    assert hard.sum() <= (0 if terrain == "ground" else 1), f"contact lists differ in envs {np.where(hard)[0][:10]}"
+    same = (pts == d["c_pt"]).all(1)
+    conv = same & (st == 0) & (d["status"] == 0) & ~near
+    ev = np.abs(v1 - b)[conv]; eq = np.abs(g1 - a)[conv]; e32 = np.abs(e_ - b)[conv]
+    scale_v = 1.0 + np.abs(b[conv])
+    live = conv[:, None] & (d["c_pt"] >= 0)
+    ln_gpu = np.einsum("ekj,ekj->ek", ct["impulse"], ct["normal"])
+    en = np.abs(ln_gpu - d["c_lambda"][:, :, 2])[live]
+    lam_scale = max(1.0, np.abs(d["c_lambda"][:, :, 2][live]).max()) if live.any() else 1.0
+    # 10 control steps from the start state
+    bt.integrate(9)
+    gN, _ = bt.get_state()
+    o64.step(a, b, n_steps=9, ptarget=ptd, vtarget=vt, kp=kp, kd=kd)
+    o32.step(c, e_, n_steps=9, ptarget=ptd, vtarget=vt, kp=kp, kd=kd)
+    e = np.sort(np.abs(gN - a).max(1))[:n - flips]; ef = np.abs(c - a).max(1)
+    print(f"   {name} {terrain}: oracle limit rows {np.bincount(d['nlimits'], minlength=5).tolist()}, dofs at their effort limit "
+          f"{int(sat_ref.sum())}")
+    cr = int((3 * d["ncontacts"] + d["nlimits"]).max())
+    _row(name, cfg, n, cnt.mean(), cr, f"{terrain:6s} | converged {100 * conv.mean():.0f} % | 1 step: gv err median {np.median(ev.max(1)):.1e} "
+         f"(f32 oracle {np.median(e32.max(1)):.1e}), normal impulse p99 {np.quantile(en, .99) if en.size else 0:.1e} | 10 steps: gc err median "
+         f"{np.median(e):.1e} p90 {np.quantile(e, .9):.1e} p99 {np.quantile(e, .99):.1e} (f32 oracle p99 {np.quantile(ef, .99):.1e})")
+    assert conv.mean() > converged
+    assert np.median(ev.max(1)) < max(2e-5, 3 * np.median(e32.max(1)))
+    assert np.max(ev / scale_v) < max(5e-3, 3 * np.max(e32 / scale_v))
+    assert eq.max() < 5e-3 * dt * (1.0 + np.abs(b[conv]).max()) + 2e-6
+    assert en.size == 0 or np.quantile(en, 0.99) < 1e-4 * lam_scale
+    # Signorini and Coulomb on the GPU result itself, with the friction in force
+    on = np.arange(ct["impulse"].shape[1])[None, :] < cnt[:, None]
+    assert (ln_gpu[on] >= -1e-6).all()
+    lt = np.linalg.norm(ct["impulse"] - ln_gpu[:, :, None] * ct["normal"], axis=2)
+    assert (lt[on] <= mu * ln_gpu[on] + 1e-4 * (1 + ln_gpu[on])).all()
+    assert np.isfinite(gN).all() and flips <= n // 25
+    # positions drift from the oracle's in proportion to the step: the absolute floors are those of the default dt, 0.0025
+    grow = max(1.0, dt / 0.0025)
+    assert np.median(e) < 2e-5 * grow and np.median(e) < 5 * np.median(ef) + 1e-6
+    assert np.quantile(e, 0.9) < max(1e-4 * grow, 5 * np.quantile(ef, 0.9))
+    assert np.quantile(e, 0.99) < max(5e-3 * grow, 5 * np.quantile(ef, 0.99))
+    return dict(t=t, bt=bt, d=d, ct=ct, cnt=cnt, pts=pts, st=st, conv=conv, ln_gpu=ln_gpu, lt=lt, on=on)

@@ -32,6 +32,25 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(capi.Params) == 4 * 19      # rsb_params: 16 words of round 1 + accel_m, accel_start, stall_reg
 
 
+def test_set_params_refuses_non_finite_fields_before_the_batch():
+    """every non-finite float field of rsb_params is refused by name, before the batch is looked at; a valid set reaches the
+    null-batch check"""
+    L = capi.lib()
+    p = capi.Params()
+    assert L.rsb_params_default(ctypes.byref(p)) == 0
+    assert L.rsb_batch_set_params(None, ctypes.byref(p)) == -1 and "null argument" in L.rsb_last_error().decode()
+    fields = ["dt", "erp", "alpha_init", "alpha_min", "alpha_decay", "threshold", "mu", "restitution", "rest_threshold", "stall_ratio", "stall_reg"]
+    for f in fields + [f"gravity[{i}]" for i in range(3)]:
+        for v in (float("nan"), float("inf"), float("-inf")):
+            q = capi.Params.from_buffer_copy(bytes(p))
+            if f.startswith("gravity"):
+                q.gravity[int(f[8])] = v
+            else:
+                setattr(q, f, v)
+            assert L.rsb_batch_set_params(None, ctypes.byref(q)) == -1
+            assert L.rsb_last_error().decode() == f"params: {f} is not finite", (f, v)
+
+
 @pytest.mark.parametrize("src", ["anymal_c_like.urdf", "atlas_like.urdf", PENDULUM_URDF, BOX_URDF, REALISTIC_URDF,
                                  pytest.param(QUAD_FEET, id="quad_feet"), pytest.param(QUAD_PRISMATIC, id="quad_prismatic"),
                                  pytest.param(QUAD_BRANCHED, id="quad_branched"), pytest.param(HEXAPOD, id="hexapod"), pytest.param(MAX32, id="max32")])
