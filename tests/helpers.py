@@ -475,6 +475,14 @@ def _batch(capi, monkeypatch, name, n, terrain, seed, wpc=None, params=None):
     return t, bt, o64, o32, gc, gv, kp, kd, pt, cfg
 
 
+def effort_limits(t):
+    """[nv] URDF effort limit of every dof in the batch's gv order (the base: unlimited)"""
+    lim = np.full(t["nv"], 1e30)
+    for b in range(1, t["nb"]):
+        lim[t["vidx"][b]] = t["jeffort"][b]
+    return lim
+
+
 def _at_effort_limit(t, tau_applied):
     lim = np.array([t["jeffort"][i] for i in range(1, t["nb"])])
     return np.abs(np.abs(tau_applied[:, 6:]) - lim[None, :]) < 1e-9 * lim[None, :]

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, RSC
-from helpers import ANYMAL_GC0, THRESH, setup_batch
+from helpers import ANYMAL_GC0, THRESH, effort_limits, setup_batch
 from oracle.oracle import Oracle
 from test_gpu_contact_forces import _make, _outputs, _same
 from test_self_collision_oracle import anymal_leg_pairs
@@ -34,12 +34,7 @@ SETUPS = {"quadruped_hm": ("quadruped", "hm", False), "humanoid_ground": ("human
 MODES = ("pd", "force")
 
 
-def _limits(t):
-    """[nv] URDF effort limit of every dof in the batch's gv order (the base: unlimited)"""
-    lim = np.full(t["nv"], 1e30)
-    for b in range(1, t["nb"]):
-        lim[t["vidx"][b]] = t["jeffort"][b]
-    return lim
+_limits = effort_limits
 
 
 def _setup(capi, monkeypatch, which, n, seed, mode="pd", wpc=None):
