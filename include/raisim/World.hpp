@@ -125,10 +125,11 @@ struct LockStep {
   // rows the device fills: deferred, every environment's, valid until the next launch (the height scan: until the next state write or
   // terrain upload); immediate, the reader's row of the last read
   Rows<float> tauApplied, cfForce, scan, scanXy;   // [nv], [S][3] and [S] of the contact bodies (setContactBodies), [P] and [P][2] of the scan
+  Rows<float> imuLin, imuAng;               // [I][3] each: the IMUs' readings (setImus)
   Rows<int32_t> ncontacts, cfSteps;
   Rows<rsb_contact> contacts;               // [RSB_KMAX]
-  int cfBodies = 0, scanPoints = 0;
-  bool stateValid = false, tauAppliedValid = false, contactsValid = false, cfValid = false, scanValid = false;
+  int cfBodies = 0, scanPoints = 0, imus = 0;
+  bool stateValid = false, tauAppliedValid = false, contactsValid = false, cfValid = false, scanValid = false, imuValid = false;
   // terrain of every environment of a deferred mirror (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding
   // the same heights share one MapEntry; `atlas` is what the device holds, in atlas order (atlasSingle: one map set without an index)
   struct MapEntry {
@@ -249,7 +250,7 @@ struct LockStep {
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
-    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = false;
+    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = imuValid = false;
   }
   // every environment is parked (or finished) with the same number of integrate() calls pending
   void flush() {
@@ -287,6 +288,13 @@ struct LockStep {
     refill(env, cfValid, [&](int lo, int k, bool all) {
       rsbCheck(rsb_batch_get_body_contact_forces(batch, lo, k, all || force ? cfForce.row(lo) : nullptr, all || steps ? cfSteps.row(lo) : nullptr, RSB_HOST),
                "getBodyContactForce");
+    });
+  }
+  void needImuReadings(int env, bool lin, bool ang) {
+    if (imuLin.w != size_t(imus) * 3) { imuLin.init(n, size_t(imus) * 3, 0.f); imuAng.init(n, size_t(imus) * 3, 0.f); imuValid = false; }
+    refill(env, imuValid, [&](int lo, int k, bool all) {
+      rsbCheck(rsb_batch_get_imu_readings(batch, lo, k, all || lin ? imuLin.row(lo) : nullptr, all || ang ? imuAng.row(lo) : nullptr, RSB_HOST),
+               "getImuReadings");
     });
   }
   // deferred: one call scans every environment, after the rows written since the last launch went up (a reset() that moved a robot is seen)
@@ -493,6 +501,22 @@ class BatchedWorld {
     throw std::runtime_error("getBodyContactForce: body " + std::to_string(bodyIdx) + " is not among the bodies given to setContactBodies()");
   }
   size_t numContactBodies() const { return contactBodies_.size(); }
+  // IMUs at model frames (ArticulatedSystem::setImus): one list for all environments
+  void setImus(const std::vector<size_t>& frames) {
+    if (frames == imuFrames_) return;          // every environment of a VectorizedEnvironment sets the same list in its constructor
+    std::vector<int32_t> body(frames.size());
+    std::vector<float> pos(3 * frames.size()), rot(9 * frames.size());
+    for (size_t k = 0; k < frames.size(); k++) {
+      double p[3], r[9];
+      rsbCheck(rsb_model_frame(model_, int(frames[k]), &body[k], p, r), "setImus");
+      for (int c = 0; c < 3; c++) pos[3 * k + c] = float(p[c]);
+      for (int c = 0; c < 9; c++) rot[9 * k + c] = float(r[c]);
+    }
+    rsbCheck(rsb_batch_set_imus(batch_, body.data(), pos.data(), rot.data(), int(frames.size())), "setImus");
+    imuFrames_ = frames;
+    ls_.imus = int(frames.size()); ls_.imuValid = false;
+  }
+  size_t numImus() const { return imuFrames_.size(); }
   // terrain height-scan points (ArticulatedSystem::setHeightScan): one list for all environments
   void setHeightScan(const std::vector<int32_t>& bodies, const std::vector<float>& xy, bool yawAligned) {
     if (bodies == scanBodies_ && xy == scanXy_ && yawAligned == scanYaw_) return;   // every environment sets the same list in its constructor
@@ -531,6 +555,7 @@ class BatchedWorld {
  private:
   LockStep ls_;
   std::vector<size_t> contactBodies_;
+  std::vector<size_t> imuFrames_;
   std::vector<int32_t> scanBodies_;
   std::vector<float> scanXy_;
   std::vector<int32_t> anDofs_;
@@ -1014,6 +1039,23 @@ class ArticulatedSystem {
     const size_t s = w_->contactBodySlot(bodyIdx);
     m_.needContactForces(env_, false, true);
     return m_.cfSteps.row(env_)[s];
+  }
+  // setImus: IMUs at the model frames frameIndices (getFrameIdxByName order, at most RSB_MAX_IMUS), the sensor's axes those of the frame.
+  // The list belongs to the batch: every environment shares it, and each environment of a VectorizedEnvironment may set the same list in
+  // its constructor.
+  void setImus(const std::vector<size_t>& frameIndices) { w_->setImus(frameIndices); }
+  // IMU i's mean specific force [m/s^2, sensor frame] over the integrate() calls since the last state access (the fused launch; the one
+  // step of a stand-alone integrate()): what an accelerometer measures, +|g| upwards at rest and 0 in free fall
+  void getImuLinearAcceleration(size_t i, Vec<3>& out) {
+    if (i >= w_->numImus()) throw std::runtime_error("getImuLinearAcceleration: IMU " + std::to_string(i) + " was not given to setImus()");
+    m_.needImuReadings(env_, true, false);
+    for (int k = 0; k < 3; k++) out[k] = m_.imuLin.row(env_)[i * 3 + k];
+  }
+  // IMU i's mean angular rate [rad/s, sensor frame] over the same integrate() calls
+  void getImuAngularVelocity(size_t i, Vec<3>& out) {
+    if (i >= w_->numImus()) throw std::runtime_error("getImuAngularVelocity: IMU " + std::to_string(i) + " was not given to setImus()");
+    m_.needImuReadings(env_, false, true);
+    for (int k = 0; k < 3; k++) out[k] = m_.imuAng.row(env_)[i * 3 + k];
   }
   // setHeightScan: terrain height samples at horizontal offsets (x, y) from bodies (getBodyIdx order, at most RSB_MAX_SCAN_POINTS),
   // turned with each body's heading (yawAligned) or along the world axes: what an upstream observe() builds with one

@@ -394,6 +394,41 @@ int rsb_batch_set_contact_bodies(rsb_batch* b, const int32_t* body, int n);
 /* force [n][S][3] float32, steps_in_contact [n][S] int32, S = the number of bodies set; a NULL output is skipped; RSB_ERR_INVALID when
  * no bodies are set.  A plain copy of a contiguous slice of the batch's rows in stream order: no launch, host or device destination. */
 int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count, float* force, int32_t* steps_in_contact, int where);
+/* ---- IMU readings over a whole launch: what an accelerometer and a gyroscope rigidly attached to a body measure, for every
+ *      environment at once, gathered by the step kernel as the sub-steps go by.
+ *      Sensors: up to RSB_MAX_IMUS, shared by all environments.  Sensor k is attached to body[k]: its origin is at pos[k] and its
+ *      orientation is rot[k], both in the body frame (the triple rsb_model_frame returns for a URDF link frame, as for
+ *      rsb_batch_set_frames).
+ *      Notation: a launch that advances the state (rsb_batch_integrate, rsb_batch_integrate2, rsb_batch_control_step, rsb_batch_gym_step)
+ *      runs S sub-steps; (q_s, v_s) is the state at the start of sub-step s and v_{s+1} the velocity it produces.  x_k(q) is the
+ *      sensor's world point, R_k(q) = R_body(q) * rot[k] its world orientation, J_p, J_r the point and rotational Jacobians of
+ *      rsb_batch_get_frame_jacobians, g = rsb_params.gravity, dt = rsb_params.dt.
+ *      Per sub-step:
+ *        specific force  f_s = R_k(q_s)^T [ J_p(q_s) (v_{s+1} - v_s) / dt + Jdot_p(q_s, v_s) v_s - g ]: the classical acceleration of the
+ *                        sensor point that the sub-step's generalized acceleration gives at its start state, minus gravity.  The
+ *                        velocity difference is the one the step forms before it adds it to v_s.
+ *        angular rate    w_s = R_k(q_s)^T J_r(q_s) v_{s+1}: the rate the semi-implicit update turns the pose by over the sub-step (a
+ *                        floating base's quaternion update uses exactly this omega).
+ *      Output of a launch, per environment and sensor, float32 in the sensor frame: lin_acc = (sum_s f_s) * (1 / S) [m/s^2] and ang_vel =
+ *      (sum_s w_s) * (1 / S) [rad/s], summed in sub-step order and multiplied by the float32 reciprocal of S.
+ *      So a sensor at rest on a robot standing still reads +|g| along the sensor-frame direction opposite to gravity, a robot in free fall
+ *      reads 0, and a body spinning at a constant rate w reads the centripetal -w^2 r_perp and the rate w.
+ *      Each advancing launch overwrites both outputs; every other launch (rsb_batch_integrate1, the kinematics pass of the lazy getters,
+ *      rsb_batch_update_kinematics, the frame getters, the height scan) leaves them as they are.  They read zero from rsb_batch_set_imus()
+ *      until the first advancing launch.  In rsb_batch_gym_step an environment that terminates keeps the readings of the sub-steps that
+ *      ended it: the reset comes after them.  rsb_batch_set_state changes nothing until the next launch; a reading covers its own launch
+ *      only, so there is no history to reset.  A diverged environment may read NaN.  One lane per sensor and sub-steps in time order:
+ *      readings are bit-identical from run to run and for every launch shape.  With no sensors set the step computes and stores
+ *      nothing for this.  Noise, bias and drift are left to the caller; the sensor's orientation comes from the frame getters or gc. */
+#define RSB_MAX_IMUS 8
+/* body[n] in rsb_model_body_index order, pos[n][3], rot[n][9] row-major (NULL = identity).  n = 0 clears.  Refused with
+ * RSB_ERR_INVALID, changing nothing: a null batch, n < 0 or > RSB_MAX_IMUS, body or pos NULL with n > 0, a body out of range, a pos or
+ * rot entry that is not finite, a rot that is not a rotation (|R^T R - I| > 1e-4 in some entry, or det R <= 0, in double precision). */
+int rsb_batch_set_imus(rsb_batch* b, const int32_t* body, const float* pos, const float* rot, int n);
+/* lin_acc [n][I][3], ang_vel [n][I][3] float32, I = the number of sensors set; a NULL output is skipped; RSB_ERR_INVALID when no
+ * sensors are set, or for a bad range or `where`.  A plain copy of a contiguous slice of the batch's rows in stream order: no launch,
+ * host or device destination. */
+int rsb_batch_get_imu_readings(rsb_batch* b, int env_begin, int env_count, float* lin_acc, float* ang_vel, int where);
 /* ---- terrain height scans (what an upstream ENVIRONMENT builds in observe() with HeightMap::getHeight(x, y) once per point, for
  *      every environment at once).  One list of points, shared by all environments; point i hangs on body[i] at the horizontal
  *      offset xy[i][2].  Its sample is, with (p, R) the body's world pose:

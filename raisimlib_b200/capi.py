@@ -168,6 +168,8 @@ SIGNATURES = {
     "rsb_batch_get_frame_jacobians": [_P, _I, _I, _P, _I],
     "rsb_batch_set_contact_bodies": [_P, _P, _I],
     "rsb_batch_get_body_contact_forces": [_P, _I, _I, _P, _P, _I],
+    "rsb_batch_set_imus": [_P, _P, _P, _P, _I],
+    "rsb_batch_get_imu_readings": [_P, _I, _I, _P, _P, _I],
     "rsb_batch_set_height_scan": [_P, _P, _P, _I, _I],
     "rsb_batch_get_height_scan": [_P, _I, _I, _P, _P, _I],
     "rsb_batch_ob_dim": [_P],
@@ -319,7 +321,7 @@ class Batch:
         h = C.c_void_p()
         _ck(lib().rsb_batch_create(model.h, num_envs, device, C.byref(h)))
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
-        self.device, self.nframes, self.ncontact_bodies, self.nscan = device, 0, 0, 0
+        self.device, self.nframes, self.ncontact_bodies, self.nscan, self.nimus = device, 0, 0, 0, 0
         self.hm_shape = None                 # (ys, xs) of the height map(s) set through this object
         self.an_shape = None                 # (listed dofs, history) of the actuator network set through this object
 
@@ -607,6 +609,44 @@ class Batch:
         n, S = self._count(env_begin, env_count), self.ncontact_bodies
         _ck(lib().rsb_batch_get_body_contact_forces(self.h, env_begin, n, self._device_out(force, (n, S, 3), "force"),
                                                     self._device_out(steps, (n, S), "steps", "int32"), DEVICE))
+
+    # IMU readings over a whole launch
+    def set_imus(self, body, pos, rot=None):
+        """IMU sensors shared by all environments (at most 8): sensor k hangs on body[k] at pos[k] [3] with orientation rot[k] [3, 3]
+        (None: identity), both in the body frame.  Every launch that advances the state gathers their mean specific force and angular
+        rate over all its sub-steps.  An empty list clears them; a refused call keeps the sensors set before."""
+        bd = np.ascontiguousarray(body, np.int32).reshape(-1)
+        p = np.ascontiguousarray(pos, np.float32).reshape(-1, 3)
+        r = None if rot is None else np.ascontiguousarray(rot, np.float32).reshape(-1, 9)
+        if len(p) != len(bd) or (r is not None and len(r) != len(bd)):
+            raise ValueError(f"set_imus: {len(bd)} bodies, {len(p)} positions, {'no' if r is None else len(r)} rotations")
+        _ck(lib().rsb_batch_set_imus(self.h, bd.ctypes.data_as(C.c_void_p), p.ctypes.data_as(C.c_void_p),
+                                     None if r is None else r.ctypes.data_as(C.c_void_p), len(bd)))
+        self.nimus = len(bd)
+
+    def set_imus_by_frame(self, names):
+        """IMUs at the URDF link frames (or joint names) `names`, as rsb_model_frame gives them"""
+        L = lib()
+        body, pos, rot = [], np.zeros((len(names), 3)), np.zeros((len(names), 9))
+        for k, name in enumerate(names):
+            f, b = _ck(L.rsb_model_frame_index(self.model.h, name.encode())), C.c_int()
+            _ck(L.rsb_model_frame(self.model.h, f, C.byref(b), pos[k].ctypes.data_as(C.c_void_p), rot[k].ctypes.data_as(C.c_void_p)))
+            body.append(b.value)
+        self.set_imus(body, pos, rot)
+
+    def imu_readings(self, env_begin=0, env_count=None):
+        """(lin_acc [n, I, 3], ang_vel [n, I, 3]) float32 in the sensor frames: mean specific force [m/s^2] and angular rate [rad/s] over
+        the last launch that advanced the state"""
+        n = self._count(env_begin, env_count)
+        lin, ang = np.empty((n, self.nimus, 3), np.float32), np.empty((n, self.nimus, 3), np.float32)
+        _ck(lib().rsb_batch_get_imu_readings(self.h, env_begin, n, lin.ctypes.data_as(C.c_void_p), ang.ctypes.data_as(C.c_void_p), HOST))
+        return lin, ang
+
+    def imu_readings_into(self, lin_acc=None, ang_vel=None, env_begin=0, env_count=None):
+        """imu_readings() copied into torch CUDA float32 tensors [n, I, 3] (None skips one), in the batch's stream order: no launch"""
+        n, I = self._count(env_begin, env_count), self.nimus
+        _ck(lib().rsb_batch_get_imu_readings(self.h, env_begin, n, self._device_out(lin_acc, (n, I, 3), "lin_acc"),
+                                             self._device_out(ang_vel, (n, I, 3), "ang_vel"), DEVICE))
 
     # terrain height scans
     def set_height_scan(self, body, xy, align="yaw"):

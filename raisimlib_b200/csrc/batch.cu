@@ -132,6 +132,11 @@ struct rsb_batch {
   std::vector<uint8_t> contact_bodies;
   DevBuf<float> cf_force;
   DevBuf<int> cf_steps;
+  // IMU sensors of rsb_batch_set_imus (none: empty): body, position and rotation in the body frame as the kernel parameters carry them,
+  // and the rows the step kernel fills, tight for the current list: imu_lin, imu_ang [N][I][3]; allocated once, for RSB_MAX_IMUS
+  std::vector<uint8_t> imu_body;
+  std::vector<float> imu_pos, imu_rot;
+  DevBuf<float> imu_lin, imu_ang;
   // points of rsb_batch_set_height_scan (scan.n = 0: none) in one device allocation sized for RSB_MAX_SCAN_POINTS; scan_off_root: a
   // point hangs on a body whose pose comes from the kinematics pass
   ScanTable scan{};
@@ -427,6 +432,12 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
   if (phase_mask == 0 && !b->contact_bodies.empty()) {   // only a launch that advances the state accumulates (and overwrites) the contact forces
     a.cf_force = b->cf_force.get(); a.cf_steps = b->cf_steps.get(); a.cf_n = (int)b->contact_bodies.size();
     std::memcpy(a.cf_body, b->contact_bodies.data(), b->contact_bodies.size());
+  }
+  if (phase_mask == 0 && !b->imu_body.empty()) {   // likewise the IMU readings
+    a.imu_lin = b->imu_lin.get(); a.imu_ang = b->imu_ang.get(); a.imu_n = (int)b->imu_body.size();
+    std::memcpy(a.imu_body, b->imu_body.data(), b->imu_body.size());
+    std::memcpy(a.imu_pos, b->imu_pos.data(), b->imu_pos.size() * 4);
+    std::memcpy(a.imu_rot, b->imu_rot.data(), b->imu_rot.size() * 4);
   }
   a.ncontacts = b->ncontacts.get(); a.contacts = b->contacts.get(); a.contact_pt = b->contact_pt.get(); a.iters = b->iters.get(); a.diverged = b->diverged.get();
   a.resid = b->resid.get(); a.solver_status = b->solver_status.get();
@@ -1366,6 +1377,55 @@ int rsb_batch_get_body_contact_forces(rsb_batch* b, int env_begin, int env_count
   const size_t S = b->contact_bodies.size();
   rc = force ? copy_out(b, force, b->cf_force.get() + (size_t)env_begin * S * 3, (size_t)env_count * S * 3 * 4, where) : RSB_OK; if (rc) return rc;
   return steps_in_contact ? copy_out(b, steps_in_contact, b->cf_steps.get() + (size_t)env_begin * S, (size_t)env_count * S * 4, where) : RSB_OK;
+}
+// ---- IMU readings over a whole launch: the step kernel accumulates them sub-step by sub-step into the batch's rows -------------------
+int rsb_batch_set_imus(rsb_batch* b, const int32_t* body, const float* pos, const float* rot, int n) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (n < 0 || n > RSB_MAX_IMUS) return fail(RSB_ERR_INVALID, "at most " + std::to_string(RSB_MAX_IMUS) + " IMUs per batch (got " + std::to_string(n) + ")");
+  if (n > 0 && (!body || !pos)) return fail(RSB_ERR_INVALID, "null IMU body or position list");
+  std::vector<float> R(9 * (size_t)n);
+  for (int k = 0; k < n; k++) {
+    const std::string who = "IMU " + std::to_string(k) + ": ";
+    if (body[k] < 0 || body[k] >= b->nb) return fail(RSB_ERR_INVALID, who + "body index out of range (the model has " + std::to_string(b->nb) + ")");
+    for (int c = 0; c < 3; c++)
+      if (!std::isfinite(pos[3 * k + c])) return fail(RSB_ERR_INVALID, who + "position is not finite");
+    for (int c = 0; c < 9; c++) {
+      R[9 * k + c] = rot ? rot[9 * k + c] : (c % 4 == 0 ? 1.f : 0.f);
+      if (!std::isfinite(R[9 * k + c])) return fail(RSB_ERR_INVALID, who + "rotation is not finite");
+    }
+    const float* r = &R[9 * k];
+    double dev = 0.0;   // largest entry of |R^T R - I|
+    for (int i = 0; i < 3; i++)
+      for (int j = 0; j < 3; j++) {
+        double e = (i == j) ? -1.0 : 0.0;
+        for (int m = 0; m < 3; m++) e += (double)r[3 * m + i] * (double)r[3 * m + j];
+        dev = std::max(dev, std::fabs(e));
+      }
+    const double det = (double)r[0] * ((double)r[4] * r[8] - (double)r[5] * r[7]) - (double)r[1] * ((double)r[3] * r[8] - (double)r[5] * r[6]) +
+                       (double)r[2] * ((double)r[3] * r[7] - (double)r[4] * r[6]);
+    if (!(dev <= 1e-4) || !(det > 0.0)) return fail(RSB_ERR_INVALID, who + "orientation is not a rotation (|R^T R - I| <= 1e-4 and det R > 0 needed)");
+  }
+  if (n == 0) { b->imu_body.clear(); b->imu_pos.clear(); b->imu_rot.clear(); return RSB_OK; }
+  CK(cudaSetDevice(b->device));
+  const size_t words = (size_t)b->N * RSB_MAX_IMUS * 3;
+  CK(b->imu_lin.ensure(words * 4, b->stream));
+  CK(b->imu_ang.ensure(words * 4, b->stream));
+  // the rows of a new list read zero until a launch advances the state (in stream order: a step enqueued before this call still wrote the old layout)
+  CK(cudaMemsetAsync(b->imu_lin.get(), 0, words * 4, b->stream));
+  CK(cudaMemsetAsync(b->imu_ang.get(), 0, words * 4, b->stream));
+  b->imu_body.assign(body, body + n);
+  b->imu_pos.assign(pos, pos + 3 * (size_t)n);
+  b->imu_rot = R;
+  return RSB_OK;
+}
+int rsb_batch_get_imu_readings(rsb_batch* b, int env_begin, int env_count, float* lin_acc, float* ang_vel, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (b->imu_body.empty()) return fail(RSB_ERR_INVALID, "no IMUs: call rsb_batch_set_imus() first");
+  if (env_count == 0) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  const size_t I = b->imu_body.size();
+  rc = lin_acc ? copy_out(b, lin_acc, b->imu_lin.get() + (size_t)env_begin * I * 3, (size_t)env_count * I * 3 * 4, where) : RSB_OK; if (rc) return rc;
+  return ang_vel ? copy_out(b, ang_vel, b->imu_ang.get() + (size_t)env_begin * I * 3, (size_t)env_count * I * 3 * 4, where) : RSB_OK;
 }
 // ---- terrain height scans: the surface height under body-attached sample points, one launch of rsb_height_scan_kernel -------------
 int rsb_batch_set_height_scan(rsb_batch* b, const int32_t* body, const float* xy, int n, int align) {

@@ -237,6 +237,14 @@ struct StepArgs {
   int* cf_steps;       // [N][cf_n] sub-steps in which the body had a contact in the list
   int cf_n;
   uint8_t cf_body[RSB_MAX_CONTACT_BODIES];
+  // IMU readings over the whole launch (rsb_batch_set_imus); imu_lin null = no sensors set or the launch does not advance the state.
+  // Sensor k hangs on body imu_body[k] at imu_pos[k] with orientation imu_rot[k] (row-major), both in the body frame
+  float* imu_lin;      // [N][imu_n][3] mean specific force in the sensor frame: the row itself is the accumulator over the sub-steps
+  float* imu_ang;      // [N][imu_n][3] mean angular rate in the sensor frame, likewise
+  int imu_n;
+  uint8_t imu_body[RSB_MAX_IMUS];
+  float imu_pos[RSB_MAX_IMUS][3];
+  float imu_rot[RSB_MAX_IMUS][9];
   float *dbg_M, *dbg_h, *dbg_R, *dbg_p;   // optional (integrate1 / getters)
   float* obs;          // optional [N][ob_dim]: RaisimGym observation row of the final state, written by this kernel
   int ob_dim;
@@ -419,6 +427,91 @@ __device__ __forceinline__ float rsqrt_nr(float x) {
   float r;
   asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r * (1.5f - 0.5f * x * r * r);
+}
+
+// IMU sensor `lane` (rsb_batch_set_imus, lane < imu_n) at the end of stage E of sub-step `sub`, before the state update: s_gc, s_gv hold
+// the sub-step's start state (q_s, v_s) and s_rhs the velocity change dv of stage E.  The lane walks its body's chain from the root with
+// stage A's classical-acceleration recursion plus the generalized acceleration qdd = dv / dt, and carries the angular velocity of
+// v_s + dv (the sum stage E stores) beside it.  It does not use stage A's poses: from stage C on the Delassus matrix G overlays them
+// whenever there is a constraint row.  The accumulator is the environment's own output row, which only this lane touches: stored at the
+// first sub-step, read back and added to at the later ones, scaled by 1 / substeps at the last.
+__device__ __forceinline__ void imu_substep(const StepArgs& args, int env, int sub, int lane, const float* bodyf, const int* bodyi,
+                                            const int* anc, int nbp, int floating, bool jrot_identity, const float* s_gc,
+                                            const float* s_gv, const float* s_rhs) {
+  float* lo = args.imu_lin + ((size_t)env * args.imu_n + lane) * 3;
+  float* ao = args.imu_ang + ((size_t)env * args.imu_n + lane) * 3;
+  f3 acc_f = mk(0.f, 0.f, 0.f), acc_w = mk(0.f, 0.f, 0.f);
+  if (sub > 0) { acc_f = mk(lo[0], lo[1], lo[2]); acc_w = mk(ao[0], ao[1], ao[2]); }   // issued before the walk, which hides the L2 round trip
+  const float idt = 1.0f / args.prm.dt;
+  float R[9];
+  f3 w, w1, wd, vd;      // angular velocity at v_s and at v_s + dv, angular and classical linear acceleration of the body origin
+  if (floating) {
+    float qw = s_gc[3], qx = s_gc[4], qy = s_gc[5], qz = s_gc[6];
+    const float inv = 1.0f / sqrtf(qw * qw + qx * qx + qy * qy + qz * qz);
+    qw *= inv; qx *= inv; qy *= inv; qz *= inv;
+    R[0] = 1.f - 2.f * (qy * qy + qz * qz); R[1] = 2.f * (qx * qy - qw * qz); R[2] = 2.f * (qx * qz + qw * qy);
+    R[3] = 2.f * (qx * qy + qw * qz); R[4] = 1.f - 2.f * (qx * qx + qz * qz); R[5] = 2.f * (qy * qz - qw * qx);
+    R[6] = 2.f * (qx * qz - qw * qy); R[7] = 2.f * (qy * qz + qw * qx); R[8] = 1.f - 2.f * (qx * qx + qy * qy);
+    w = mk(s_gv[3], s_gv[4], s_gv[5]);
+    w1 = mk(s_gv[3] + s_rhs[3], s_gv[4] + s_rhs[4], s_gv[5] + s_rhs[5]);
+    wd = idt * mk(s_rhs[3], s_rhs[4], s_rhs[5]);
+    vd = idt * mk(s_rhs[0], s_rhs[1], s_rhs[2]);
+  } else {
+#pragma unroll
+    for (int k = 0; k < 9; k++) R[k] = bodyf[(BF_JROT + k) * nbp];
+    w = w1 = wd = vd = mk(0.f, 0.f, 0.f);
+  }
+  vd = vd - mk(args.prm.gravity[0], args.prm.gravity[1], args.prm.gravity[2]);
+  const int b = args.imu_body[lane];
+  const int depth = bodyi[BF_DEPTH * nbp + b];
+#pragma unroll 1
+  for (int d = 1; d <= depth; d++) {
+    const int j = anc[(d - 1) * nbp + b];
+    const f3 jp = mk(bodyf[(BF_JPOS + 0) * nbp + j], bodyf[(BF_JPOS + 1) * nbp + j], bodyf[(BF_JPOS + 2) * nbp + j]);
+    const f3 al = mk(bodyf[(BF_AXIS + 0) * nbp + j], bodyf[(BF_AXIS + 1) * nbp + j], bodyf[(BF_AXIS + 2) * nbp + j]);
+    float Rj[9];
+    if (jrot_identity) {
+#pragma unroll
+      for (int k = 0; k < 9; k++) Rj[k] = R[k];
+    } else {
+      float Jr[9];
+#pragma unroll
+      for (int k = 0; k < 9; k++) Jr[k] = bodyf[(BF_JROT + k) * nbp + j];
+      matmul3(R, Jr, Rj);
+    }
+    const f3 aj = mulR(Rj, al);
+    const int vi = bodyi[BF_VIDX * nbp + j];
+    const float q = s_gc[bodyi[BF_QIDX * nbp + j]], qd = s_gv[vi], dq = s_rhs[vi];
+    const bool rev = bodyi[BF_JTYPE * nbp + j] == 1;
+    f3 r = mulR(R, jp);
+    if (!rev) r = r + q * aj;
+    vd = vd + cross(wd, r) + cross(w, cross(w, r));
+    const f3 qa = qd * aj, qdda = (dq * idt) * aj;
+    if (rev) {
+      float sq, cq;
+      sincosf(q, &sq, &cq);
+      const float t = 1.f - cq;
+      const float Rq[9] = {t * al.x * al.x + cq, t * al.x * al.y - sq * al.z, t * al.x * al.z + sq * al.y,
+                           t * al.x * al.y + sq * al.z, t * al.y * al.y + cq, t * al.y * al.z - sq * al.x,
+                           t * al.x * al.z - sq * al.y, t * al.y * al.z + sq * al.x, t * al.z * al.z + cq};
+      matmul3(Rj, Rq, R);
+      wd = wd + cross(w, qa) + qdda;
+      w = w + qa;
+      w1 = w1 + (qd + dq) * aj;
+    } else {
+#pragma unroll
+      for (int k = 0; k < 9; k++) R[k] = Rj[k];
+      vd = vd + 2.f * cross(w, qa) + qdda;
+    }
+  }
+  // the sensor point: a = a_origin + wd x r + w x (w x r), r = R pos; both readings turned into the sensor frame, (R rot)^T = rot^T R^T
+  const f3 rs = mulR(R, mk(args.imu_pos[lane][0], args.imu_pos[lane][1], args.imu_pos[lane][2]));
+  const f3 fb = mulRt(R, vd + cross(wd, rs) + cross(w, cross(w, rs))), wb = mulRt(R, w1);
+  const float* Ro = args.imu_rot[lane];
+  f3 f = acc_f + mulRt(Ro, fb), g = acc_w + mulRt(Ro, wb);
+  if (sub == args.substeps - 1) { const float s = 1.0f / (float)args.substeps; f = s * f; g = s * g; }
+  lo[0] = f.x; lo[1] = f.y; lo[2] = f.z;
+  ao[0] = g.x; ao[1] = g.y; ao[2] = g.z;
 }
 
 // ---- compile-time topology: floating base + four serial chains of three joints (every 12-joint quadruped) -------------
@@ -1804,6 +1897,10 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
           }
           __syncwarp();
         }
+      }
+      if (args.imu_lin) {   // IMU readings (rsb_batch_set_imus): a launch-uniform branch
+        if (lane < args.imu_n) imu_substep(args, env, sub, lane, bodyf, bodyi, anc, nbp, floating, (H.flags & 1) != 0, s_gc, s_gv, s_rhs);
+        __syncwarp();       // every sensor lane has read v_s before the update below overwrites it
       }
 #pragma unroll 1
       for (int i = lane; i < nv; i += 32) {

@@ -111,6 +111,16 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void body_contact_forces(uintptr_t force_dev, uintptr_t steps_dev) {
     check(rsb_batch_get_body_contact_forces(b_, 0, view_.num_envs, reinterpret_cast<float*>(force_dev), reinterpret_cast<int32_t*>(steps_dev), RSB_DEVICE), "body_contact_forces");
   }
+  // IMU sensors shared by all environments: body [I], pos [I*3] and rot [I*9] (empty: identity) in the body frame (empty body clears)
+  void set_imus(const std::vector<int32_t>& body, const std::vector<float>& pos, const std::vector<float>& rot) {
+    if (pos.size() != 3 * body.size() || (!rot.empty() && rot.size() != 9 * body.size())) throw std::runtime_error("set_imus: need 3 positions and 0 or 9 rotation entries per sensor");
+    check(rsb_batch_set_imus(b_, body.data(), pos.data(), rot.empty() ? nullptr : rot.data(), (int)body.size()), "set_imus");
+  }
+  // their mean specific force and angular rate over the last stepping launch into tensor addresses ([num_envs, I, 3] float32, contiguous,
+  // sensor frames); 0 skips an output.  A copy in the batch's stream order: no launch
+  void imu_readings(uintptr_t lin_dev, uintptr_t ang_dev) {
+    check(rsb_batch_get_imu_readings(b_, 0, view_.num_envs, reinterpret_cast<float*>(lin_dev), reinterpret_cast<float*>(ang_dev), RSB_DEVICE), "imu_readings");
+  }
   // terrain height-scan points shared by all environments: body [P], xy [P*2] horizontal offsets, align "yaw" or "world" (empty clears)
   void set_height_scan(const std::vector<int32_t>& body, const std::vector<float>& xy, const std::string& align) {
     if (xy.size() != 2 * body.size()) throw std::runtime_error("set_height_scan: need 2 offset entries per point");
@@ -208,6 +218,8 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("frame_jacobians", &Batch::frame_jacobians, py::arg("jac_dev"))
       .def("set_contact_bodies", &Batch::set_contact_bodies, py::arg("body"))
       .def("body_contact_forces", &Batch::body_contact_forces, py::arg("force_dev"), py::arg("steps_dev"))
+      .def("set_imus", &Batch::set_imus, py::arg("body"), py::arg("pos"), py::arg("rot") = std::vector<float>())
+      .def("imu_readings", &Batch::imu_readings, py::arg("lin_acc_dev"), py::arg("ang_vel_dev"))
       .def("set_height_scan", &Batch::set_height_scan, py::arg("body"), py::arg("xy"), py::arg("align") = std::string("yaw"))
       .def("height_scan", &Batch::height_scan, py::arg("height_dev"), py::arg("xy_dev"))
       .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
