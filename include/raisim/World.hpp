@@ -121,7 +121,7 @@ struct LockStep {
   Rows<float> actuator;                     // [nv][3] kp, kd, effort limit (setPdGains / setActuationLimits; -1: the batch's); empty until the first one
   Rows<int32_t> delay;                      // [1] ArticulatedSystem::setActuationDelay since the last upload (-1: unchanged); empty until the first one
   Rows<char> actHistReset;                  // [1] ArticulatedSystem::resetActuatorHistory() since the last upload
-  size_t actHistWords = 0;                  // words of one environment's actuator-network history (0: no network, or history 1)
+  size_t actHistWords = 0;                  // words of one environment's actuator-network history or LSTM state (0: no network, or history 1)
   // rows the device fills: deferred, every environment's, valid until the next launch (the height scan: until the next state write or
   // terrain upload); immediate, the reader's row of the last read
   Rows<float> tauApplied, cfForce, scan, scanXy;   // [nv], [S][3] and [S] of the contact bodies (setContactBodies), [P] and [P][2] of the scan
@@ -529,7 +529,7 @@ class BatchedWorld {
   // the learned actuator network (ArticulatedSystem::setActuatorNetwork): one for the batch.  Setting it zeroes every history, so a
   // repeat of the network already set (every environment of a VectorizedEnvironment sets it in its constructor) is not passed on
   void setActuatorNetwork(const std::vector<int32_t>& dofs, int history, int layers, int width, const std::vector<float>& params) {
-    if (dofs == anDofs_ && history == anH_ && layers == anL_ && width == anW_ && params == anParams_) return;
+    if (!anLstm_ && dofs == anDofs_ && history == anH_ && layers == anL_ && width == anW_ && params == anParams_) return;
     if (!dofs.empty()) {
       const size_t count = size_t(2 * history) * width + width + size_t(layers - 1) * (size_t(width) * width + width) + width + 1;
       if (history < 1 || layers < 1 || width < 1 || params.size() != count)
@@ -537,8 +537,23 @@ class BatchedWorld {
                                  ", " + std::to_string(layers) + " layers of width " + std::to_string(width));
     }
     rsbCheck(rsb_batch_set_actuator_network(batch_, dofs.data(), int(dofs.size()), history, layers, width, params.data()), "setActuatorNetwork");
-    anDofs_ = dofs; anH_ = history; anL_ = layers; anW_ = width; anParams_ = params;
+    anLstm_ = false; anDofs_ = dofs; anH_ = history; anL_ = layers; anW_ = width; anParams_ = params;
     ls_.actHistWords = dofs.empty() ? 0 : dofs.size() * 2 * size_t(history - 1); ls_.actHistReset = {};
+  }
+  // the LSTM actuator network (ArticulatedSystem::setActuatorLstm), in place of any network set before; a repeat of the one already
+  // set is not passed on, as for setActuatorNetwork
+  void setActuatorLstm(const std::vector<int32_t>& dofs, int layers, int hidden, const std::vector<float>& params) {
+    if (anLstm_ && dofs == anDofs_ && layers == anL_ && hidden == anW_ && params == anParams_) return;
+    if (!dofs.empty()) {
+      size_t count = size_t(hidden) + 1;
+      for (int l = 0; l < layers; l++) count += size_t(4 * hidden) * ((l == 0 ? 2 : hidden) + hidden + 2);
+      if (layers < 1 || hidden < 1 || params.size() != count)
+        throw std::runtime_error("setActuatorLstm: " + std::to_string(params.size()) + " parameters for " + std::to_string(layers) +
+                                 " layers of hidden size " + std::to_string(hidden));
+    }
+    rsbCheck(rsb_batch_set_actuator_lstm(batch_, dofs.data(), int(dofs.size()), layers, hidden, params.data()), "setActuatorLstm");
+    anLstm_ = true; anDofs_ = dofs; anH_ = 0; anL_ = layers; anW_ = hidden; anParams_ = params;
+    ls_.actHistWords = dofs.size() * size_t(layers) * 2 * size_t(hidden); ls_.actHistReset = {};
   }
   // zero environment env's actuator history, and set its actuation delay in sub-steps (ArticulatedSystem::setActuationDelay)
   void resetActuatorHistory(int env) { ls_.resetActuatorHistory(env); }
@@ -559,6 +574,7 @@ class BatchedWorld {
   std::vector<int32_t> scanBodies_;
   std::vector<float> scanXy_;
   std::vector<int32_t> anDofs_;
+  bool anLstm_ = false;                  // anDofs_ .. anParams_ describe the LSTM (setActuatorLstm), else the MLP
   int anH_ = 0, anL_ = 0, anW_ = 0;
   std::vector<float> anParams_;
   bool scanYaw_ = true;
@@ -1074,7 +1090,13 @@ class ArticulatedSystem {
   void setActuatorNetwork(const std::vector<size_t>& dofs, int history, int layers, int width, const std::vector<float>& params) {
     w_->setActuatorNetwork(std::vector<int32_t>(dofs.begin(), dofs.end()), history, layers, width, params);
   }
-  // zero this environment's actuator-network history (setState keeps it): call it in reset()
+  // setActuatorLstm: the LSTM actuator network of rsb_batch_set_actuator_lstm (include/rsb.h) for the dofs listed, with params in
+  // torch.nn.LSTM order (weight_ih_l0, weight_hh_l0, bias_ih_l0, bias_hh_l0, ..., then the read-out weight and bias).  It replaces any
+  // network set before and belongs to the batch as setActuatorNetwork's does.  Setting it zeroes every (h, c) state.
+  void setActuatorLstm(const std::vector<size_t>& dofs, int layers, int hidden, const std::vector<float>& params) {
+    w_->setActuatorLstm(std::vector<int32_t>(dofs.begin(), dofs.end()), layers, hidden, params);
+  }
+  // zero this environment's actuator-network history, or the LSTM's (h, c) state (setState keeps either): call it in reset()
   void resetActuatorHistory() { w_->resetActuatorHistory(env_); }
   // setActuationDelay: from now on every joint command (PD targets, feed-forward torque) of this robot takes effect subSteps physics
   // sub-steps after it was set (rsb_batch_set_actuation_delay, include/rsb.h); setting it empties the command history, so the first

@@ -290,7 +290,27 @@ int rsb_batch_clear_actuator_params(rsb_batch* b);
 #define RSB_ACTNET_MAX_LAYERS 4
 #define RSB_ACTNET_MAX_WIDTH 32
 int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs, int history, int layers, int width, const float* params);
-/* History rows [env_count][n_dofs][2][H - 1] float32 (errors then velocities, most recent first), host or device (`where`).  rows ==
+/* Learned LSTM actuator network (the model legged_gym and Isaac Lab use for ANYmal): the torque of each listed dof is the read-out of a
+ * torch.nn.LSTM over its (position error, velocity), whose hidden and cell state each environment carries from sub-step to sub-step.
+ *   One actuator network per batch: this call and rsb_batch_set_actuator_network each replace whichever network is set, and n_dofs = 0
+ *   in either clears it.  The dof rules, the torque (tau_ff + net: explicit, saturated at the effort limit, reported by
+ *   rsb_batch_get_generalized_force; kp, kd and the velocity target of the dof ignored), PD mode only, and the launches that advance it
+ *   are the MLP's above.  A set LSTM counts as PD gains for rsb_batch_gym_step.
+ *   Input: x = [e, v], the MLP's e and v of the sub-step's start (with an actuation delay, e is taken on the applied command).
+ *   Cell (torch gate order i, f, g, o): i = sigmoid(W_ii x + b_ii + W_hi h + b_hi), f and o likewise, g = tanh(...), c' = f c + i g,
+ *   h' = o tanh(c'); layer k > 0 takes layer k - 1's h' as its x.  Output net = w_out . h'_L + b_out.
+ *   params in torch order (host memory): per layer weight_ih_l{k}[4 hidden][n_in], weight_hh_l{k}[4 hidden][hidden], bias_ih_l{k}[4 hidden],
+ *   bias_hh_l{k}[4 hidden], with n_in = 2 for layer 0 and hidden after it; then the read-out weight[1][hidden], bias[1]:
+ *   sum over layers of 4 hidden (n_in + hidden + 2), plus hidden + 1 floats.  layers in [1, RSB_ACTNET_MAX_LAYERS], hidden in
+ *   [1, RSB_ACTNET_MAX_WIDTH].
+ *   State: per environment and listed dof, (h, c) of every layer, read and written with rsb_batch_{get,set}_actuator_history.  Every
+ *   advancing launch steps the cell once per sub-step.  This call, rsb_batch_gym_reset and a termination in rsb_batch_gym_step (that
+ *   environment's rows) zero it; rsb_batch_set_state does not.
+ *   Refused with RSB_ERR_INVALID, changing nothing (the old network and its state stay): a null batch, n_dofs outside [0, nv], a NULL,
+ *   out-of-range, duplicated or base dof, layers or hidden out of range, NULL params with n_dofs > 0, a parameter that is not finite. */
+int rsb_batch_set_actuator_lstm(rsb_batch* b, const int32_t* dofs, int n_dofs, int layers, int hidden, const float* params);
+/* History rows of the network that is set, float32, host or device (`where`): for the MLP [env_count][n_dofs][2][H - 1] (errors then
+ * velocities, most recent first), for the LSTM [env_count][n_dofs][layers][2][hidden] (h then c of every layer).  rows ==
  * NULL zeroes the range.  The rows are checked on the device in the batch's staging buffer before any of them is committed; the call
  * waits for that check.  With H = 1 the rows have no words and both calls succeed without doing anything.  Refused with
  * RSB_ERR_INVALID, changing nothing: a null batch, no network, a bad range or `where`, a value that is not finite. */

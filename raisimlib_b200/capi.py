@@ -146,6 +146,7 @@ SIGNATURES = {
     "rsb_batch_set_actuator_network": [_P, _P, _I, _I, _I, _I, _P],
     "rsb_batch_set_actuator_history": [_P, _P, _I, _I, _I],
     "rsb_batch_get_actuator_history": [_P, _P, _I, _I, _I],
+    "rsb_batch_set_actuator_lstm": [_P, _P, _I, _I, _I, _P],
     "rsb_batch_set_actuation_delay": [_P, _P, _I, _I, _I],
     "rsb_batch_clear_actuation_delay": [_P],
     "rsb_batch_integrate1": [_P],
@@ -259,6 +260,52 @@ def _network_layers(layers):
     return out
 
 
+ACTNET_MAX_LAYERS, ACTNET_MAX_WIDTH = 4, 32     # RSB_ACTNET_MAX_LAYERS, RSB_ACTNET_MAX_WIDTH of include/rsb.h
+
+
+def _lstm_params(lstm, readout):
+    """(layers, hidden, float32 parameters in the order of rsb_batch_set_actuator_lstm) of an LSTM actuator network.  lstm: a
+    torch.nn.LSTM, or a list of per-layer (weight_ih, weight_hh, bias_ih, bias_hh) arrays in torch order; readout: a
+    torch.nn.Linear(hidden, 1) or a (weight [1, hidden], bias [1]) pair"""
+    if hasattr(lstm, "all_weights") and hasattr(lstm, "hidden_size"):
+        if lstm.input_size != 2:
+            raise ValueError(f"set_actuator_lstm: the LSTM's input_size must be 2 (position error, velocity), got {lstm.input_size}")
+        if not lstm.bias:
+            raise ValueError("set_actuator_lstm: the LSTM needs its biases (bias=True)")
+        if lstm.bidirectional:
+            raise ValueError("set_actuator_lstm: a bidirectional LSTM cannot run one step at a time")
+        if getattr(lstm, "proj_size", 0) > 0:
+            raise ValueError("set_actuator_lstm: a projected LSTM (proj_size > 0) is not supported")
+        sd = lstm.state_dict()
+        lstm = [tuple(sd[f"{k}_l{l}"].detach().cpu().numpy() for k in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+                for l in range(lstm.num_layers)]
+    layers = [tuple(np.asarray(a, np.float32) for a in p) for p in lstm]
+    if any(len(p) != 4 for p in layers):
+        raise ValueError("set_actuator_lstm: every layer needs (weight_ih, weight_hh, bias_ih, bias_hh)")
+    if not 1 <= len(layers) <= ACTNET_MAX_LAYERS:
+        raise ValueError(f"set_actuator_lstm: {len(layers)} layers outside [1, {ACTNET_MAX_LAYERS}]")
+    hidden = layers[0][1].shape[1] if layers[0][1].ndim == 2 else -1
+    if not 1 <= hidden <= ACTNET_MAX_WIDTH:
+        raise ValueError(f"set_actuator_lstm: hidden size {hidden} outside [1, {ACTNET_MAX_WIDTH}]")
+    for l, (wih, whh, bih, bhh) in enumerate(layers):
+        nin = 2 if l == 0 else hidden
+        want = ((4 * hidden, nin), (4 * hidden, hidden), (4 * hidden,), (4 * hidden,))
+        got = (wih.shape, whh.shape, bih.shape, bhh.shape)
+        if got != want:
+            raise ValueError(f"set_actuator_lstm: layer {l}: need weight_ih, weight_hh, bias_ih, bias_hh of shapes {want}, got {got}")
+    if hasattr(readout, "weight") and hasattr(readout, "in_features"):
+        if readout.bias is None:
+            raise ValueError("set_actuator_lstm: the read-out Linear needs a bias")
+        readout = (readout.weight.detach().cpu().numpy(), readout.bias.detach().cpu().numpy())
+    if len(readout) != 2:
+        raise ValueError("set_actuator_lstm: the read-out must be a Linear or a (weight, bias) pair")
+    wo, bo = (np.asarray(a, np.float32) for a in readout)
+    if wo.shape != (1, hidden) or bo.shape != (1,):
+        raise ValueError(f"set_actuator_lstm: the read-out needs weight (1, {hidden}) and bias (1,), got {wo.shape} and {bo.shape}")
+    params = np.concatenate([a.ravel() for p in layers for a in p] + [wo.ravel(), bo.ravel()])
+    return len(layers), hidden, np.ascontiguousarray(params, np.float32)
+
+
 class Model:
     def __init__(self, path_or_xml, cache=False):
         """URDF path / XML text, or (cache=True) a binary model cache written by Model.save()"""
@@ -324,6 +371,7 @@ class Batch:
         self.device, self.nframes, self.ncontact_bodies, self.nscan, self.nimus = device, 0, 0, 0, 0
         self.hm_shape = None                 # (ys, xs) of the height map(s) set through this object
         self.an_shape = None                 # (listed dofs, history) of the actuator network set through this object
+        self.lstm_shape = None               # (listed dofs, layers, hidden) of the LSTM actuator network set through this object
 
     def __del__(self):
         if getattr(self, "h", None) and lib is not None and _lib is not None:
@@ -801,18 +849,10 @@ class Batch:
         (W, b) numpy pairs, torch.nn.Linear order (W [width, 2 * history], b [width], ..., W [1, width], b [1]), or a torch.nn.Sequential
         of Linear and Softsign only (Linear, Softsign, ..., Linear).  Input features: [e_t .. e_{t-H+1}, v_t .. v_{t-H+1}].  An empty
         dof list clears the network.  Every call zeroes all histories; a refused call changes nothing."""
-        names = list(dofs_or_joint_names)
-        if any(isinstance(d, str) for d in names):
-            t = self.model.tables()
-            by_name = {nm: int(t["vidx"][i]) for i, nm in enumerate(t["joint_names"]) if i > 0}
-            missing = [d for d in names if isinstance(d, str) and d not in by_name]
-            if missing:
-                raise ValueError(f"set_actuator_network: unknown joints {missing}")
-            names = [by_name[d] if isinstance(d, str) else d for d in names]
-        dofs = np.ascontiguousarray(names, np.int32).reshape(-1)
+        dofs = self._an_dofs(dofs_or_joint_names, "set_actuator_network")
         if len(dofs) == 0:
             _ck(lib().rsb_batch_set_actuator_network(self.h, None, 0, 0, 0, 0, None))
-            self.an_shape = None
+            self.an_shape = self.lstm_shape = None
             return
         pairs = _network_layers(layers)
         H = int(history)
@@ -826,15 +866,48 @@ class Batch:
         params = np.ascontiguousarray(np.concatenate([np.concatenate([w.ravel(), b.ravel()]) for w, b in pairs]), np.float32)
         _ck(lib().rsb_batch_set_actuator_network(self.h, dofs.ctypes.data_as(C.c_void_p), len(dofs), H, len(pairs) - 1, width,
                                                  params.ctypes.data_as(C.c_void_p)))
-        self.an_shape = (len(dofs), H)
+        self.an_shape, self.lstm_shape = (len(dofs), H), None
+
+    def _an_dofs(self, dofs_or_joint_names, who):
+        """int32 gv indices of a dof list given as indices or joint names"""
+        names = list(dofs_or_joint_names)
+        if any(isinstance(d, str) for d in names):
+            t = self.model.tables()
+            by_name = {nm: int(t["vidx"][i]) for i, nm in enumerate(t["joint_names"]) if i > 0}
+            missing = [d for d in names if isinstance(d, str) and d not in by_name]
+            if missing:
+                raise ValueError(f"{who}: unknown joints {missing}")
+            names = [by_name[d] if isinstance(d, str) else d for d in names]
+        return np.ascontiguousarray(names, np.int32).reshape(-1)
+
+    def set_actuator_lstm(self, dofs_or_joint_names, lstm, readout):
+        """One LSTM actuator network for the batch, in place of any network set before: at every sub-step the step kernel advances
+        the cell of each listed dof (gv indices, or joint names) on x = (ptarget - q, v) and applies tau_ff + readout(h) in place of
+        the dof's PD law.  lstm: a torch.nn.LSTM (input_size 2, bias, not bidirectional, no projection; batch_first does not matter)
+        or a list of per-layer (weight_ih, weight_hh, bias_ih, bias_hh) arrays in torch order; readout: a torch.nn.Linear(hidden, 1)
+        with bias, or a (weight [1, hidden], bias [1]) pair.  An empty dof list clears the network.  Every call zeroes all states; a
+        refused call changes nothing."""
+        dofs = self._an_dofs(dofs_or_joint_names, "set_actuator_lstm")
+        if len(dofs) == 0:
+            _ck(lib().rsb_batch_set_actuator_lstm(self.h, None, 0, 0, 0, None))
+            self.an_shape = self.lstm_shape = None
+            return
+        layers, hidden, params = _lstm_params(lstm, readout)
+        _ck(lib().rsb_batch_set_actuator_lstm(self.h, dofs.ctypes.data_as(C.c_void_p), len(dofs), layers, hidden,
+                                              params.ctypes.data_as(C.c_void_p)))
+        self.an_shape, self.lstm_shape = None, (len(dofs), layers, hidden)
 
     def _an_rows(self):
+        if getattr(self, "lstm_shape", None) is not None:
+            n, layers, hidden = self.lstm_shape
+            return (n, layers, 2, hidden)
         if self.an_shape is None:
             raise ValueError("actuator history: no actuator network set through this object")
         return (self.an_shape[0], 2, self.an_shape[1] - 1)
 
     def actuator_history(self, env_begin=0, env_count=None):
-        """[n, dofs, 2, H - 1] float32: errors then velocities of the last H - 1 sub-steps of every listed dof, most recent first"""
+        """[n, dofs, 2, H - 1] float32: errors then velocities of the last H - 1 sub-steps of every listed dof, most recent first.
+        With an LSTM set: [n, dofs, layers, 2, hidden], h then c of every layer.  The same shapes hold for the variants below."""
         return self._read(lib().rsb_batch_get_actuator_history, self._an_rows(), np.float32, env_begin, env_count)
 
     def actuator_history_into(self, rows, env_begin=0, env_count=None):
@@ -850,8 +923,8 @@ class Batch:
             _ck(lib().rsb_batch_set_actuator_history(self.h, None, env_begin, self._count(env_begin, env_count), HOST))
             return
         r = np.ascontiguousarray(rows, np.float32)
-        if r.ndim != 4 or r.shape[1:] != shape:
-            raise ValueError(f"rows: need shape [n, {shape[0]}, {shape[1]}, {shape[2]}], got {r.shape}")
+        if r.ndim != 1 + len(shape) or r.shape[1:] != shape:
+            raise ValueError(f"rows: need shape [n, {', '.join(map(str, shape))}], got {r.shape}")
         _ck(lib().rsb_batch_set_actuator_history(self.h, r.ctypes.data_as(C.c_void_p), env_begin, r.shape[0], HOST))
 
     def set_actuator_history_from(self, rows, env_begin=0):

@@ -147,9 +147,11 @@ struct rsb_batch {
   // of the check a call's rows pass before they replace any of them
   EnvRows body_inertia, contact_friction, actuator;
   DevBuf<int> row_bad;
-  // learned actuator network of rsb_batch_set_actuator_network (an_dofs empty: none): its parameters as the step kernel reads them
-  // (ActNetDesc::params) and the history rows [N][n][2][H - 1]
+  // learned actuator network of rsb_batch_set_actuator_network (an_lstm false) or rsb_batch_set_actuator_lstm (an_lstm true; an_dofs
+  // empty: none): its parameters as the step kernel reads them (ActNetDesc::params) and the history rows, [N][n][2][H - 1] for the MLP,
+  // [N][n][L][2][W] for the LSTM
   std::vector<int32_t> an_dofs;
+  bool an_lstm = false;
   int an_H = 0, an_L = 0, an_W = 0;
   DevBuf<float> an_params, an_hist;
   // actuation delays of rsb_batch_set_actuation_delay while delay_active: (delay, sub-steps since the history was emptied) rows [N][2]
@@ -164,8 +166,10 @@ static int round_up(int x, int m) { return (x + m - 1) / m * m; }
 static bool pd_active(const rsb_batch* b) {
   return b->control_mode == RSB_PD_PLUS_FEEDFORWARD_TORQUE && (b->pd_set || b->actuator.active || !b->an_dofs.empty());
 }
-// words of one environment's actuator history rows
-static size_t an_hist_words(const rsb_batch* b) { return b->an_dofs.size() * 2 * (size_t)std::max(0, b->an_H - 1); }
+// words of one environment's actuator history rows (the LSTM's (h, c) of every layer)
+static size_t an_hist_words(const rsb_batch* b) {
+  return b->an_dofs.size() * 2 * (b->an_lstm ? (size_t)b->an_L * b->an_W : (size_t)std::max(0, b->an_H - 1));
+}
 
 // ------------------------------------------------------------------ blob ------------------------
 static void build_blob(const Model& md, const Overrides& ov, LaunchConfig& cfg) {
@@ -450,6 +454,7 @@ static int do_launch(rsb_batch* b, int substeps, int phase_mask, bool debug, con
   if (!b->an_dofs.empty() && a.use_pd) {   // the network and its history act in PD mode only
     a.an.params = b->an_params.get(); a.an.hist = b->an_hist.get();
     a.an.n = (int)b->an_dofs.size(); a.an.H = b->an_H; a.an.L = b->an_L; a.an.W = b->an_W;
+    a.an.lstm = b->an_lstm ? 1 : 0; a.an.words = (int)an_hist_words(b);
     for (int s = 0; s < a.an.n; s++) { a.an.dof[s] = (uint8_t)b->an_dofs[s]; a.an.mask |= 1ull << b->an_dofs[s]; }
   }
   if (b->delay_active && phase_mask == 0) { a.delay_state = b->delay_state.get(); a.delay_ring = b->delay_ring.get(); }   // only advancing launches record a command
@@ -1092,20 +1097,26 @@ int rsb_batch_clear_actuator_params(rsb_batch* b) {
   b->actuator.active = false;
   return RSB_OK;
 }
-// ---- learned actuator network (one per batch, shared by the listed dofs): checked and repacked on the host, the history on the device
-int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs, int history, int layers, int width, const float* params) {
-  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+// the dof list of an actuator network call: n_dofs in [1, nv], joint dofs only, none twice (who: the message prefix)
+static int check_an_dofs(const rsb_batch* b, const int32_t* dofs, int n_dofs, const char* who) {
   const int nv = b->nv, nbase = b->model->md.floating ? 6 : 0;
-  if (n_dofs < 0 || n_dofs > nv) return fail(RSB_ERR_INVALID, "actuator network: n_dofs " + std::to_string(n_dofs) + " outside [0, " + std::to_string(nv) + "]");
-  if (n_dofs == 0) { b->an_dofs.clear(); return RSB_OK; }
-  if (!dofs) return fail(RSB_ERR_INVALID, "actuator network: null dof list");
+  if (!dofs) return fail(RSB_ERR_INVALID, std::string(who) + ": null dof list");
   std::vector<char> seen(nv, 0);
   for (int s = 0; s < n_dofs; s++) {
     const int d = dofs[s];
-    if (d < nbase || d >= nv) return fail(RSB_ERR_INVALID, "actuator network: dof " + std::to_string(d) + " outside the actuated dofs [" + std::to_string(nbase) + ", " + std::to_string(nv) + ")");
-    if (seen[d]) return fail(RSB_ERR_INVALID, "actuator network: dof " + std::to_string(d) + " listed twice");
+    if (d < nbase || d >= nv) return fail(RSB_ERR_INVALID, std::string(who) + ": dof " + std::to_string(d) + " outside the actuated dofs [" + std::to_string(nbase) + ", " + std::to_string(nv) + ")");
+    if (seen[d]) return fail(RSB_ERR_INVALID, std::string(who) + ": dof " + std::to_string(d) + " listed twice");
     seen[d] = 1;
   }
+  return RSB_OK;
+}
+// ---- learned actuator network (one per batch, shared by the listed dofs): checked and repacked on the host, the history on the device
+int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs, int history, int layers, int width, const float* params) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  const int nv = b->nv;
+  if (n_dofs < 0 || n_dofs > nv) return fail(RSB_ERR_INVALID, "actuator network: n_dofs " + std::to_string(n_dofs) + " outside [0, " + std::to_string(nv) + "]");
+  if (n_dofs == 0) { b->an_dofs.clear(); return RSB_OK; }
+  int rc = check_an_dofs(b, dofs, n_dofs, "actuator network"); if (rc) return rc;
   if (history < 1 || history > RSB_ACTNET_MAX_HISTORY || layers < 1 || layers > RSB_ACTNET_MAX_LAYERS || width < 1 || width > RSB_ACTNET_MAX_WIDTH)
     return fail(RSB_ERR_INVALID, "actuator network: history, layers and width must lie in [1, " + std::to_string(RSB_ACTNET_MAX_HISTORY) + "], [1, " +
                                  std::to_string(RSB_ACTNET_MAX_LAYERS) + "] and [1, " + std::to_string(RSB_ACTNET_MAX_WIDTH) + "]");
@@ -1133,7 +1144,55 @@ int rsb_batch_set_actuator_network(rsb_batch* b, const int32_t* dofs, int n_dofs
   if (hist_words > 0) CK(cudaMemsetAsync(b->an_hist.get(), 0, hist_words * 4, b->stream));
   CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
   b->an_dofs.assign(dofs, dofs + n_dofs);
+  b->an_lstm = false;
   b->an_H = history; b->an_L = layers; b->an_W = width;
+  return RSB_OK;
+}
+int rsb_batch_set_actuator_lstm(rsb_batch* b, const int32_t* dofs, int n_dofs, int layers, int hidden, const float* params) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  const int nv = b->nv;
+  if (n_dofs < 0 || n_dofs > nv) return fail(RSB_ERR_INVALID, "actuator lstm: n_dofs " + std::to_string(n_dofs) + " outside [0, " + std::to_string(nv) + "]");
+  if (n_dofs == 0) { b->an_dofs.clear(); return RSB_OK; }
+  int rc = check_an_dofs(b, dofs, n_dofs, "actuator lstm"); if (rc) return rc;
+  if (layers < 1 || layers > RSB_ACTNET_MAX_LAYERS || hidden < 1 || hidden > RSB_ACTNET_MAX_WIDTH)
+    return fail(RSB_ERR_INVALID, "actuator lstm: layers and hidden must lie in [1, " + std::to_string(RSB_ACTNET_MAX_LAYERS) + "] and [1, " +
+                                 std::to_string(RSB_ACTNET_MAX_WIDTH) + "]");
+  if (!params) return fail(RSB_ERR_INVALID, "actuator lstm: null parameters");
+  const int W = hidden, W4 = 4 * hidden;
+  size_t count = (size_t)W + 1, packed = (size_t)W + 1;
+  for (int l = 0; l < layers; l++) {
+    const int nin = l == 0 ? 2 : W;
+    count += (size_t)W4 * (nin + W + 2);
+    packed += (size_t)W4 * (nin + W + 1);
+  }
+  for (size_t k = 0; k < count; k++)
+    if (!std::isfinite(params[k])) return fail(RSB_ERR_INVALID, "actuator lstm: parameter " + std::to_string(k) + " is not finite; nothing changed");
+  // torch.nn.LSTM order (weight_ih [4W][n_in], weight_hh [4W][W], bias_ih [4W], bias_hh [4W] per layer; read-out [1][W], [1]) ->
+  // ActNetDesc::params: per layer [n_in + W][4][W] (row g W + j of torch is gate g of unit j), then bias_ih + bias_hh [4][W]
+  std::vector<float> pk(packed);
+  size_t so = 0, po = 0;
+  for (int l = 0; l < layers; l++) {
+    const int nin = l == 0 ? 2 : W;
+    const float *wih = params + so, *whh = wih + (size_t)W4 * nin, *bih = whh + (size_t)W4 * W, *bhh = bih + W4;
+    for (int r = 0; r < W4; r++) {
+      for (int k = 0; k < nin; k++) pk[po + (size_t)k * W4 + r] = wih[(size_t)r * nin + k];
+      for (int k = 0; k < W; k++) pk[po + (size_t)(nin + k) * W4 + r] = whh[(size_t)r * W + k];
+      pk[po + (size_t)(nin + W) * W4 + r] = bih[r] + bhh[r];
+    }
+    so += (size_t)W4 * (nin + W + 2);
+    po += (size_t)W4 * (nin + W + 1);
+  }
+  for (int k = 0; k <= W; k++) pk[po + k] = params[so + k];   // read-out weights [W] and bias
+  CK(cudaSetDevice(b->device));
+  const size_t hist_words = (size_t)b->N * n_dofs * layers * 2 * W;
+  CK(b->an_params.ensure(packed * 4, b->stream));
+  CK(b->an_hist.ensure(hist_words * 4, b->stream));
+  CK(cudaMemcpyAsync(b->an_params.get(), pk.data(), packed * 4, cudaMemcpyHostToDevice, b->stream));
+  CK(cudaMemsetAsync(b->an_hist.get(), 0, hist_words * 4, b->stream));
+  CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
+  b->an_dofs.assign(dofs, dofs + n_dofs);
+  b->an_lstm = true;
+  b->an_H = 0; b->an_L = layers; b->an_W = W;
   return RSB_OK;
 }
 int rsb_batch_set_actuator_history(rsb_batch* b, const float* rows, int env_begin, int env_count, int where) {

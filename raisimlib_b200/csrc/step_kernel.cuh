@@ -194,14 +194,20 @@ struct GymConfig {
   float torque_coeff, forward_vel_coeff, terminal_reward;
 };
 
-// learned actuator network (rsb_batch_set_actuator_network), read by stage C; params == null: no network, or a launch that applies no
-// PD laws (force mode)
+// learned actuator network (rsb_batch_set_actuator_network: an MLP, or rsb_batch_set_actuator_lstm: an LSTM), read by stage C;
+// params == null: no network, or a launch that applies no PD laws (force mode)
 constexpr int AN_MAX_DOFS = 64;          // >= nv of every model (32 bodies)
 struct ActNetDesc {
-  const float* params;   // per hidden layer: weights transposed [n_in][W] (lanes read consecutive words), bias [W]; output weights [W], bias
-  float* hist;           // [num_envs][n][2][H - 1]: errors then velocities of the last H - 1 sub-steps, most recent first
+  // MLP: per hidden layer: weights transposed [n_in][W] (lanes read consecutive words), bias [W]; output weights [W], bias.
+  // LSTM: per layer: weights [n_in + W][4][W] (input then recurrent columns, gates i f g o), summed bias [4][W]; output weights [W], bias
+  const float* params;
+  // MLP: [num_envs][n][2][H - 1]: errors then velocities of the last H - 1 sub-steps, most recent first.
+  // LSTM: [num_envs][n][L][2][W]: h then c of every layer
+  float* hist;
   unsigned long long mask;   // bit i: dof i is listed
+  int lstm;                  // 0: the MLP, 1: the LSTM (H unused)
   int n, H, L, W;
+  int words;                 // hist words of one environment
   uint8_t dof[AN_MAX_DOFS];
 };
 
@@ -942,6 +948,109 @@ __device__ __forceinline__ void actuator_network(const ActNetDesc& an, int env, 
   }
 }
 
+// Stage C: the LSTM actuator network of every listed dof of environment env, one cell step per sub-step from x = (e, v) at its start;
+// net[i] = its output for listed dof i, and the environment's (h, c) rows advance in place.  The mapping is the MLP's: lane j is hidden
+// unit j and holds its four gate pre-activations for the AN_G dofs of a group, every weight load serving the whole group.  A layer's
+// pre-activations are accumulated in two passes over s_x ([input][AN_G], 16-byte broadcast loads): the layer input first, then this
+// layer's h of the last sub-step, so that the scratch never holds more than RSB_ACTNET_MAX_WIDTH inputs.  Every lane reads and writes
+// only its own unit's (h, c) words.  The evaluation order is fixed (bias, input columns, recurrent columns, one fmaf each), so the
+// result does not depend on the launch shape.
+__device__ __forceinline__ float an_sigmoid(float a) { return 1.f / (1.f + expf(-a)); }
+__device__ __forceinline__ void actuator_lstm(const ActNetDesc& an, int env, int lane, const float* s_gc, const float* s_gv, const float* s_pt,
+                                              const int* dofq, float* s_x, float* net) {
+  const int L = an.L, W = an.W, n = an.n, W4 = 4 * W;
+  const bool on = lane < W;
+  float* const st = an.hist + (size_t)env * an.words;
+#pragma unroll 1
+  for (int g0 = 0; g0 < n; g0 += AN_G) {
+    // layer 0's input: lane = (dof d of the group, feature k); 0 past the end of the list
+    if (lane < 2 * AN_G) {
+      const int d = lane >> 1, k = lane & 1, s = g0 + d;
+      float x = 0.f;
+      if (s < n) {
+        const int i = an.dof[s];
+        if (k) x = s_gv[i];
+        else { const int q = dofq[i]; x = s_pt[q] - s_gc[q]; }
+      }
+      s_x[k * AN_G + d] = x;
+    }
+    __syncwarp();
+    const float* p = an.params;
+    float h[AN_G] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 1
+    for (int l = 0, nin = 2; l < L; l++, nin = W) {
+      float a[4][AN_G];
+#pragma unroll
+      for (int g = 0; g < 4; g++) {
+        const float bg = on ? __ldg(p + (nin + W) * W4 + g * W + lane) : 0.f;
+#pragma unroll
+        for (int d = 0; d < AN_G; d++) a[g][d] = bg;
+      }
+      // pass 1: the layer input
+#pragma unroll 2
+      for (int k = 0; k < nin; k++) {
+        const float4 xk = *reinterpret_cast<const float4*>(s_x + k * AN_G);
+#pragma unroll
+        for (int g = 0; g < 4; g++) {
+          const float w = on ? __ldg(p + (k * 4 + g) * W + lane) : 0.f;
+          a[g][0] = fmaf(w, xk.x, a[g][0]); a[g][1] = fmaf(w, xk.y, a[g][1]); a[g][2] = fmaf(w, xk.z, a[g][2]); a[g][3] = fmaf(w, xk.w, a[g][3]);
+        }
+      }
+      __syncwarp();   // every lane has read the layer input
+      // this layer's state of the last sub-step: h staged for pass 2, c kept in the lane
+      float c[AN_G];
+#pragma unroll
+      for (int d = 0; d < AN_G; d++) {
+        h[d] = 0.f; c[d] = 0.f;
+        if (on && g0 + d < n) {
+          const float* r = st + ((size_t)((g0 + d) * L + l) * 2) * W + lane;
+          h[d] = r[0]; c[d] = r[W];
+        }
+      }
+      if (on) *reinterpret_cast<float4*>(s_x + lane * AN_G) = make_float4(h[0], h[1], h[2], h[3]);
+      __syncwarp();
+      // pass 2: the recurrent input
+      const float* pr = p + nin * W4;
+#pragma unroll 2
+      for (int k = 0; k < W; k++) {
+        const float4 xk = *reinterpret_cast<const float4*>(s_x + k * AN_G);
+#pragma unroll
+        for (int g = 0; g < 4; g++) {
+          const float w = on ? __ldg(pr + (k * 4 + g) * W + lane) : 0.f;
+          a[g][0] = fmaf(w, xk.x, a[g][0]); a[g][1] = fmaf(w, xk.y, a[g][1]); a[g][2] = fmaf(w, xk.z, a[g][2]); a[g][3] = fmaf(w, xk.w, a[g][3]);
+        }
+      }
+      // the cell (torch gate order i, f, g, o); lanes >= W end with h = c = 0
+#pragma unroll
+      for (int d = 0; d < AN_G; d++) {
+        const float ig = an_sigmoid(a[0][d]) * tanhf(a[2][d]);
+        c[d] = fmaf(an_sigmoid(a[1][d]), c[d], ig);
+        h[d] = an_sigmoid(a[3][d]) * tanhf(c[d]);
+        if (on && g0 + d < n) {
+          float* r = st + ((size_t)((g0 + d) * L + l) * 2) * W + lane;
+          r[0] = h[d];
+          r[W] = c[d];
+        }
+      }
+      p += (nin + W) * W4 + W4;
+      __syncwarp();   // every lane has read the recurrent input
+      if (on) *reinterpret_cast<float4*>(s_x + lane * AN_G) = make_float4(h[0], h[1], h[2], h[3]);   // the next layer's input
+      __syncwarp();
+    }
+    // read-out: a butterfly sum over the hidden units (lanes >= W hold 0)
+    const float wo = on ? __ldg(p + lane) : 0.f;
+    float o0 = wo * h[0], o1 = wo * h[1], o2 = wo * h[2], o3 = wo * h[3];
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) {
+      o0 += __shfl_xor_sync(FULL, o0, m); o1 += __shfl_xor_sync(FULL, o1, m);
+      o2 += __shfl_xor_sync(FULL, o2, m); o3 += __shfl_xor_sync(FULL, o3, m);
+    }
+    const float o = lane == 0 ? o0 : lane == 1 ? o1 : lane == 2 ? o2 : o3;
+    if (lane < AN_G && g0 + lane < n) net[an.dof[g0 + lane]] = __ldg(p + W) + o;
+    __syncwarp();   // s_x is refilled by the next group
+  }
+}
+
 // Stage C: the actuation delay of environment env at one advancing sub-step.  The command of a joint dof j (nbase + j) is the triple
 // (ptarget[q], vtarget, tau_ff); it goes into ring slot t % DELAY_SLOTS, and the one of sub-step max(t - d, 0) replaces it in s_pt,
 // s_vt and s_tau, where the PD law, the actuator network and stage E read it.  At sub-step 0 of a launch the command is what the
@@ -1460,7 +1569,11 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
       if constexpr (DL) actuation_delay(args.delay_state, args.delay_ring, env, sub, nbase, nv, dofq, s_pt, s_vt, s_tau, lane);
       // actuator network: a listed dof has no PD law and the feed-forward torque tau_ff + net, its network torque kept in s_vt (its
       // velocity target, which it does not use; reloaded by every launch) for stage E.  Scratch: the Anderson history of stage D
-      if constexpr (AN) { actuator_network(args.an, env, lane, s_gc, s_gv, s_pt, dofq, s_hist, s_vt); __syncwarp(); }
+      if constexpr (AN) {
+        if (args.an.lstm) actuator_lstm(args.an, env, lane, s_gc, s_gv, s_pt, dofq, s_hist, s_vt);
+        else actuator_network(args.an, env, lane, s_gc, s_gv, s_pt, dofq, s_hist, s_vt);
+        __syncwarp();
+      }
 #pragma unroll 1
       for (int i = lane; i < nv; i += 32) {
         const bool an = AN && ((args.an.mask >> i) & 1ull);
@@ -2000,7 +2113,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 14 ? 2 : 1)) rsb_step_kernel
 #pragma unroll 1
         for (int i = lane; i < nv; i += 32) s_gv[i] = args.gym.gv_init[i];
         if constexpr (AN) {
-          const int hw = args.an.n * 2 * (args.an.H - 1);
+          const int hw = args.an.words;
 #pragma unroll 1
           for (int i = lane; i < hw; i += 32) args.an.hist[(size_t)env * hw + i] = 0.f;
         }

@@ -154,7 +154,22 @@ class Batch : public std::enable_shared_from_this<Batch> {
     }
     check(rsb_batch_set_actuator_network(b_, dofs.data(), (int)dofs.size(), history, layers, width, params.data()), "set_actuator_network");
   }
-  // its history rows [env_count, dofs, 2, history - 1] float32 at a device address (0: zeroes the range)
+  // LSTM actuator network: dofs (gv indices), parameters in torch.nn.LSTM order then the read-out (host); an empty dof list clears it
+  void set_actuator_lstm(const std::vector<int32_t>& dofs, int layers, int hidden, const std::vector<float>& params) {
+    if (!dofs.empty()) {   // the library reads exactly this many floats
+      size_t count = 0;
+      if (layers >= 1 && hidden >= 1) {
+        count = size_t(hidden) + 1;
+        for (int l = 0; l < layers; l++) count += size_t(4 * hidden) * ((l == 0 ? 2 : hidden) + hidden + 2);
+      }
+      if (count == 0 || params.size() != count)
+        throw std::runtime_error("set_actuator_lstm: " + std::to_string(params.size()) + " parameters for " + std::to_string(layers) +
+                                 " layers of hidden size " + std::to_string(hidden) + " (need " + std::to_string(count) + ")");
+    }
+    check(rsb_batch_set_actuator_lstm(b_, dofs.data(), (int)dofs.size(), layers, hidden, params.data()), "set_actuator_lstm");
+  }
+  // the network's history rows at a device address (0: zeroes the range): [env_count, dofs, 2, history - 1] float32 for the MLP,
+  // [env_count, dofs, layers, 2, hidden] for the LSTM
   void set_actuator_history(uintptr_t rows_dev, int env_begin, int env_count) {
     check(rsb_batch_set_actuator_history(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_actuator_history");
   }
@@ -226,6 +241,7 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("set_contact_friction", &Batch::set_contact_friction, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_actuator_params", &Batch::set_actuator_params, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_actuator_network", &Batch::set_actuator_network, py::arg("dofs"), py::arg("history"), py::arg("layers"), py::arg("width"), py::arg("params"))
+      .def("set_actuator_lstm", &Batch::set_actuator_lstm, py::arg("dofs"), py::arg("layers"), py::arg("hidden"), py::arg("params"))
       .def("set_actuator_history", &Batch::set_actuator_history, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("actuator_history", &Batch::actuator_history, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_heightmaps", &Batch::set_heightmaps, py::arg("count"), py::arg("xs"), py::arg("ys"), py::arg("x_size"), py::arg("y_size"),
