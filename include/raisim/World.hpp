@@ -126,10 +126,12 @@ struct LockStep {
   // terrain upload); immediate, the reader's row of the last read
   Rows<float> tauApplied, cfForce, scan, scanXy;   // [nv], [S][3] and [S] of the contact bodies (setContactBodies), [P] and [P][2] of the scan
   Rows<float> imuLin, imuAng;               // [I][3] each: the IMUs' readings (setImus)
+  Rows<float> rayDist;                      // [R] the ray casts' distances (setRays), valid as the height scan is
+  Rows<int32_t> rayHit;                     // [R] what each ray hit
   Rows<int32_t> ncontacts, cfSteps;
   Rows<rsb_contact> contacts;               // [RSB_KMAX]
-  int cfBodies = 0, scanPoints = 0, imus = 0;
-  bool stateValid = false, tauAppliedValid = false, contactsValid = false, cfValid = false, scanValid = false, imuValid = false;
+  int cfBodies = 0, scanPoints = 0, imus = 0, rays = 0;
+  bool stateValid = false, tauAppliedValid = false, contactsValid = false, cfValid = false, scanValid = false, imuValid = false, rayValid = false;
   // terrain of every environment of a deferred mirror (World::addHeightMap / addGround), uploaded by pushTerrain().  Environments holding
   // the same heights share one MapEntry; `atlas` is what the device holds, in atlas order (atlasSingle: one map set without an index)
   struct MapEntry {
@@ -175,7 +177,7 @@ struct LockStep {
   float* stateRow(int env, Rows<float>& a) {
     sync(env);
     if (deferred) needState(env);
-    scanValid = false;
+    scanValid = rayValid = false;
     return write(env, a);
   }
   float* inertiaRow(int env) {               // every environment starts from the model's rows
@@ -250,7 +252,7 @@ struct LockStep {
     rsbCheck(rsb_batch_integrate(batch, k), "integrate");
     launches++;
     for (int& p : pending) p = 0;
-    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = imuValid = false;
+    stateValid = tauAppliedValid = contactsValid = cfValid = scanValid = imuValid = rayValid = false;
   }
   // every environment is parked (or finished) with the same number of integrate() calls pending
   void flush() {
@@ -303,6 +305,15 @@ struct LockStep {
     if (scan.w != size_t(scanPoints)) { scan.init(n, size_t(scanPoints), 0.f); scanXy.init(n, size_t(scanPoints) * 2, 0.f); scanValid = false; }
     refill(env, scanValid, [&](int lo, int k, bool all) {
       rsbCheck(rsb_batch_get_height_scan(batch, lo, k, scan.row(lo), all || samples ? scanXy.row(lo) : nullptr, RSB_HOST), "getHeightScan");
+    });
+  }
+  // the ray casts, by the height scan's rule: deferred, one call casts every environment after the rows written since the last launch
+  // went up
+  void needRayCasts(int env, bool hits) {
+    current(env);
+    if (rayDist.w != size_t(rays)) { rayDist.init(n, size_t(rays), 0.f); rayHit.init(n, size_t(rays), 0); rayValid = false; }
+    refill(env, rayValid, [&](int lo, int k, bool all) {
+      rsbCheck(rsb_batch_get_ray_casts(batch, lo, k, rayDist.row(lo), all || hits ? rayHit.row(lo) : nullptr, RSB_HOST), "getRayCasts");
     });
   }
 
@@ -394,7 +405,7 @@ struct LockStep {
       mapUploads++;
     }
     terrainDirty = false;
-    scanValid = false;
+    scanValid = rayValid = false;
   }
 };
 
@@ -526,6 +537,16 @@ class BatchedWorld {
     ls_.scanPoints = int(bodies.size()); ls_.scanValid = false;
   }
   size_t numHeightScanPoints() const { return scanBodies_.size(); }
+  // rays (ArticulatedSystem::setRays): one list for all environments
+  void setRays(const std::vector<int32_t>& bodies, const std::vector<float>& origins, const std::vector<float>& dirs, float maxDistance, bool seeRobot) {
+    if (bodies == rayBodies_ && origins == rayOrigins_ && dirs == rayDirs_ && maxDistance == rayMax_ && seeRobot == raySeeRobot_) return;   // every environment sets the same list in its constructor
+    if (origins.size() != 3 * bodies.size() || dirs.size() != 3 * bodies.size()) throw std::runtime_error("setRays: one origin and one direction per body");
+    rsbCheck(rsb_batch_set_rays(batch_, bodies.data(), origins.data(), dirs.data(), int(bodies.size()), maxDistance,
+                                seeRobot ? RSB_RAYS_TERRAIN_AND_ROBOT : RSB_RAYS_TERRAIN), "setRays");
+    rayBodies_ = bodies; rayOrigins_ = origins; rayDirs_ = dirs; rayMax_ = maxDistance; raySeeRobot_ = seeRobot;
+    ls_.rays = int(bodies.size()); ls_.rayValid = false;
+  }
+  size_t numRays() const { return rayBodies_.size(); }
   // the learned actuator network (ArticulatedSystem::setActuatorNetwork): one for the batch.  Setting it zeroes every history, so a
   // repeat of the network already set (every environment of a VectorizedEnvironment sets it in its constructor) is not passed on
   void setActuatorNetwork(const std::vector<int32_t>& dofs, int history, int layers, int width, const std::vector<float>& params) {
@@ -573,6 +594,10 @@ class BatchedWorld {
   std::vector<size_t> imuFrames_;
   std::vector<int32_t> scanBodies_;
   std::vector<float> scanXy_;
+  std::vector<int32_t> rayBodies_;
+  std::vector<float> rayOrigins_, rayDirs_;
+  float rayMax_ = 0.f;
+  bool raySeeRobot_ = false;
   std::vector<int32_t> anDofs_;
   bool anLstm_ = false;                  // anDofs_ .. anParams_ describe the LSTM (setActuatorLstm), else the MLP
   int anH_ = 0, anL_ = 0, anW_ = 0;
@@ -1084,6 +1109,20 @@ class ArticulatedSystem {
     for (size_t i = 0; i < offsets.size(); i++) { xy[2 * i] = float(offsets[i][0]); xy[2 * i + 1] = float(offsets[i][1]); }
     w_->setHeightScan(b, xy, yawAligned);
   }
+  // setRays: rays from bodies (getBodyIdx order, at most RSB_MAX_RAYS), each with an origin and a direction in the body frame (any
+  // length, normalised when set): a depth camera or a lidar on the robot.  getRayCasts reports the first hit within maxDistance against
+  // the terrain and, with seeRobot, the robot's own collision bodies (a shape that contains a ray's origin is ignored, so a camera inside
+  // the base box sees out of it).  The list belongs to the batch: every environment shares it, and each environment of a
+  // VectorizedEnvironment may set the same list in its constructor.
+  void setRays(const std::vector<size_t>& bodies, const std::vector<Vec<3>>& origins, const std::vector<Vec<3>>& directions, double maxDistance,
+               bool seeRobot = false) {
+    if (origins.size() != bodies.size() || directions.size() != bodies.size()) throw std::runtime_error("setRays: one origin and one direction per body");
+    std::vector<int32_t> b(bodies.begin(), bodies.end());
+    std::vector<float> o(3 * bodies.size()), d(3 * bodies.size());
+    for (size_t i = 0; i < bodies.size(); i++)
+      for (int k = 0; k < 3; k++) { o[3 * i + k] = float(origins[i][k]); d[3 * i + k] = float(directions[i][k]); }
+    w_->setRays(b, o, d, float(maxDistance), seeRobot);
+  }
   // setActuatorNetwork: the learned actuator network of rsb_batch_set_actuator_network (include/rsb.h) for the dofs listed (generalized
   // velocity indices of joints), with params in torch.nn.Linear order.  The network belongs to the batch: every environment shares it,
   // and each environment of a VectorizedEnvironment may set the same one in its constructor.  Setting it zeroes every history.
@@ -1120,6 +1159,21 @@ class ArticulatedSystem {
     if (samples) {
       samples->resize(P);
       for (size_t i = 0; i < P; i++) { (*samples)[i][0] = xy[2 * i]; (*samples)[i][1] = xy[2 * i + 1]; }
+    }
+  }
+  // the first hit along every ray at the current state, in setRays order: distances (+inf: nothing within maxDistance, NaN: a diverged
+  // state) and (hits, optional) what each hit: RSB_RAY_TERRAIN, the collision-body index, or RSB_RAY_MISS.  In a VectorizedEnvironment
+  // one call casts every environment's rays for the control step; a stand-alone World casts this environment's
+  void getRayCasts(VecDyn& distances, std::vector<int>* hits = nullptr) {
+    const size_t R = w_->numRays();
+    if (R == 0) throw std::runtime_error("getRayCasts: call setRays() first");
+    m_.needRayCasts(env_, hits != nullptr);
+    const float* d = m_.rayDist.row(env_);
+    distances.resize(R);
+    for (size_t i = 0; i < R; i++) distances[i] = d[i];
+    if (hits) {
+      const int32_t* h = m_.rayHit.row(env_);
+      hits->assign(h, h + R);
     }
   }
   int env() const { return env_; }

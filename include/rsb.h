@@ -474,6 +474,40 @@ int rsb_batch_set_height_scan(rsb_batch* b, const int32_t* body, const float* xy
 /* height [n][P] (world z of the surface at each sample) and xy_out [n][P][2] (the world sample location), P = the number of points
  * set; a NULL output is skipped (both NULL: nothing is launched).  RSB_ERR_INVALID when no points are set or there is no terrain. */
 int rsb_batch_get_height_scan(rsb_batch* b, int env_begin, int env_count, float* height, float* xy_out, int where);
+/* ---- ray casts (a body-mounted depth camera or lidar, for every environment at once).  One list of rays, shared by all environments;
+ *      ray i hangs on body[i] with origin origin[i][3] and direction dir[i][3] in the body frame.  With (p, R) the body's world pose the
+ *      ray is o + t d, o = p + R origin, d = R dir^ (dir^ = dir normalised in double when the list is set).
+ *      distance: the smallest t in (0, max_distance] at which the ray enters a target from outside, +inf when there is none;
+ *      hit: RSB_RAY_TERRAIN, the collision body c >= 0 (rsb_model_tables order) or RSB_RAY_MISS.  A ray whose world o or d is not
+ *      finite (a diverged environment) reads NaN with RSB_RAY_MISS.
+ *      Targets:
+ *        ground at z0: the infinite plane, hit only coming down onto it from above (d_z < 0, o_z > z0);
+ *        height map: the environment's own map (terrain atlas), two triangles per cell split along P00-P11, over the map's rectangle
+ *                    only (no walls at its edges); a hit is the first point where the ray crosses a triangle from its upper side to
+ *                    its lower side, so a ray starting under the surface hits only after it has come back up and gone down again.
+ *                    Watertight: a ray that goes from above the surface to below it within range always reports a hit, also exactly
+ *                    on a cell boundary, a vertex or a diagonal;
+ *        robot (RSB_RAYS_TERRAIN_AND_ROBOT only): every collision body with the shape it collides with (sphere, capsule, box,
+ *                    cylinder; a mesh as its bounding box), the world-welded root of a fixed-base robot included.  A ray whose origin is
+ *                    inside or on a shape ignores that shape (a camera inside the base's collision box sees out of it).
+ *      With no terrain the terrain is absent: its rays miss.  The terrain is read at call time.
+ *      Poses: with RSB_RAYS_TERRAIN a ray on the root of a floating-base robot takes its pose from gc (the quaternion normalised as the
+ *      observation row does), so a terrain-only base camera is one launch after any step; every other ray uses the kinematics pass's
+ *      poses, which the call runs first when they are stale, as the height scan does.  The call writes only its outputs and has no effect
+ *      on any later step.  Host outputs are staged through the batch's staging buffer (env_count * n * 8 bytes). */
+#define RSB_MAX_RAYS 16384
+#define RSB_RAY_MISS (-1)              /* hit id: nothing within max_distance                */
+#define RSB_RAY_TERRAIN (-2)           /* hit id: the ground or the environment's height map */
+#define RSB_RAYS_TERRAIN 0             /* rays see the terrain only                          */
+#define RSB_RAYS_TERRAIN_AND_ROBOT 1   /* ... and the robot's own collision bodies           */
+/* body[n] in rsb_model_body_index order, origin[n][3], dir[n][3]; max_distance and targets for all rays.  n = 0 clears.  Kept until the
+ * next call (set-params calls, terrain calls and gym resets keep it).  Refused with RSB_ERR_INVALID, changing nothing: n < 0 or
+ * > RSB_MAX_RAYS, body, origin or dir NULL with n > 0, a body out of range, an origin or direction entry that is not finite,
+ * |dir| < 1e-6, a max_distance that is not finite or not > 0, another targets. */
+int rsb_batch_set_rays(rsb_batch* b, const int32_t* body, const float* origin, const float* dir, int n, float max_distance, int targets);
+/* distance [n][R] float32 and hit [n][R] int32, R = the number of rays set; a NULL output is skipped (both NULL: nothing is launched).
+ * RSB_ERR_INVALID when no rays are set. */
+int rsb_batch_get_ray_casts(rsb_batch* b, int env_begin, int env_count, float* distance, int32_t* hit, int where);
 /* FK, M and h of the CURRENT state for the getters above, without touching the contact records of the last integrate()
  * (upstream's getters are lazy the same way).  The getters call it themselves when the state changed through this API;
  * call it explicitly after writing the state through rsb_batch_device_ptrs() views. */

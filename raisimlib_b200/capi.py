@@ -17,6 +17,9 @@ HOST, DEVICE = 0, 1
 FORCE_AND_TORQUE, PD_PLUS_FEEDFORWARD_TORQUE = 0, 1
 SCAN_YAW, SCAN_WORLD = 0, 1
 MAX_SCAN_POINTS = 1024
+MAX_RAYS = 16384
+RAY_MISS, RAY_TERRAIN = -1, -2           # hit ids of ray_casts() besides a collision-body index
+RAYS_TERRAIN, RAYS_TERRAIN_AND_ROBOT = 0, 1
 ACTUATION_DELAY_MAX = 16   # RSB_MAX_ACTUATION_DELAY: sub-steps
 
 
@@ -67,6 +70,21 @@ def generate_terrain(x_samples=129, y_samples=129, x_size=12.8, y_size=12.8, fre
     out = np.empty((y_samples, x_samples), np.float32)
     _ck(lib().rsb_terrain_generate(C.byref(p), out.ctypes.data_as(C.c_void_p)))
     return out
+
+
+def pinhole_rays(width, height, hfov_deg):
+    """unit directions [height * width, 3] float64 of a pinhole camera's rays through the pixel centres, row-major from the top-left
+    pixel, in the camera frame: optical axis +x, image right -y, image down -z.  The vertical field of view follows from the square
+    pixels: tan(vfov / 2) = tan(hfov / 2) * height / width.  With ray_casts() distances d [.., height * width] the z-depth image (distance
+    along the optical axis) is d * dirs[:, 0]."""
+    if width < 1 or height < 1 or not 0.0 < hfov_deg < 180.0:
+        raise ValueError(f"pinhole_rays: need width, height >= 1 and 0 < hfov_deg < 180, got {width}, {height}, {hfov_deg}")
+    f = 0.5 * width / np.tan(np.radians(hfov_deg) / 2)      # focal length in pixels
+    u = np.arange(width) + 0.5 - 0.5 * width                 # pixel centre right of the axis
+    v = np.arange(height) + 0.5 - 0.5 * height               # pixel centre below the axis
+    V, U = np.meshgrid(v, u, indexing="ij")
+    d = np.stack([np.full(U.shape, f), -U, -V], -1).reshape(-1, 3)
+    return d / np.linalg.norm(d, axis=1, keepdims=True)
 
 
 def read_heightmap_text(path):
@@ -173,6 +191,8 @@ SIGNATURES = {
     "rsb_batch_get_imu_readings": [_P, _I, _I, _P, _P, _I],
     "rsb_batch_set_height_scan": [_P, _P, _P, _I, _I],
     "rsb_batch_get_height_scan": [_P, _I, _I, _P, _P, _I],
+    "rsb_batch_set_rays": [_P, _P, _P, _P, _I, _F, _I],
+    "rsb_batch_get_ray_casts": [_P, _I, _I, _P, _P, _I],
     "rsb_batch_ob_dim": [_P],
     "rsb_batch_observe": [_P, _P, _I, _I, _I],
     "rsb_batch_control_step": [_P, _P, _P, _I, _I, _P, _I],
@@ -368,7 +388,7 @@ class Batch:
         h = C.c_void_p()
         _ck(lib().rsb_batch_create(model.h, num_envs, device, C.byref(h)))
         self.h, self.n, self.nq, self.nv, self.nb = h, num_envs, model.nq, model.nv, model.nb
-        self.device, self.nframes, self.ncontact_bodies, self.nscan, self.nimus = device, 0, 0, 0, 0
+        self.device, self.nframes, self.ncontact_bodies, self.nscan, self.nimus, self.nrays = device, 0, 0, 0, 0, 0
         self.hm_shape = None                 # (ys, xs) of the height map(s) set through this object
         self.an_shape = None                 # (listed dofs, history) of the actuator network set through this object
         self.lstm_shape = None               # (listed dofs, layers, hidden) of the LSTM actuator network set through this object
@@ -727,6 +747,42 @@ class Batch:
         """height_scan() written into torch CUDA tensors [n, P] / [n, P, 2] (None skips one), in the batch's stream order"""
         n, P = self._count(env_begin, env_count), self.nscan
         _ck(lib().rsb_batch_get_height_scan(self.h, env_begin, n, self._device_out(height, (n, P), "height"), self._device_out(xy, (n, P, 2), "xy"), DEVICE))
+
+    # ray casts (depth cameras, lidars)
+    def set_rays(self, body, origin, dir, max_distance, targets="terrain"):
+        """rays shared by all environments: ray i hangs on body[i] with origin[i] [3] and direction dir[i] [3] (any length >= 1e-6,
+        normalised here) in the body frame; ray_casts() reports the first hit within max_distance.  targets "terrain" sees the ground
+        or height map only, "all" also the robot's own collision bodies (a shape that contains the ray's origin is ignored).  An empty
+        list clears them; a refused call keeps the rays set before.  pinhole_rays() gives a camera's directions."""
+        modes = {"terrain": RAYS_TERRAIN, "all": RAYS_TERRAIN_AND_ROBOT}
+        if targets not in modes:
+            raise ValueError(f"set_rays: targets must be 'terrain' or 'all', got {targets!r}")
+        bd = np.ascontiguousarray(body, np.int32).reshape(-1)
+        o = np.ascontiguousarray(origin, np.float32).reshape(-1, 3)
+        d = np.ascontiguousarray(dir, np.float32).reshape(-1, 3)
+        if len(o) != len(bd) or len(d) != len(bd):
+            raise ValueError(f"set_rays: {len(bd)} bodies, {len(o)} origins, {len(d)} directions")
+        _ck(lib().rsb_batch_set_rays(self.h, bd.ctypes.data_as(C.c_void_p), o.ctypes.data_as(C.c_void_p), d.ctypes.data_as(C.c_void_p),
+                                     len(bd), max_distance, modes[targets]))
+        self.nrays = len(bd)
+
+    def set_rays_by_name(self, names, origin, dir, max_distance, targets="terrain"):
+        """set_rays() with the bodies given by link name (rsb_model_body_index: a merged link names its body)"""
+        self.set_rays([self.model.body_index(n) for n in names], origin, dir, max_distance, targets)
+
+    def ray_casts(self, env_begin=0, env_count=None):
+        """(distance [n, R] float32: the first hit along each ray at the current state, +inf for none, NaN for a diverged
+        environment; hit [n, R] int32: RAY_TERRAIN, the collision-body index, or RAY_MISS)"""
+        n = self._count(env_begin, env_count)
+        dist, hit = np.empty((n, self.nrays), np.float32), np.empty((n, self.nrays), np.int32)
+        _ck(lib().rsb_batch_get_ray_casts(self.h, env_begin, n, dist.ctypes.data_as(C.c_void_p), hit.ctypes.data_as(C.c_void_p), HOST))
+        return dist, hit
+
+    def ray_casts_into(self, distance=None, hit=None, env_begin=0, env_count=None):
+        """ray_casts() written into torch CUDA tensors [n, R] (float32 / int32; None skips one), in the batch's stream order"""
+        n, R = self._count(env_begin, env_count), self.nrays
+        _ck(lib().rsb_batch_get_ray_casts(self.h, env_begin, n, self._device_out(distance, (n, R), "distance"),
+                                          self._device_out(hit, (n, R), "hit", "int32"), DEVICE))
 
     def diverged(self, env_begin=0, env_count=None):
         return self._read(lib().rsb_batch_get_diverged, (), np.int32, env_begin, env_count)

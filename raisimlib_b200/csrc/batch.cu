@@ -15,6 +15,7 @@
 #include "model.hpp"
 #include "step_kernel.cuh"
 #include "aux_kernels.cuh"
+#include "ray_cast.cuh"
 
 using namespace rsb;
 
@@ -142,6 +143,11 @@ struct rsb_batch {
   ScanTable scan{};
   DevBuf<int> scan_tab;
   bool scan_off_root = false;
+  // rays of rsb_batch_set_rays (rays.n = 0: none) and the model's collision bodies, in one device allocation sized for RSB_MAX_RAYS;
+  // ray_kin: a ray's pose comes from the kinematics pass
+  RayTable rays{};
+  DevBuf<float> ray_tab;
+  bool ray_kin = false;
   // per-environment rows: inertial ones of rsb_batch_set_body_inertia [N][nb][BI_WORDS], terrain friction of
   // rsb_batch_set_contact_friction [N][ncoll], kp | kd | effort limit of rsb_batch_set_actuator_params [N][3][nv]; row_bad: the verdict
   // of the check a call's rows pass before they replace any of them
@@ -1536,6 +1542,79 @@ int rsb_batch_get_height_scan(rsb_batch* b, int env_begin, int env_count, float*
   if (where != RSB_HOST) return RSB_OK;
   if (height) { rc = copy_out(b, height, dh, rows * 4, RSB_HOST); if (rc) return rc; }
   return xy_out ? copy_out(b, xy_out, dxy, rows * 2 * 4, RSB_HOST) : RSB_OK;
+}
+// ---- ray casts: a body-mounted depth camera or lidar, one launch of rsb_ray_cast_kernel ----------------------------------------------
+int rsb_batch_set_rays(rsb_batch* b, const int32_t* body, const float* origin, const float* dir, int n, float max_distance, int targets) {
+  if (!b) return fail(RSB_ERR_INVALID, "null batch");
+  if (n < 0 || n > RSB_MAX_RAYS) return fail(RSB_ERR_INVALID, "at most " + std::to_string(RSB_MAX_RAYS) + " rays per batch (got " + std::to_string(n) + ")");
+  if (n > 0 && (!body || !origin || !dir)) return fail(RSB_ERR_INVALID, "null ray body, origin or direction list");
+  if (!std::isfinite(max_distance) || !(max_distance > 0.f)) return fail(RSB_ERR_INVALID, "ray max_distance must be finite and > 0");
+  if (targets != RSB_RAYS_TERRAIN && targets != RSB_RAYS_TERRAIN_AND_ROBOT) return fail(RSB_ERR_INVALID, "ray targets must be RSB_RAYS_TERRAIN or RSB_RAYS_TERRAIN_AND_ROBOT");
+  const Model& md = b->model->md;
+  const int M = RSB_MAX_RAYS, ncoll = md.ncoll();
+  if (ncoll > RAY_MAX_SHAPES) return fail(RSB_ERR_UNSUPPORTED, "ray casts: more than " + std::to_string(RAY_MAX_SHAPES) + " collision bodies");
+  std::vector<float> W((size_t)7 * M + (size_t)RAY_SHAPE_WORDS * ncoll, 0.f);   // body[M] | origin[M][3] | dir[M][3] | shapes
+  int32_t* Wb = reinterpret_cast<int32_t*>(W.data());
+  for (int i = 0; i < n; i++) {
+    const std::string at = "ray " + std::to_string(i) + ": ";
+    if (body[i] < 0 || body[i] >= b->nb) return fail(RSB_ERR_INVALID, at + "body index out of range (the model has " + std::to_string(b->nb) + ")");
+    double d2 = 0;
+    for (int k = 0; k < 3; k++) {
+      if (!std::isfinite(origin[3 * i + k]) || !std::isfinite(dir[3 * i + k])) return fail(RSB_ERR_INVALID, at + "origin or direction is not finite");
+      d2 += (double)dir[3 * i + k] * dir[3 * i + k];
+    }
+    const double nrm = std::sqrt(d2);
+    if (!(nrm >= 1e-6)) return fail(RSB_ERR_INVALID, at + "direction is shorter than 1e-6");
+    Wb[i] = body[i];
+    for (int k = 0; k < 3; k++) { W[M + 3 * i + k] = origin[3 * i + k]; W[4 * M + 3 * i + k] = (float)(dir[3 * i + k] / nrm); }
+  }
+  if (n == 0) { b->rays.n = 0; return RSB_OK; }
+  float* S = W.data() + (size_t)7 * M;
+  for (int c = 0; c < ncoll; c++, S += RAY_SHAPE_WORDS) {
+    const double* sz = &md.csize[3 * c];
+    int32_t ib[2] = {md.cbody[c], md.ctype[c]};
+    std::memcpy(S, ib, 8);
+    for (int k = 0; k < 3; k++) { S[2 + k] = (float)sz[k]; S[5 + k] = (float)md.cpos[3 * c + k]; }
+    for (int k = 0; k < 9; k++) S[8 + k] = (float)md.crot[9 * c + k];
+    double bound = sz[0];   // sphere
+    if (md.ctype[c] == CT_BOX) bound = std::sqrt(sz[0] * sz[0] + sz[1] * sz[1] + sz[2] * sz[2]);
+    else if (md.ctype[c] != CT_SPHERE) bound = sz[0] + sz[1];
+    S[17] = (float)(bound * 1.0001 + 1e-6);   // widened so that float32 rounding never culls a ray that touches the shape
+  }
+  const bool from_gc = md.floating && targets == RSB_RAYS_TERRAIN;
+  bool kin = targets == RSB_RAYS_TERRAIN_AND_ROBOT;
+  for (int i = 0; i < n; i++) kin = kin || !(body[i] == 0 && from_gc);
+  CK(cudaSetDevice(b->device));
+  CK(b->ray_tab.ensure((size_t)(7 * M + RAY_SHAPE_WORDS * RAY_MAX_SHAPES) * 4, b->stream));   // sized for the largest list: the layout never moves
+  CK(cudaMemcpyAsync(b->ray_tab.get(), W.data(), W.size() * 4, cudaMemcpyHostToDevice, b->stream));
+  CK(cudaStreamSynchronize(b->stream));   // the pageable source goes out of scope here
+  const float* T = b->ray_tab.get();
+  b->rays = RayTable{n, targets, from_gc ? 1 : 0, ncoll, max_distance, reinterpret_cast<const int*>(T), T + M, T + 4 * M, T + 7 * M};
+  b->ray_kin = kin;
+  return RSB_OK;
+}
+int rsb_batch_get_ray_casts(rsb_batch* b, int env_begin, int env_count, float* distance, int32_t* hit, int where) {
+  int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;
+  if (b->rays.n == 0) return fail(RSB_ERR_INVALID, "no rays: call rsb_batch_set_rays() first");
+  if (env_count == 0 || !(distance || hit)) return RSB_OK;
+  CK(cudaSetDevice(b->device));
+  // poses from the kinematics pass; after integrate2() its buffers hold the state before the step
+  if (b->ray_kin) { rc = b->kin_prestep ? rsb_batch_update_kinematics(b) : ensure_kinematics(b); if (rc) return rc; }
+  const size_t rows = (size_t)env_count * b->rays.n;
+  float* dd = distance;
+  int* dh = hit;
+  if (where == RSB_HOST) {
+    float* s = staging(b, (distance ? rows : 0) + (hit ? rows : 0)); if (!s) return RSB_ERR_CUDA;
+    if (distance) { dd = s; s += rows; }
+    if (hit) dh = reinterpret_cast<int*>(s);
+  }
+  const dim3 grid((unsigned)env_count, (unsigned)((b->rays.n + 255) / 256));
+  rsb_ray_cast_kernel<<<grid, 256, 0, b->stream>>>(b->rays, b->ter, b->gc.get(), b->gc_stride, b->dbg_R.get(), b->dbg_p.get(), b->nb, env_begin, dd, dh);
+  CK(cudaGetLastError());
+  b->launches++;
+  if (where != RSB_HOST) return RSB_OK;
+  if (distance) { rc = copy_out(b, distance, dd, rows * 4, RSB_HOST); if (rc) return rc; }
+  return hit ? copy_out(b, hit, dh, rows * 4, RSB_HOST) : RSB_OK;
 }
 int rsb_batch_get_contacts(rsb_batch* b, rsb_contact* out, int32_t* counts, int env_begin, int env_count, int where) {
   int rc = check_range(b, env_begin, env_count, where); if (rc) return rc;

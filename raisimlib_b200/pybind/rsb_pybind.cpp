@@ -131,6 +131,16 @@ class Batch : public std::enable_shared_from_this<Batch> {
   void height_scan(uintptr_t height_dev, uintptr_t xy_dev) {
     check(rsb_batch_get_height_scan(b_, 0, view_.num_envs, reinterpret_cast<float*>(height_dev), reinterpret_cast<float*>(xy_dev), RSB_DEVICE), "height_scan");
   }
+  // rays shared by all environments: body [R], origin [R*3], dir [R*3] in the body frame, targets "terrain" or "all" (empty clears)
+  void set_rays(const std::vector<int32_t>& body, const std::vector<float>& origin, const std::vector<float>& dir, float max_distance, const std::string& targets) {
+    if (origin.size() != 3 * body.size() || dir.size() != 3 * body.size()) throw std::runtime_error("set_rays: need 3 origin and 3 direction entries per ray");
+    if (targets != "terrain" && targets != "all") throw std::runtime_error("set_rays: targets must be 'terrain' or 'all'");
+    check(rsb_batch_set_rays(b_, body.data(), origin.data(), dir.data(), (int)body.size(), max_distance, targets == "all" ? RSB_RAYS_TERRAIN_AND_ROBOT : RSB_RAYS_TERRAIN), "set_rays");
+  }
+  // the ray casts of every environment into tensor addresses ([num_envs, R] float32 and int32, contiguous); 0 skips an output
+  void ray_casts(uintptr_t distance_dev, uintptr_t hit_dev) {
+    check(rsb_batch_get_ray_casts(b_, 0, view_.num_envs, reinterpret_cast<float*>(distance_dev), reinterpret_cast<int32_t*>(hit_dev), RSB_DEVICE), "ray_casts");
+  }
   // per-environment inertial rows [env_count, nb, 10] float32 (mass, com, inertia xx xy xz yy yz zz) from a device address
   void set_body_inertia(uintptr_t rows_dev, int env_begin, int env_count) {
     check(rsb_batch_set_body_inertia(b_, reinterpret_cast<const float*>(rows_dev), env_begin, env_count, RSB_DEVICE), "set_body_inertia");
@@ -237,6 +247,8 @@ PYBIND11_MODULE(_rsb_py, m) {
       .def("imu_readings", &Batch::imu_readings, py::arg("lin_acc_dev"), py::arg("ang_vel_dev"))
       .def("set_height_scan", &Batch::set_height_scan, py::arg("body"), py::arg("xy"), py::arg("align") = std::string("yaw"))
       .def("height_scan", &Batch::height_scan, py::arg("height_dev"), py::arg("xy_dev"))
+      .def("set_rays", &Batch::set_rays, py::arg("body"), py::arg("origin"), py::arg("dir"), py::arg("max_distance"), py::arg("targets") = std::string("terrain"))
+      .def("ray_casts", &Batch::ray_casts, py::arg("distance_dev"), py::arg("hit_dev"))
       .def("set_body_inertia", &Batch::set_body_inertia, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_contact_friction", &Batch::set_contact_friction, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
       .def("set_actuator_params", &Batch::set_actuator_params, py::arg("rows_dev"), py::arg("env_begin"), py::arg("env_count"))
